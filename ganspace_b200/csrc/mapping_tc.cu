@@ -75,7 +75,8 @@ mapping_layer_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __gri
     const int num_n_tiles = (p.N_total + TC_BLOCK_N - 1) / TC_BLOCK_N;
     const int num_k_blocks = (p.K + TC_BLOCK_K - 1) / TC_BLOCK_K;
     // work unit = (row tile, group of consecutive N tiles); n_groups = 1: a CTA walks through all N tiles of its row tile
-    // (its A rows are re-read out of L2), n_groups = num_n_tiles: one output tile per unit (few row tiles: more parallelism)
+    // (its A rows are re-read out of L2), n_groups = num_n_tiles: one output tile per unit (few row tiles: more parallelism;
+    // many: a shorter last round, tc_launch_layer)
     const int n_groups = p.n_groups, tiles_per_group = num_n_tiles / n_groups;
     const int num_units = num_m_tiles * n_groups;
 
@@ -384,7 +385,11 @@ static int tc_launch_layer(const CUtensorMap &tm_ah, const CUtensorMap &tm_al, c
     int avail = num_sms() - leave_free_sms;
     if (avail < 16) avail = 16;
     if (avail > num_sms()) avail = num_sms();
-    p.n_groups = (m_tiles >= 2 * avail) ? 1 : n_tiles;
+    // work units: whole row tiles (n_groups = 1, the A rows of the second N tile come out of L2 while still hot) unless single
+    // tiles make the last round shorter -- a 70k-row chunk on 100 CTAs: 547 row tiles take 6 rounds, 1094 tiles 5.5
+    const int64_t rounds_rows = (int64_t)(m_tiles + avail - 1) / avail * n_tiles;          // in tile times
+    const int64_t rounds_tiles = ((int64_t)m_tiles * n_tiles + avail - 1) / avail;
+    p.n_groups = (m_tiles < 2 * avail || rounds_tiles < rounds_rows) ? n_tiles : 1;
     {
         static int dbg = -1;
         if (dbg < 0) { const char *e = getenv("GANSPACE_B200_MAPPING_DBG"); dbg = e ? atoi(e) : 0; }
