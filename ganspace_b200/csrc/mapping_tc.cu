@@ -13,34 +13,39 @@
 // the bf16 MMA rate gives this accuracy in 3 MMAs; TF32 would need 3 MMAs at half the rate.
 //
 // Kernel (one launch per layer; activations travel between layers as fp16 hi/lo pairs = the same 4 B/element
-// as fp32): persistent, one CTA per SM, warp-specialised, 128 x 256 output tiles:
-//     warps 8-11  producer warpgroup: one thread issues the TMA loads (A_hi, A_lo: 128 x 64 boxes; W_hi, W_lo: 256 x 64
-//                 boxes; SWIZZLE_128B, K-major); the warpgroup hands most of its registers to the consumers (setmaxnreg)
-//     warps 0-7   two consumer warpgroups, 64 rows of the tile each: wgmma m64n128k16 on both 128-column halves of
-//                 the tile, 6 per K step of 16 (the accumulator, 128 fp32 per thread, lives in registers), then the
-//                 epilogue (2^-s, +bias, leaky-ReLU, *sqrt2 -> split to fp16 hi/lo for the next layer, or fp32 for
-//                 the last layer) through a swizzled shared-memory staging box and a TMA store
-// smem: 2 stages x 96 KB (A_hi 16K, A_lo 16K, W_hi 32K, W_lo 32K) with mbarrier full/empty pairs, + 2 x 16 KB staging.
+// as fp32): persistent, one CTA per SM, warp-specialised, ping-pong: each consumer warpgroup owns whole 128 x 128 output
+// tiles, and the two take turns on the tensor cores, so that one's epilogue runs under the other's MMAs:
+//     warps 8-11  producer warpgroup: one thread issues the TMA loads of the CTA's tiles in order (A_hi, A_lo, W_hi, W_lo:
+//                 128 x 64 boxes; SWIZZLE_128B, K-major); the warpgroup hands most of its registers to the consumers
+//                 (setmaxnreg)
+//     warps 0-7   two consumer warpgroups; tile i of the CTA belongs to warpgroup i & 1.  Main loop: wgmma m64n128k16 on
+//                 rows 0-63 and 64-127 of the tile, 6 per K step of 16 each (the accumulator, 128 fp32 per thread, lives in
+//                 registers), one wgmma group kept in flight.  A warpgroup starts its main loop when the other has issued
+//                 all of its own (an mbarrier hand-over per tile), then runs the epilogue (2^-s, +bias, leaky-ReLU, *sqrt2
+//                 -> split to fp16 hi/lo for the next layer, or fp32 for the last layer) through a swizzled shared-memory
+//                 staging box and TMA stores while the other warpgroup's MMAs run
+// smem: 3 stages x 64 KB (A_hi, A_lo, W_hi, W_lo: 16 KB each) with mbarrier full/empty pairs, + 2 x 16 KB staging.
 #include "tc_common.cuh"
 #include <stdlib.h>
 
 namespace gsb {
 
 constexpr int TC_BLOCK_M = 128;
-constexpr int TC_BLOCK_N = 256;
+constexpr int TC_BLOCK_N = 128;
 constexpr int TC_BLOCK_K = 64;           // 64 fp16 = one 128-byte swizzle row
-constexpr int TC_STAGES = 2;
-constexpr int TC_WG_ROWS = 64;           // rows of the tile per consumer warpgroup
+constexpr int TC_STAGES = 3;
+constexpr int TC_FRAG_ROWS = 64;         // rows of one m64n128 accumulator fragment (two per tile)
 constexpr uint32_t TC_A_BYTES = TC_BLOCK_M * TC_BLOCK_K * 2;   // 16 KB
-constexpr uint32_t TC_W_BYTES = TC_BLOCK_N * TC_BLOCK_K * 2;   // 32 KB
-constexpr uint32_t TC_STAGE_BYTES = 2 * TC_A_BYTES + 2 * TC_W_BYTES;   // 96 KB
-constexpr uint32_t TC_BOX_BYTES = TC_WG_ROWS * 128;             // one 64-row x 128-byte output box: 8 KB
+constexpr uint32_t TC_W_BYTES = TC_BLOCK_N * TC_BLOCK_K * 2;   // 16 KB
+constexpr uint32_t TC_STAGE_BYTES = 2 * TC_A_BYTES + 2 * TC_W_BYTES;   // 64 KB
+constexpr uint32_t TC_BOX_BYTES = TC_FRAG_ROWS * 128;           // one 64-row x 128-byte output box: 8 KB
 constexpr uint32_t TC_STAGING_BYTES = 2 * 2 * TC_BOX_BYTES;     // per warpgroup: (hi, lo) of 64 columns, or 2 x 32 fp32 columns
 // a whole producer warpgroup, so that setmaxnreg can move registers to the consumers: 40 + 2 x 232 per thread of each
 // sub-partition's three warps fits its 16K registers (with 9 warps and no redistribution the cap is 168 and the 128-float
 // accumulator spills)
 constexpr int TC_THREADS = tc::CONSUMER_THREADS + 128;
 constexpr uint32_t TC_SMEM_BYTES = TC_STAGES * TC_STAGE_BYTES + TC_STAGING_BYTES + 64 /*barriers*/ + 1024 /*align slack*/;
+static_assert(TC_SMEM_BYTES <= 232448, "mapping_layer_tc_kernel: shared memory exceeds the H100's 227 KB per block");
 
 struct TcParams {
     const float *bias;      // [N_total] pre-multiplied by lr_mul
@@ -51,7 +56,6 @@ struct TcParams {
     const float *inv_wscale;   // device pointer to 2^-s of this layer
     int M, N_total, K;
     int mode;               // 0: (acc 2^-s + bias) -> leaky-ReLU * sqrt2 (EqualLinear);  1: plain acc 2^-s (tc_gemm_plain);  2: acc 2^-s + bias
-    int n_groups;           // work units per row tile (1 or N_total / 256)
     int dbg;                // profiling experiments (GANSPACE_B200_MAPPING_DBG): 1 no stores, 2 no W loads, 4 no A loads, 8 no MMAs
 };
 
@@ -66,7 +70,8 @@ mapping_layer_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __gri
     uint8_t *staging = smem + TC_STAGES * TC_STAGE_BYTES;
     uint64_t *bars = reinterpret_cast<uint64_t *>(staging + TC_STAGING_BYTES);
     uint64_t *full_bar = bars;                         // [TC_STAGES]
-    uint64_t *empty_bar = bars + TC_STAGES;            // [TC_STAGES]: one arrival per consumer warp
+    uint64_t *empty_bar = bars + TC_STAGES;            // [TC_STAGES]: one arrival per warp of the consuming warpgroup
+    uint64_t *turn_bar = bars + 2 * TC_STAGES;         // [2]: warpgroup wg may start its next main loop (arrivals: the other's warps)
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int num_m_tiles = (p.M + TC_BLOCK_M - 1) / TC_BLOCK_M;
@@ -74,14 +79,13 @@ mapping_layer_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __gri
     // clips stores (the 128/64/32-channel StyledConv blocks: N = 9 cout = 1152 / 576 / 288, K = cin down to 32)
     const int num_n_tiles = (p.N_total + TC_BLOCK_N - 1) / TC_BLOCK_N;
     const int num_k_blocks = (p.K + TC_BLOCK_K - 1) / TC_BLOCK_K;
-    // work unit = (row tile, group of consecutive N tiles); n_groups = 1: a CTA walks through all N tiles of its row tile
-    // (its A rows are re-read out of L2), n_groups = num_n_tiles: one output tile per unit (few row tiles: more parallelism;
-    // many: a shorter last round, tc_launch_layer)
-    const int n_groups = p.n_groups, tiles_per_group = num_n_tiles / n_groups;
-    const int num_units = num_m_tiles * n_groups;
+    // work unit = one 128 x 128 output tile, N fastest: neighbouring CTAs read the same A rows while they are in L2.  CTA b
+    // takes units b, b + grid, b + 2 grid, ...; its i-th unit belongs to consumer warpgroup i & 1.
+    const int num_units = num_m_tiles * num_n_tiles;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < TC_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CONSUMER_THREADS / 32); }
+        for (int s = 0; s < TC_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 4); }
+        mbar_init(&turn_bar[0], 4); mbar_init(&turn_bar[1], 4);
         mbar_fence_init();
     }
     if (warp == PRODUCER_WARP && lane == 0) {
@@ -97,23 +101,20 @@ mapping_layer_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __gri
         if (warp == PRODUCER_WARP && lane == 0) {
             int stage = 0; uint32_t phase = 0;
             for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
-                const int m0 = (u / n_groups) * TC_BLOCK_M, ng = u % n_groups;
-                for (int nt = ng * tiles_per_group; nt < (ng + 1) * tiles_per_group; ++nt) {
-                    const int n0 = nt * TC_BLOCK_N;
-                    for (int kb = 0; kb < num_k_blocks; ++kb) {
-                        mbar_wait(&empty_bar[stage], phase ^ 1);          // every consumer warp has left this stage
-                        uint8_t *st = smem + stage * TC_STAGE_BYTES;
-                        mbar_arrive_expect_tx(&full_bar[stage], ((p.dbg & 4) ? 0u : 2 * TC_A_BYTES) + ((p.dbg & 2) ? 0u : 2 * TC_W_BYTES));
-                        if (!(p.dbg & 4)) {
-                            tma_load_2d(&tm_a_hi, &full_bar[stage], st, kb * TC_BLOCK_K, m0);
-                            tma_load_2d(&tm_a_lo, &full_bar[stage], st + TC_A_BYTES, kb * TC_BLOCK_K, m0);
-                        }
-                        if (!(p.dbg & 2)) {
-                            tma_load_2d(&tm_w_hi, &full_bar[stage], st + 2 * TC_A_BYTES, kb * TC_BLOCK_K, n0);
-                            tma_load_2d(&tm_w_lo, &full_bar[stage], st + 2 * TC_A_BYTES + TC_W_BYTES, kb * TC_BLOCK_K, n0);
-                        }
-                        if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
+                const int m0 = (u / num_n_tiles) * TC_BLOCK_M, n0 = (u % num_n_tiles) * TC_BLOCK_N;
+                for (int kb = 0; kb < num_k_blocks; ++kb) {
+                    mbar_wait(&empty_bar[stage], phase ^ 1);              // the warpgroup that consumed this stage has left it
+                    uint8_t *st = smem + stage * TC_STAGE_BYTES;
+                    mbar_arrive_expect_tx(&full_bar[stage], ((p.dbg & 4) ? 0u : 2 * TC_A_BYTES) + ((p.dbg & 2) ? 0u : 2 * TC_W_BYTES));
+                    if (!(p.dbg & 4)) {
+                        tma_load_2d(&tm_a_hi, &full_bar[stage], st, kb * TC_BLOCK_K, m0);
+                        tma_load_2d(&tm_a_lo, &full_bar[stage], st + TC_A_BYTES, kb * TC_BLOCK_K, m0);
                     }
+                    if (!(p.dbg & 2)) {
+                        tma_load_2d(&tm_w_hi, &full_bar[stage], st + 2 * TC_A_BYTES, kb * TC_BLOCK_K, n0);
+                        tma_load_2d(&tm_w_lo, &full_bar[stage], st + 2 * TC_A_BYTES + TC_W_BYTES, kb * TC_BLOCK_K, n0);
+                    }
+                    if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
                 }
             }
         }
@@ -125,7 +126,7 @@ mapping_layer_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __gri
         // 128-byte lines, rows past M clipped by the tensor map.
         asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
         const int wg = warp >> 2;
-        const int rr0 = (warp & 3) * 16 + (lane >> 2);             // fragment rows rr0, rr0 + 8 of this warpgroup's 64
+        const int rr0 = (warp & 3) * 16 + (lane >> 2);             // fragment rows rr0, rr0 + 8 of each 64-row fragment
         const int q2 = 2 * (lane & 3);                              // fragment column pair within each 8-column group
         const bool has_bias = (p.mode != 1);
         const float slope = (p.mode == 0) ? 0.2f : 1.0f, gain = (p.mode == 0) ? 1.41421356237309515f : 1.0f;
@@ -133,15 +134,13 @@ mapping_layer_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __gri
         uint8_t *stg = staging + wg * (2 * TC_BOX_BYTES);
         const bool storer = ((threadIdx.x & 127) == 0);
         const bool to_f32 = (p.out_f32 != nullptr);
-        const uint32_t a_off = (uint32_t)wg * (TC_A_BYTES / 2);
-        int stage = 0; uint32_t phase = 0;
         bool ovf = false;
-        float acc0[64], acc1[64];                                    // columns [0, 128) and [128, 256) of the tile
+        float acc0[64], acc1[64];                                    // rows [0, 64) and [64, 128) of the tile
 #pragma unroll
         for (int j = 0; j < 64; ++j) { acc0[j] = 0.f; acc1[j] = 0.f; }
 
-        // columns [c0, c0 + 64) of the tile (fragment indices ib .. ib + 31 of `acc`) -> staging -> TMA store
-        auto store_chunk = [&](const float (&acc)[64], const int ib, const int m0, const int n0, const int c0) {
+        // rows [mrow, mrow + 64) x columns [c0, c0 + 64) of the tile (fragment indices ib .. ib + 31 of `acc`) -> staging -> TMA store
+        auto store_chunk = [&](const float (&acc)[64], const int ib, const int mrow, const int n0, const int c0) {
             if (storer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // staging has been read out
             asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
 #pragma unroll
@@ -179,7 +178,6 @@ mapping_layer_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __gri
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");          // generic-proxy writes -> visible to the TMA unit
             asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
             if (storer && !(p.dbg & 1) && n0 + c0 < p.N_total) {
-                const int mrow = m0 + wg * TC_WG_ROWS;
                 if (to_f32) {
                     tma_store_2d(&tm_o0, stg, n0 + c0, mrow);
                     if (n0 + c0 + 32 < p.N_total) tma_store_2d(&tm_o0, stg + TC_BOX_BYTES, n0 + c0 + 32, mrow);
@@ -191,29 +189,42 @@ mapping_layer_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __gri
             }
         };
 
-        for (int u = blockIdx.x; u < num_units; u += gridDim.x)
-        for (int nt = (u % n_groups) * tiles_per_group; nt < (u % n_groups + 1) * tiles_per_group; ++nt) {
-            const int m0 = (u / n_groups) * TC_BLOCK_M, n0 = nt * TC_BLOCK_N;
+        // the CTA's i-th unit (i = 2 j + wg) is this warpgroup's j-th tile; the producer fills the ring with the CTA's k-blocks
+        // in order, so k-block kb of unit i is the CTA's k-block i num_k_blocks + kb, which fixes its stage and phase
+        for (int i = wg;; i += 2) {
+            const int u = blockIdx.x + i * gridDim.x;
+            if (u >= num_units) break;
+            const int m0 = (u / num_n_tiles) * TC_BLOCK_M, n0 = (u % num_n_tiles) * TC_BLOCK_N;
+            const int g0 = i * num_k_blocks;
+            int stage = g0 % TC_STAGES, prev = stage;
+            uint32_t phase = (uint32_t)(g0 / TC_STAGES) & 1;
+            // ping-pong: the main loop starts once the other warpgroup has issued all MMAs of unit i - 1 (its (i - 1) / 2-th
+            // hand-over), so the two main loops alternate on the tensor cores instead of interleaving
+            if (i > 0) mbar_wait(&turn_bar[wg], (uint32_t)((i - 1) >> 1) & 1);
             for (int kb = 0; kb < num_k_blocks; ++kb) {
                 mbar_wait(&full_bar[stage], phase);                // TMA bytes have landed
                 if (!(p.dbg & 8)) {
                     const uint32_t st = smem_u32(smem + stage * TC_STAGE_BYTES);
-                    const uint64_t d_ah = sw128_kmajor_desc(st + a_off), d_al = sw128_kmajor_desc(st + TC_A_BYTES + a_off);
                     const uint32_t sw = st + 2 * TC_A_BYTES;
+                    const uint64_t d_wh = sw128_kmajor_desc(sw), d_wl = sw128_kmajor_desc(sw + TC_W_BYTES);
                     wgmma_fence();
-                    split_kblock_m64n128(acc0, d_ah, d_al, sw128_kmajor_desc(sw), sw128_kmajor_desc(sw + TC_W_BYTES), kb > 0);
-                    split_kblock_m64n128(acc1, d_ah, d_al, sw128_kmajor_desc(sw + TC_W_BYTES / 2),
-                                         sw128_kmajor_desc(sw + TC_W_BYTES + TC_W_BYTES / 2), kb > 0);
+                    split_kblock_m64n128(acc0, sw128_kmajor_desc(st), sw128_kmajor_desc(st + TC_A_BYTES), d_wh, d_wl, kb > 0);
+                    split_kblock_m64n128(acc1, sw128_kmajor_desc(st + TC_A_BYTES / 2),
+                                         sw128_kmajor_desc(st + TC_A_BYTES + TC_A_BYTES / 2), d_wh, d_wl, kb > 0);
                     wgmma_commit();
-                    wgmma_wait_all();
                 }
-                if (lane == 0) mbar_arrive(&empty_bar[stage]);     // frees the smem slot
+                wgmma_wait_1();                                     // k-block kb - 1's MMAs have completed ...
+                if (kb > 0 && lane == 0) mbar_arrive(&empty_bar[prev]);   // ... so its smem slot is free
+                if (kb == num_k_blocks - 1 && lane == 0) mbar_arrive(&turn_bar[wg ^ 1]);   // hand the tensor cores over
+                prev = stage;
                 if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
             }
+            wgmma_wait_all();
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
             store_chunk(acc0, 0, m0, n0, 0);
             store_chunk(acc0, 32, m0, n0, 64);
-            store_chunk(acc1, 0, m0, n0, 128);
-            store_chunk(acc1, 32, m0, n0, 192);
+            store_chunk(acc1, 0, m0 + TC_FRAG_ROWS, n0, 0);
+            store_chunk(acc1, 32, m0 + TC_FRAG_ROWS, n0, 64);
         }
         if (ovf) atomicOr(p.overflow, 1u);
         if (storer) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");     // all output boxes are in global memory
@@ -309,7 +320,7 @@ static int make_tmap_f32_out(CUtensorMap *map, const void *base, uint64_t rows, 
     if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return GSB_ERR_CUDA; }
     cuuint64_t gdim[2] = {cols, rows};
     cuuint64_t gstride[1] = {cols * 4};
-    cuuint32_t box[2] = {32, (cuuint32_t)TC_WG_ROWS};
+    cuuint32_t box[2] = {32, (cuuint32_t)TC_FRAG_ROWS};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void *>(base), gdim, gstride, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -368,42 +379,40 @@ static int tc_ensure_attr() {
     return GSB_OK;
 }
 
-// one launch of the layer kernel over all row tiles; W tensor maps must have been built with box rows 256
+// one launch of the layer kernel over all output tiles; A and W tensor maps must have been built with box rows 128
 static int tc_launch_layer(const CUtensorMap &tm_ah, const CUtensorMap &tm_al, const CUtensorMap &tm_wh, const CUtensorMap &tm_wl,
                            TcParams p, int leave_free_sms, cudaStream_t st) {
-    // output boxes of the epilogue's TMA stores (64 rows: one consumer warpgroup's half of the tile): fp16 hi / lo [M, N]
+    // output boxes of the epilogue's TMA stores (64 rows: one accumulator fragment, half of the tile): fp16 hi / lo [M, N]
     // (the next layer's A operand) or fp32 [M, N]
     CUtensorMap tm_o0, tm_o1;
     if (p.out_f32) {
         if (int r = make_tmap_f32_out(&tm_o0, p.out_f32, (uint64_t)p.M, (uint64_t)p.N_total)) return r;
         tm_o1 = tm_o0;
     } else {
-        if (int r = make_tmap_f16(&tm_o0, p.out_hi, (uint64_t)p.M, (uint64_t)p.N_total, TC_WG_ROWS)) return r;
-        if (int r = make_tmap_f16(&tm_o1, p.out_lo, (uint64_t)p.M, (uint64_t)p.N_total, TC_WG_ROWS)) return r;
+        if (int r = make_tmap_f16(&tm_o0, p.out_hi, (uint64_t)p.M, (uint64_t)p.N_total, TC_FRAG_ROWS)) return r;
+        if (int r = make_tmap_f16(&tm_o1, p.out_lo, (uint64_t)p.M, (uint64_t)p.N_total, TC_FRAG_ROWS)) return r;
     }
     const int m_tiles = (p.M + TC_BLOCK_M - 1) / TC_BLOCK_M, n_tiles = (p.N_total + TC_BLOCK_N - 1) / TC_BLOCK_N;
     int avail = num_sms() - leave_free_sms;
     if (avail < 16) avail = 16;
     if (avail > num_sms()) avail = num_sms();
-    // work units: whole row tiles (n_groups = 1, the A rows of the second N tile come out of L2 while still hot) unless single
-    // tiles make the last round shorter -- a 70k-row chunk on 100 CTAs: 547 row tiles take 6 rounds, 1094 tiles 5.5
-    const int64_t rounds_rows = (int64_t)(m_tiles + avail - 1) / avail * n_tiles;          // in tile times
-    const int64_t rounds_tiles = ((int64_t)m_tiles * n_tiles + avail - 1) / avail;
-    p.n_groups = (m_tiles < 2 * avail || rounds_tiles < rounds_rows) ? n_tiles : 1;
     {
         static int dbg = -1;
         if (dbg < 0) { const char *e = getenv("GANSPACE_B200_MAPPING_DBG"); dbg = e ? atoi(e) : 0; }
         p.dbg = dbg;
     }
-    const int units = m_tiles * p.n_groups;
-    const int grid = units < avail ? units : avail;
+    // work units: single 128 x 128 tiles, two consumer warpgroups per CTA -- a 70k-row chunk (2,188 tiles) on 100 CTAs wastes
+    // about 1 % in the last round
+    const int64_t units = (int64_t)m_tiles * n_tiles;
+    const int grid = units < avail ? (int)units : avail;
     mapping_layer_tc_kernel<<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(tm_ah, tm_al, tm_wh, tm_wl, tm_o0, tm_o1, p);
     GSB_CHECK_LAUNCH();
     return GSB_OK;
 }
 
 // out[M, N] (fp32, row-major) = (A_hi + A_lo)[M, K] * (W_hi + W_lo)[N, K]^T * inv_wscale   -- the same persistent
-// tensor-core kernel with the plain epilogue.  Both operands are K-major fp16 hi/lo pairs; K % 64 == 0, N % 256 == 0.
+// tensor-core kernel with the plain epilogue.  Both operands are K-major fp16 hi/lo pairs; N % 32 == 0, K % 8 == 0 (the TMA
+// unit zero-fills the operand boxes of a ragged last N or K tile and clips its stores).
 // Used by the modulated-convolution path (synthesis.cu): one dense contraction per 3x3 tap.
 int tc_gemm_plain(const __half *a_hi, const __half *a_lo, int64_t M, int K, const __half *w_hi, const __half *w_lo, int N,
                   const float *inv_wscale, float *out, unsigned *overflow, int leave_free_sms, cudaStream_t st) {
@@ -417,7 +426,7 @@ int tc_gemm_plain(const __half *a_hi, const __half *a_lo, int64_t M, int K, cons
     if (int r = make_tmap_f16(&tm_wl, w_lo, (uint64_t)N, (uint64_t)K, TC_BLOCK_N)) return r;
     TcParams p;
     p.bias = nullptr; p.out_hi = nullptr; p.out_lo = nullptr; p.out_f32 = out; p.overflow = overflow;
-    p.inv_wscale = inv_wscale; p.M = (int)M; p.N_total = N; p.K = K; p.mode = 1; p.n_groups = 1;
+    p.inv_wscale = inv_wscale; p.M = (int)M; p.N_total = N; p.K = K; p.mode = 1;
     return tc_launch_layer(tm_ah, tm_al, tm_wh, tm_wl, p, leave_free_sms, st);
 }
 
@@ -431,7 +440,7 @@ size_t tc_linear_workspace_bytes(int64_t n, int N, int K) {
 
 int tc_linear(const float *x, const float *w, const float *bias, float *y, int64_t n, int N, int K, bool lrelu, void *ws,
               cudaStream_t st) {
-    GSB_CHECK_ARG(N % TC_BLOCK_N == 0 && K % TC_BLOCK_K == 0 && n > 0 && n < (1ll << 31) && bias, "tc_linear: need N%%256==0, K%%64==0, bias");
+    GSB_CHECK_ARG(N % 256 == 0 && K % TC_BLOCK_K == 0 && n > 0 && n < (1ll << 31) && bias, "tc_linear: need N%%256==0, K%%64==0, bias");
     if (int r = tc_ensure_attr()) return r;
     char *p0 = reinterpret_cast<char *>(ws);
     const size_t xb = align_up((size_t)n * K * 2, 256), wb = align_up((size_t)N * K * 2, 256);
@@ -454,7 +463,7 @@ int tc_linear(const float *x, const float *w, const float *bias, float *y, int64
     if (int r = make_tmap_f16(&tm_wl, w_lo, (uint64_t)N, (uint64_t)K, TC_BLOCK_N)) return r;
     TcParams p;
     p.bias = bias; p.out_hi = nullptr; p.out_lo = nullptr; p.out_f32 = y; p.overflow = overflow;
-    p.inv_wscale = scal; p.M = (int)n; p.N_total = N; p.K = K; p.mode = lrelu ? 0 : 2; p.n_groups = 1;
+    p.inv_wscale = scal; p.M = (int)n; p.N_total = N; p.K = K; p.mode = lrelu ? 0 : 2;
     return tc_launch_layer(tm_ah, tm_al, tm_wh, tm_wl, p, 0, st);
 }
 
@@ -462,7 +471,7 @@ int tc_linear(const float *x, const float *w, const float *bias, float *y, int64
 int mapping_forward_tc(const float *pb, void *tc_base, int n_layers, int dim,
                        const float *d_z, float *d_w, int64_t n, bool pixelnorm, void *ws, int leave_free_sms,
                        cudaStream_t st) {
-    GSB_CHECK_ARG(dim % TC_BLOCK_N == 0 && dim % TC_BLOCK_K == 0, "mapping_forward_tc: dim must be a multiple of 256");
+    GSB_CHECK_ARG(dim % 256 == 0 && dim % TC_BLOCK_K == 0, "mapping_forward_tc: dim must be a multiple of 256");
     GSB_CHECK_ARG(n < (1ll << 31), "mapping_forward_tc: too many rows");
     TcPackView v = tc_pack_view(tc_base, n_layers, dim);
     const size_t buf = align_up((size_t)n * dim * 2, 256);
@@ -491,7 +500,7 @@ int mapping_forward_tc(const float *pb, void *tc_base, int n_layers, int dim,
         p.out_f32 = last ? d_w : nullptr;
         p.overflow = v.overflow;
         p.inv_wscale = v.inv_wscale + l;
-        p.M = (int)n; p.N_total = dim; p.K = dim; p.mode = 0; p.n_groups = 1;
+        p.M = (int)n; p.N_total = dim; p.K = dim; p.mode = 0;
         if (int r = tc_launch_layer(tm_ah, tm_al, tm_wh, tm_wl, p, leave_free_sms, st)) return r;
     }
     return GSB_OK;

@@ -1,8 +1,9 @@
 // wgmma / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (stats_tc.cu, gram_tc.cu, mapping_tc.cu).
 // sm_90a (Hopper).  The shared-memory descriptor encoding follows cute::GMMA::GmmaDescriptor.
 //
-// Warp layout of every kernel here: warpgroups 0 and 1 (warps 0-7) are the MMA consumers, each owns 64 rows of a
-// 128-row tile and keeps its accumulator in registers; warp 8 is the TMA producer (one elected thread).
+// Warp layout: warpgroups 0 and 1 (warps 0-7) are the MMA consumers and keep their accumulators in registers; warp 8 holds
+// the TMA producer (one elected thread).  In stats_tc.cu and gram_tc.cu each consumer warpgroup owns 64 rows of a 128-row
+// tile; mapping_tc.cu gives each whole 128 x 128 tiles in turns and makes warps 8-11 a producer warpgroup (setmaxnreg).
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
@@ -66,6 +67,8 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, const void 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// all but the most recently committed wgmma group have completed
+__device__ __forceinline__ void wgmma_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
 // K-major, SWIZZLE_128B shared-memory matrix descriptor (tile base 1024-byte aligned):
 //   [0,14) start>>4 | [16,30) LBO>>4 (unused for swizzled K-major) | [32,46) SBO>>4 (8 rows * 128 B = 1024)
