@@ -45,11 +45,6 @@ SIGNATURES = {
     "gsb_ipca_reset": (_I, [_P, _I, _I, _P]),
     "gsb_ipca_chain_step": (_I, [_P, _I, _I, _L, _L, _P, _P, _P, _Z, _P]),
     "gsb_ipca_export": (_I, [_P, _I, _I, _L, _P, _P, _P, _P, _P, _P, _P]),
-    "gsb_ipca_chain_persistent_supported": (_I, [_I, _I]),
-    "gsb_ipca_queue_bytes": (_Z, [_I]),
-    "gsb_ipca_queue_reset": (_I, [_P, _I, _P]),
-    "gsb_ipca_queue_publish": (_I, [_P, _I, _I, _I, _P, _P, _I, _I, _I, _I, _I, _P]),
-    "gsb_ipca_chain_run": (_I, [_P, _I, _I, _L, _P, _I, _I, _I, _P, _Z, _P]),
     "gsb_sym_eig_top": (_I, [_P, _I, _I, _P, _P, _P, _Z, _P]),
     "gsb_eig_status": (_I, [_P, _P]),
     "gsb_project_std_workspace_bytes": (_Z, [_I]),
@@ -116,7 +111,7 @@ def load():
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(lib, name)          # AttributeError if the header and the library drift apart
             fn.restype, fn.argtypes = res, args
-        if lib.gsb_abi_version() != 1:
+        if lib.gsb_abi_version() != 2:
             raise NativeError("ABI version mismatch between ganspace_b200/_native.py and the library")
         _lib = lib
     return _lib
@@ -518,70 +513,12 @@ class IPCAChain:
         # kernels per step: first step = direct solve (8) + seeding of the subspace form (1); later steps = one cluster
         # launch (orthogonal iteration, csrc/subspace.cu).  Shapes outside the subspace kernel's range: direct solve (8).
         subspace = (self.d % 128 == 0 and 128 <= self.d <= 512 and self.c % 8 == 0 and 8 <= self.c <= 128
-                    and os.environ.get("GANSPACE_B200_CHAIN", "") not in ("direct", "lanczos") and not _chain_forced_direct)
+                    and os.environ.get("GANSPACE_B200_CHAIN", "") != "direct" and not _chain_forced_direct)
         instrument.count((1 if self.n_seen > 0 else 9) if subspace else 8)
         self.n_seen += int(n_batch)
 
-    # ---- persistent run: ONE resident cluster kernel for steps 1 .. K-1, fed through a device queue (csrc/subspace.cu) --------
-    def begin_run(self, n_groups: int, n_batch: int) -> bool:
-        """Declare a run of ``n_groups`` equal batches.  Returns False (and changes nothing) when the shape has no persistent
-        kernel or GANSPACE_B200_CHAIN_PERSISTENT=0; then every step() is its own launch."""
-        lib = load()
-        # Opt-in (GANSPACE_B200_CHAIN_PERSISTENT=1).  Measured on config 2: no gain over one launch per step once the producers
-        # leave SMs free, and a hazard: with CUDA's lazy module loading the first launch of any not-yet-loaded kernel blocks until
-        # the resident kernel exits (it then gives up after its timeout).  Use with CUDA_MODULE_LOADING=EAGER or after a warm-up.
-        if (n_groups < 2 or self.n_seen != 0 or os.environ.get("GANSPACE_B200_CHAIN_PERSISTENT", "0") != "1"
-                or not lib.gsb_ipca_chain_persistent_supported(self.d, self.c)):
-            return False
-        self._run = {"K": int(n_groups), "nb": int(n_batch), "next": 0, "keep": [], "closed": False}
-        self._queue = torch.empty(lib.gsb_ipca_queue_bytes(n_groups), dtype=torch.uint8, device=self.dev)
-        with torch.cuda.device(self.dev):
-            _check(lib.gsb_ipca_queue_reset(_ptr(self._queue), n_groups, _stream()), "gsb_ipca_queue_reset")
-        return True
-
-    def _publish(self, k0, count, mean_base, gram_base, flag, round_first=0, world=1, per_rank=1):
-        with torch.cuda.device(self.dev):
-            _check(load().gsb_ipca_queue_publish(_ptr(self._queue), self._run["K"], int(k0), int(count), _ptr(mean_base), _ptr(gram_base),
-                                                 self.d, int(round_first), int(world), int(per_rank), int(flag), _stream()),
-                   "gsb_ipca_queue_publish")
-        instrument.count(1)
-
-    def run_step(self, n_batch: int, mean_b: torch.Tensor, gram_b: torch.Tensor):
-        """step() inside a declared run: group 0 is solved directly and followed by the launch of the resident kernel; later
-        groups are handed to it through the queue (the tensors are kept alive until the run ends)."""
-        run = self._run
-        k = run["next"]
-        assert not run["closed"] and k < run["K"] and int(n_batch) == run["nb"], "persistent chain: unexpected batch"
-        if k == 0:
-            self.step(n_batch, mean_b, gram_b)
-            lib = load()
-            with torch.cuda.device(self.dev):
-                stream = self.stream if self.stream is not None else torch.cuda.current_stream()
-                if self.stream is not None:
-                    self.stream.wait_stream(torch.cuda.current_stream())       # the queue has been reset
-                with torch.cuda.stream(stream):
-                    _check(lib.gsb_ipca_chain_run(_ptr(self.state), self.d, self.c, run["nb"], _ptr(self._queue), run["K"], 1, run["K"],
-                                                  _ptr(self.ws), self.ws.numel(), _stream()), "gsb_ipca_chain_run")
-            instrument.count(1)
-        else:
-            assert mean_b.dtype == torch.float64 and gram_b.dtype == torch.float64 and mean_b.is_contiguous() and gram_b.is_contiguous()
-            run["keep"].append((mean_b, gram_b))
-            self._publish(k, 1, mean_b, gram_b, 1)
-            self.n_seen += int(n_batch)
-        run["next"] = k + 1
-
-    def end_run(self):
-        """Close a declared run: if fewer than K groups were published (interrupt, early stop) tell the kernel to stop there."""
-        run = getattr(self, "_run", None)
-        if run is None or run["closed"]:
-            return
-        run["closed"] = True
-        if 1 <= run["next"] < run["K"]:
-            self._publish(run["next"], 1, None, None, 2)
-
     def join(self):
         """Make the current stream wait for every chain step enqueued so far."""
-        self.end_run()
         if self.stream is not None:
             with torch.cuda.device(self.dev):
                 torch.cuda.current_stream().wait_stream(self.stream)
@@ -625,9 +562,6 @@ def check_eig_status(what: str):
     flags = C.c_uint(0)
     _check(load().gsb_eig_status(C.byref(flags), _stream()), "gsb_eig_status")
     if flags.value:
-        if flags.value & 8:
-            raise NativeError(f"{what}: the resident chain kernel waited longer than GANSPACE_B200_CHAIN_TIMEOUT_S for a group's "
-                              f"statistics and gave up (status {flags.value})")
         raise ChainNotConverged(f"{what}: a chain step hit its iteration cap without reaching the residual tolerance "
                                 f"(status {flags.value}): the spectrum has no gap after component c (numerical rank below "
                                 "n_components?); the exact route is GANSPACE_B200_CHAIN=direct (decomposition.compute re-runs "
@@ -933,9 +867,7 @@ class BigIPCA:
                 dist.all_gather_into_tensor(allmax, self._rowmax)          # concatenated along dim 0 in rank order
                 signs = pick_global_signs(allmax.view(self.shard[1], self.c, 2))
                 _check(lib.gsb_bigd_step_commit(*self._args(nb), _ptr(signs), *tail), "gsb_bigd_step_commit")
-        lanczos = (os.environ.get("GANSPACE_B200_BIGD_CHAIN") == "lanczos" and self.n_seen > 0 and self.c % 16 == 0
-                   and self.c <= 128 and 3 * self.c <= self.rows // 2 + self.rows // 8)
-        instrument.count(7 + (37 if lanczos else 5) + (2 if self.flags & 1 else 0))
+        instrument.count(7 + 5 + (2 if self.flags & 1 else 0))
         self.n_seen += int(nb)
         self.last_nb = int(nb)
 

@@ -11,16 +11,12 @@
 //        T = M M^T  (n_s x n_s, n_s = c + n_b + 1 ~ 2100; fp32 products summed in fp32 over 8192-long chunks of d,
 //                    chunks accumulated in fp64)
 //        T = U diag(lambda) U^T  (top c; fp64 direct solver: L2-resident Householder tridiagonalisation, bisection,
-//                    inverse iteration (ipca.cu).  Optional: the warm-started block Lanczos of ipca.cu -- the previous
-//                    components are the first c coordinates of the small side and M^T maps its Krylov space onto the
-//                    feature-side one)
+//                    inverse iteration (ipca.cu))
 //        S_new = sqrt(lambda),   (S * Vt)_new = U^T M      (one skinny GEMM over M; rows 0..c-1 of M for the next step)
 // followed by sklearn's svd_flip sign rule on the rows and the Chan mean / variance merge per feature
 // (extmath._incremental_mean_and_var).  Nothing of size d x d or n_b x d ever leaves the device.
 #include "ipca_internal.cuh"
 #include <math.h>
-#include <stdlib.h>
-#include <string.h>
 
 namespace gsb {
 
@@ -44,27 +40,12 @@ static BigState big_state(void *p, int64_t d, int c) {
     return s;
 }
 
-// Measured on config 5 (convs.4, d = 524288, N = 200k, c = 80): the warm-started Lanczos step agrees with the direct
-// solver to cos 0.99994 on the trailing components (conv feature maps have much smaller eigen-gaps than W space, where
-// it reaches 0.999999997) and saves only ~16 ms of a ~90 ms step, so the exact direct solve is the default here;
-// GANSPACE_B200_BIGD_CHAIN=lanczos opts in.
-static bool bigd_use_lanczos() {
-    static int v = -1;
-    if (v == -1) {
-        const char *env = getenv("GANSPACE_B200_BIGD_CHAIN");
-        v = (env && strcmp(env, "lanczos") == 0) ? 1 : 0;
-    }
-    return v == 1;
-}
-
 struct BigWs {
     Workspace ew;          // ew.A doubles as T
-    void *lan;
-    double *mean_b, *E, *U, *lam;
+    double *mean_b, *U, *lam;
     float *Dnew, *rowmax;
     void *tc;              // operands of the tensor-core Gram (flags & GSB_BIGD_GRAM_TC)
     size_t bytes;
-    bool lanczos;
 };
 static BigWs big_ws(void *base, int64_t d, int c, int nb_max, int flags) {
     BigWs w;
@@ -74,10 +55,7 @@ static BigWs big_ws(void *base, int64_t d, int c, int nb_max, int flags) {
     auto take = [&](size_t bytes) { char *q = p + off; off += align_up(bytes, 256); return q; };
     const size_t eb = carve(nullptr, np, c).bytes;
     w.ew = carve(take(eb), np, c);
-    w.lanczos = bigd_use_lanczos() && lanczos_applicable(np, c);
-    w.lan = w.lanczos ? take(carve_lanczos(nullptr, np, c).bytes) : nullptr;
     w.mean_b = (double *)take((size_t)d * 8);
-    w.E = (double *)take((size_t)c * np * 8);
     w.U = (double *)take((size_t)c * np * 8);
     w.lam = (double *)take((size_t)c * 8);
     w.Dnew = (float *)take((size_t)c * d * 4);
@@ -217,11 +195,6 @@ bigd_gram_kernel(const float *__restrict__ M, int n_rows, int64_t d, int kchunk,
             if (ti != tj) atomicAdd(&T[(size_t)gn * ldt + gm], v);
         }
     }
-}
-
-__global__ void bigd_unit_rows_kernel(double *__restrict__ E, int c, int np) {
-    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx < c * np) E[idx] = (idx / np == idx % np) ? 1.0 : 0.0;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -429,15 +402,7 @@ extern "C" int gsb_bigd_step_solve(void *d_state, float *d_M, int64_t d, int c, 
     using namespace gsb;
     StepCtx x;
     if (int r = step_ctx(x, d_state, d_M, d, c, nb_max, n_seen, nb, flags, d_workspace, workspace_bytes, stream)) return r;
-    double *T = x.w.ew.A;
-    if (n_seen > 0 && x.w.lanczos) {
-        bigd_unit_rows_kernel<<<(c * x.np + 255) / 256, 256, 0, x.st>>>(x.w.E, c, x.np);
-        GSB_CHECK_LAUNCH();
-        LanczosWs lw = carve_lanczos(x.w.lan, x.np, c);
-        if (int r = eig_top_lanczos(lw, T, x.w.E, x.np, c, x.w.lam, x.w.U, x.st)) return r;
-    } else {
-        if (int r = eig_top(x.w.ew, x.np, c, x.w.lam, x.w.U, x.st)) return r;
-    }
+    if (int r = eig_top(x.w.ew, x.np, c, x.w.lam, x.w.U, x.st)) return r;      // ew.A holds T (and is destroyed)
     bigd_project_kernel<<<(unsigned)((d + PJ_COLS - 1) / PJ_COLS), 256, 0, x.st>>>(x.w.U, x.np, d_M, x.n_rows, d, c, x.w.Dnew);
     GSB_CHECK_LAUNCH();
     bigd_rowmax_kernel<<<c, 1024, 0, x.st>>>(x.w.Dnew, d, x.w.rowmax);

@@ -17,8 +17,6 @@
 //   4. backtransform_kernel  applies the reflectors (one warp per eigenvector) and the sign rule.
 #include "ipca_internal.cuh"
 #include <math.h>
-#include <stdlib.h>
-#include <string.h>
 
 namespace gsb {
 
@@ -959,13 +957,6 @@ int *eig_status_device_ptr() {
     return p;
 }
 
-int launch_cluster_orth(const double *lam, const double *dg, const double *e, int n, int c, double *Z, cudaStream_t st) {
-    const size_t co_smem = ((size_t)n + c + 64) * sizeof(double) + (size_t)c * sizeof(int);
-    cluster_orth_kernel<<<1, CO_THREADS, co_smem, st>>>(lam, dg, e, n, c, Z);
-    GSB_CHECK_LAUNCH();
-    return GSB_OK;
-}
-
 int eig_top(const Workspace &w, int d, int c, double *evals, double *evecs, cudaStream_t st) {
     if (d > 1024) return eig_top_big(w, d, c, evals, evecs, st);
     // Preferred: one 16-CTA cluster (hardware barrier) when the column blocks fit in shared memory.
@@ -973,14 +964,11 @@ int eig_top(const Workspace &w, int d, int c, double *evals, double *evecs, cuda
     const size_t cl_smem = ((size_t)(d / TRI_CLUSTER) * d + 5 * (size_t)d + 64) * sizeof(double);
     bool use_cluster = (d % TRI_CLUSTER == 0) && cl_smem <= 227 * 1024;
     if (use_cluster && cluster_ok == -1) {
-        const char *env = getenv("GANSPACE_B200_TRIDIAG");
-        cluster_ok = (env && strcmp(env, "grid") == 0) ? 0 : 1;
-        if (cluster_ok) {
-            if (cudaFuncSetAttribute(tridiag_kernel<true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
-                cudaFuncSetAttribute(tridiag_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
-                cluster_ok = 0;
-                (void)cudaGetLastError();
-            }
+        cluster_ok = 1;
+        if (cudaFuncSetAttribute(tridiag_kernel<true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
+            cudaFuncSetAttribute(tridiag_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
+            cluster_ok = 0;
+            (void)cudaGetLastError();
         }
         if (cluster_ok) {
             cudaLaunchConfig_t q{};
@@ -1006,10 +994,8 @@ int eig_top(const Workspace &w, int d, int c, double *evals, double *evecs, cuda
         cfg.attrs = at; cfg.numAttrs = 1;
         static int reg_variant = -1;
         if (reg_variant == -1) {
-            const char *env = getenv("GANSPACE_B200_TRIDIAG");
-            reg_variant = (env && strcmp(env, "smem") == 0) ? 0 : 1;
-            if (reg_variant &&
-                cudaFuncSetAttribute(tridiag_reg_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) {
+            reg_variant = 1;
+            if (cudaFuncSetAttribute(tridiag_reg_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) {
                 reg_variant = 0;
                 (void)cudaGetLastError();
             }
@@ -1104,167 +1090,6 @@ static int eig_top_big(const Workspace &w, int d, int c, double *evals, double *
     return GSB_OK;
 }
 
-// =============================================================================================
-// Warm-started block-Lanczos Rayleigh-Ritz chain step.
-//
-// The direct solver above costs ~n dependent reflector steps (n = 512 -> ~2 ms).  From the second chain
-// step on, the previous components V_{k-1} span the wanted invariant subspace up to O(1/k), so the top-c
-// eigenpairs of G are taken from the block Krylov space  span[Q0, Q1, Q2],  Q0 = V_{k-1}^T,
-// Q_{j+1} = orth((I - P_j) G Q_j)  (full re-orthogonalisation, twice), by Rayleigh-Ritz on the 3c x 3c
-// projection  H = Qb^T G Qb  -- solved with the same direct eigensolver at n = 3c.  Against the exact chain on
-// config 2 (100 steps, c = 80) it agrees far inside the 0.999 / 1e-3 tolerance, and the result is still
-// independent of the world size.  All of it is fp64 GEMM-shaped work spread over the whole GPU.
-// =============================================================================================
-template <bool TA, bool TB>
-__global__ void __launch_bounds__(256)
-dgemm_kernel(int M, int N, int K, double alpha, const double *__restrict__ A, int lda,
-             const double *__restrict__ B, int ldb, double beta, double *__restrict__ C, int ldc, int kchunk) {
-    // C[M,N] = alpha * op(A)[M,K] * op(B)[K,N] + beta * C   (row-major; op = transpose when the flag is set).
-    // gridDim.z > 1: split-K, every CTA adds alpha * partial with fp64 atomics (caller pre-scales C by beta).
-    __shared__ double As[16][33], Bs[16][33];
-    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-    const int m0 = blockIdx.y * 32, n0 = blockIdx.x * 32;
-    const int kbeg = blockIdx.z * kchunk, kend = (kbeg + kchunk < K) ? kbeg + kchunk : K;
-    double acc[2][2] = {{0, 0}, {0, 0}};
-    for (int k0 = kbeg; k0 < kend; k0 += 16) {
-        for (int idx = tid; idx < 512; idx += 256) {
-            int mm, kk;
-            if (TA) { mm = idx & 31; kk = idx >> 5; } else { kk = idx & 15; mm = idx >> 4; }
-            const int m = m0 + mm, k = k0 + kk;
-            As[kk][mm] = (m < M && k < kend) ? (TA ? A[(size_t)k * lda + m] : A[(size_t)m * lda + k]) : 0.0;
-            int nn, k2;
-            if (TB) { k2 = idx & 15; nn = idx >> 4; } else { nn = idx & 31; k2 = idx >> 5; }
-            const int n = n0 + nn, kb = k0 + k2;
-            Bs[k2][nn] = (n < N && kb < kend) ? (TB ? B[(size_t)n * ldb + kb] : B[(size_t)kb * ldb + n]) : 0.0;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int kk = 0; kk < 16; ++kk) {
-            const double a0 = As[kk][ty], a1 = As[kk][ty + 16], b0 = Bs[kk][tx], b1 = Bs[kk][tx + 16];
-            acc[0][0] += a0 * b0; acc[0][1] += a0 * b1; acc[1][0] += a1 * b0; acc[1][1] += a1 * b1;
-        }
-        __syncthreads();
-    }
-#pragma unroll
-    for (int r = 0; r < 2; ++r)
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-            const int m = m0 + ty + 16 * r, n = n0 + tx + 16 * q;
-            if (m < M && n < N) {
-                if (gridDim.z > 1) {
-                    atomicAdd(&C[(size_t)m * ldc + n], alpha * acc[r][q]);
-                } else {
-                    double v = alpha * acc[r][q];
-                    if (beta != 0.0) v += beta * C[(size_t)m * ldc + n];
-                    C[(size_t)m * ldc + n] = v;
-                }
-            }
-        }
-}
-
-// beta must be 0 or 1.  Splits K so that the launch fills the machine (these GEMMs have few output tiles).
-template <bool TA, bool TB>
-static int dgemm(int M, int N, int K, double alpha, const double *A, int lda, const double *B, int ldb, double beta,
-                 double *C, int ldc, cudaStream_t st) {
-    const int tiles = ((N + 31) / 32) * ((M + 31) / 32);
-    int splits = 1;
-    while (splits < 8 && tiles * splits < 2 * num_sms() && K / (splits * 2) >= 64) splits *= 2;
-    const int kchunk = ((K + splits - 1) / splits + 15) / 16 * 16;
-    if (splits > 1 && beta == 0.0) GSB_CHECK_CUDA(cudaMemset2DAsync(C, (size_t)ldc * 8, 0, (size_t)N * 8, M, st));
-    dim3 grid((N + 31) / 32, (M + 31) / 32, splits);
-    dgemm_kernel<TA, TB><<<grid, 256, 0, st>>>(M, N, K, alpha, A, lda, B, ldb, beta, C, ldc, kchunk);
-    GSB_CHECK_LAUNCH();
-    return GSB_OK;
-}
-
-// Right-looking Cholesky of the k x k Gram matrix C (k <= 128) in shared memory, one CTA of 256 threads
-// (8 warps): per column j a pivot, a column scale and a rank-1 update of the trailing lower triangle spread
-// over all threads (lane <-> column q, warp <-> row i), three barriers per column.  Pivots below
-// 1e-26 * max diagonal are clamped (numerically dependent residual directions).  Writes L (zero upper part).
-__global__ void __launch_bounds__(256)
-chol_kernel(const double *__restrict__ C, int k, double *__restrict__ Lout) {
-    extern __shared__ double smd[];
-    double *L = smd;                         // [k][k+1]
-    __shared__ double s_floor;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, ld = k + 1;
-    for (int idx = tid; idx < k * k; idx += 256) L[(idx / k) * ld + idx % k] = C[idx];
-    __syncthreads();
-    if (tid == 0) {
-        double dmax = 0.0;
-        for (int j = 0; j < k; ++j) dmax = fmax(dmax, L[j * ld + j]);
-        s_floor = fmax(dmax * 1e-26, 1e-300);
-    }
-    __syncthreads();
-    const double floor_ = s_floor;
-    for (int j = 0; j < k; ++j) {
-        double piv = L[j * ld + j];
-        if (!(piv > floor_)) piv = floor_;
-        const double inv = 1.0 / sqrt(piv);
-        __syncthreads();                                         // everyone has read the pivot
-        for (int i = j + tid; i < k; i += 256) L[i * ld + j] = (i == j) ? sqrt(piv) : L[i * ld + j] * inv;
-        __syncthreads();
-        for (int i = j + 1 + warp; i < k; i += 8) {              // trailing update, lower triangle only
-            const double lij = L[i * ld + j];
-            for (int q = j + 1 + lane; q <= i; q += 32) L[i * ld + q] -= lij * L[q * ld + j];
-        }
-        __syncthreads();
-    }
-    for (int idx = tid; idx < k * k; idx += 256) {
-        const int r = idx / k, q = idx % k;
-        Lout[idx] = (q <= r) ? L[r * ld + q] : 0.0;
-    }
-}
-
-// Q = L^-1 R for R[k,d] (rows): one thread per column of R; the solved column lives in shared memory
-// ([k][64], conflict-free) so that the loops stay rolled (a fully unrolled register version thrashes the
-// instruction cache); row dot products on four independent accumulators.
-constexpr int TRSM_THREADS = 64;
-__global__ void __launch_bounds__(TRSM_THREADS)
-trsm_rows_kernel(const double *__restrict__ Lg, int k, const double *__restrict__ R, int d, double *__restrict__ Q) {
-    extern __shared__ double smd[];
-    double *L = smd;                              // [k][k]
-    double *qs = smd + (size_t)k * k;             // [k][TRSM_THREADS]
-    for (int idx = threadIdx.x; idx < k * k; idx += TRSM_THREADS) L[idx] = Lg[idx];
-    const int col = blockIdx.x * TRSM_THREADS + threadIdx.x;
-    const bool ok = col < d;
-    double *q = qs + threadIdx.x;
-    for (int r = 0; r < k; ++r) q[r * TRSM_THREADS] = ok ? R[(size_t)r * d + col] : 0.0;
-    __syncthreads();
-    for (int r = 0; r < k; ++r) {
-        const double *lr = L + r * k;
-        double a0 = q[r * TRSM_THREADS], a1 = 0.0, a2 = 0.0, a3 = 0.0;
-        int p = 0;
-        for (; p + 4 <= r; p += 4) {
-            a0 -= lr[p] * q[p * TRSM_THREADS];
-            a1 -= lr[p + 1] * q[(p + 1) * TRSM_THREADS];
-            a2 -= lr[p + 2] * q[(p + 2) * TRSM_THREADS];
-            a3 -= lr[p + 3] * q[(p + 3) * TRSM_THREADS];
-        }
-        for (; p < r; ++p) a0 -= lr[p] * q[p * TRSM_THREADS];
-        q[r * TRSM_THREADS] = ((a0 + a1) + (a2 + a3)) / lr[r];
-    }
-    if (ok)
-        for (int r = 0; r < k; ++r) Q[(size_t)r * d + col] = q[r * TRSM_THREADS];
-}
-
-// Newton-Schulz polish of an almost orthonormal row block: given C = Q Q^T, writes N = 1.5 I - 0.5 C so that
-// Q <- N Q has orthogonality error O(||C - I||^2).
-__global__ void ns_matrix_kernel(const double *__restrict__ C, int k, double *__restrict__ N) {
-    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx < k * k) N[idx] = ((idx / k == idx % k) ? 1.5 : 0.0) - 0.5 * C[idx];
-}
-
-__global__ void symmetrize_kernel(double *__restrict__ H, int n) {
-    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= n * n) return;
-    const int i = idx / n, j = idx % n;
-    if (j > i) {
-        const double v = 0.5 * (H[(size_t)i * n + j] + H[(size_t)j * n + i]);
-        H[(size_t)i * n + j] = v;
-        H[(size_t)j * n + i] = v;
-    }
-}
-
 // svd_flip sign rule on the rows of V[c,d] (largest |.| entry positive; first index on ties)
 __global__ void sign_rows_kernel(double *__restrict__ V, int c, int d) {
     const int lane = threadIdx.x & 31, t = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -1291,104 +1116,8 @@ int sign_rows(double *V, int c, int d, cudaStream_t st) {
     return GSB_OK;
 }
 
-LanczosWs carve_lanczos(void *base, int d, int c) {
-    LanczosWs w;
-    char *p = reinterpret_cast<char *>(base);
-    size_t off = 0;
-    auto take = [&](size_t bytes) { char *q = p + off; off += align_up(bytes, 256); return q; };
-    const int kd = 3 * c;
-    w.QbT = (double *)take((size_t)kd * d * 8);
-    w.RT = (double *)take((size_t)c * d * 8);
-    w.T = (double *)take((size_t)c * kd * 8);
-    w.C = (double *)take((size_t)c * c * 8);
-    w.Linv = (double *)take((size_t)c * c * 8);
-    w.WT = (double *)take((size_t)kd * d * 8);
-    w.H = (double *)take((size_t)kd * kd * 8);
-    w.U = (double *)take((size_t)c * kd * 8);
-    w.lamH = (double *)take((size_t)c * 8);
-    w.eig_ws = take(carve(nullptr, kd, c).bytes);
-    w.bytes = off;
-    return w;
-}
 static int g_chain_force_direct = 0;     // host-side switch, read when a step is enqueued (not thread-safe across handles, as the ABI states)
 bool chain_forced_direct() { return g_chain_force_direct != 0; }
-
-bool lanczos_applicable(int d, int c) {
-    if (chain_forced_direct()) return false;
-    // Round 2: the default chain step is the residual-checked orthogonal iteration of subspace.cu; where it does not apply
-    // the step is the direct solve of the full d x d problem.  The warm-started block-Lanczos step of round 1 (no
-    // convergence check) is an explicit opt-in: GANSPACE_B200_CHAIN=lanczos.
-    static int mode = -1;            // 0 = never, 1 = opted in
-    if (mode == -1) {
-        const char *env = getenv("GANSPACE_B200_CHAIN");
-        mode = (env && strcmp(env, "lanczos") == 0) ? 1 : 0;
-    }
-    const bool shapes_ok = c % 16 == 0 && c <= 128 && 3 * c <= d / 2 + d / 8 && 3 * c <= 512;
-    if (mode == 0 || !shapes_ok) return false;
-    return mode == 1;
-}
-
-// orthonormalise the rows of RT[k,d] into out[k,d]: one CholQR pass (Gram, Cholesky, triangular solve) followed
-// by two Newton-Schulz polishing steps (Gram + small GEMM each; quadratic, no sequential dependency).  RT is scratch.
-static int cholqr2_rows(const LanczosWs &lw, double *RT, double *out, int k, int d, cudaStream_t st) {
-    const size_t smem_c = (size_t)k * (k + 1) * sizeof(double);
-    const size_t smem_t = ((size_t)k * k + (size_t)k * TRSM_THREADS) * sizeof(double);
-    static size_t set_c = 0, set_t = 0;
-    if (smem_c > set_c) {
-        GSB_CHECK_CUDA(cudaFuncSetAttribute(chol_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
-        set_c = smem_c;
-    }
-    if (smem_t > set_t) {
-        GSB_CHECK_CUDA(cudaFuncSetAttribute(trsm_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_t));
-        set_t = smem_t;
-    }
-    if (int r = dgemm<false, true>(k, k, d, 1.0, RT, d, RT, d, 0.0, lw.C, k, st)) return r;             // C = R R^T
-    chol_kernel<<<1, 256, smem_c, st>>>(lw.C, k, lw.Linv);                                             // Linv holds L
-    GSB_CHECK_LAUNCH();
-    trsm_rows_kernel<<<(unsigned)((d + TRSM_THREADS - 1) / TRSM_THREADS), TRSM_THREADS, smem_t, st>>>(lw.Linv, k, RT, d, out);
-    GSB_CHECK_LAUNCH();
-    double *cur = out, *nxt = RT;
-    for (int pass = 0; pass < 2; ++pass) {
-        if (int r = dgemm<false, true>(k, k, d, 1.0, cur, d, cur, d, 0.0, lw.C, k, st)) return r;       // C = Q Q^T
-        ns_matrix_kernel<<<(k * k + 255) / 256, 256, 0, st>>>(lw.C, k, lw.Linv);
-        GSB_CHECK_LAUNCH();
-        if (int r = dgemm<false, false>(k, d, k, 1.0, lw.Linv, k, cur, d, 0.0, nxt, d, st)) return r;   // Q <- N Q
-        double *t = cur; cur = nxt; nxt = t;
-    }
-    if (cur != out) GSB_CHECK_CUDA(cudaMemcpyAsync(out, cur, (size_t)k * d * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    return GSB_OK;
-}
-
-// top-c eigenpairs of the symmetric G[d,d] from the block Krylov space of the previous components Vprev[c,d]
-int eig_top_lanczos(const LanczosWs &lw, const double *G, const double *Vprev, int d, int c, double *evals,
-                    double *evecs, cudaStream_t st) {
-    const int kd = 3 * c;
-    GSB_CHECK_CUDA(cudaMemcpyAsync(lw.QbT, Vprev, (size_t)c * d * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    for (int j = 0; j < 2; ++j) {
-        const int kb = (j + 1) * c;                       // rows of the basis built so far
-        const double *Qj = lw.QbT + (size_t)j * c * d;
-        double *Wj = lw.WT + (size_t)j * c * d;                                                           // rows j of W = Qb G
-        if (int r = dgemm<false, false>(c, d, d, 1.0, Qj, d, G, d, 0.0, Wj, d, st)) return r;             // W_j = Q_j G
-        GSB_CHECK_CUDA(cudaMemcpyAsync(lw.RT, Wj, (size_t)c * d * sizeof(double), cudaMemcpyDeviceToDevice, st));
-        for (int pass = 0; pass < 2; ++pass) {                                                           // R -= (R B^T) B
-            if (int r = dgemm<false, true>(c, kb, d, 1.0, lw.RT, d, lw.QbT, d, 0.0, lw.T, kb, st)) return r;
-            if (int r = dgemm<false, false>(c, d, kb, -1.0, lw.T, kb, lw.QbT, d, 1.0, lw.RT, d, st)) return r;
-        }
-        if (int r = cholqr2_rows(lw, lw.RT, lw.QbT + (size_t)kb * d, c, d, st)) return r;
-    }
-    if (int r = dgemm<false, false>(c, d, d, 1.0, lw.QbT + (size_t)2 * c * d, d, G, d, 0.0, lw.WT + (size_t)2 * c * d, d,
-                                    st)) return r;                                                        // W_2 = Q_2 G
-    if (int r = dgemm<false, true>(kd, kd, d, 1.0, lw.WT, d, lw.QbT, d, 0.0, lw.H, kd, st)) return r;      // H = W Qb^T
-    symmetrize_kernel<<<(kd * kd + 255) / 256, 256, 0, st>>>(lw.H, kd);
-    GSB_CHECK_LAUNCH();
-    Workspace ew = carve(lw.eig_ws, kd, c);
-    GSB_CHECK_CUDA(cudaMemcpyAsync(ew.A, lw.H, (size_t)kd * kd * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    if (int r = eig_top(ew, kd, c, evals, lw.U, st)) return r;
-    if (int r = dgemm<false, false>(c, d, kd, 1.0, lw.U, kd, lw.QbT, d, 0.0, evecs, d, st)) return r;      // V = U Qb
-    sign_rows_kernel<<<(c + 7) / 8, 256, 0, st>>>(evecs, c, d);
-    GSB_CHECK_LAUNCH();
-    return GSB_OK;
-}
 
 static int check_dims(int d, int c) {
     GSB_CHECK_ARG(d >= 32 && d <= 1024 && d % 32 == 0, "ipca: small-d engine needs 32 <= d <= 1024, d%%32==0 (d=%d)", d);
@@ -1404,7 +1133,6 @@ extern "C" size_t gsb_ipca_state_bytes(int d, int c) {
 
 extern "C" size_t gsb_ipca_workspace_bytes(int d, int c) {
     size_t b = gsb::carve(nullptr, d, c).bytes;
-    if (gsb::lanczos_applicable(d, c)) b += gsb::carve_lanczos(nullptr, d, c).bytes;
     if (gsb::subspace_applicable(d, c)) b += gsb::carve_subspace(nullptr, d, c).bytes;
     return b;
 }
@@ -1435,8 +1163,7 @@ extern "C" int gsb_ipca_chain_step(void *d_state, int d, int c, int64_t n_seen, 
     const bool subspace = gsb::subspace_applicable(d, c);
     if (subspace && n_seen > 0) {
         // steps 2..K: orthogonal iteration on (Q, H), one cluster launch (subspace.cu)
-        size_t off = w.bytes;
-        if (gsb::lanczos_applicable(d, c)) off += gsb::carve_lanczos(nullptr, d, c).bytes;
+        const size_t off = w.bytes;
         gsb::SubspaceWs sw = gsb::carve_subspace(reinterpret_cast<char *>(d_workspace) + off, d, c);
         if (workspace_bytes < off + sw.bytes) {
             gsb::set_error("ipca_chain_step: workspace too small (%zu < %zu)", workspace_bytes, off + sw.bytes);
@@ -1449,16 +1176,7 @@ extern "C" int gsb_ipca_chain_step(void *d_state, int d, int c, int64_t n_seen, 
     gsb::build_g_kernel<<<grid, block, 0, st>>>(d_gram_b, d_mean_b, s.mean, s.S, s.V, d, c, (double)n_seen,
                                                 (double)n_batch, w.A);
     GSB_CHECK_LAUNCH();
-    if (n_seen > 0 && gsb::lanczos_applicable(d, c)) {
-        gsb::LanczosWs lw = gsb::carve_lanczos(reinterpret_cast<char *>(d_workspace) + w.bytes, d, c);
-        if (workspace_bytes < w.bytes + lw.bytes) {
-            gsb::set_error("ipca_chain_step: workspace too small (%zu < %zu)", workspace_bytes, w.bytes + lw.bytes);
-            return GSB_ERR_WORKSPACE;
-        }
-        if (int r = gsb::eig_top_lanczos(lw, w.A, s.V, d, c, w.lam, w.evecs, st)) return r;
-    } else {
-        if (int r = gsb::eig_top(w, d, c, w.lam, w.evecs, st)) return r;
-    }
+    if (int r = gsb::eig_top(w, d, c, w.lam, w.evecs, st)) return r;
     size_t tot = (size_t)c * d;
     gsb::finalize_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(
         s.hdr, s.mean, s.unnorm, s.S, s.V, d_mean_b, d_gram_b, w.lam, w.evecs, d, c, (double)n_seen,
@@ -1476,46 +1194,6 @@ extern "C" int gsb_ipca_set_chain_mode(int mode) {
     GSB_CHECK_ARG(mode == 0 || mode == 1, "ipca_set_chain_mode: mode must be 0 or 1");
     gsb::g_chain_force_direct = mode;
     return GSB_OK;
-}
-
-// ---- persistent chain (subspace.cu): steps k_begin .. k_end-1 in ONE launch, fed through a queue -----------------------------
-extern "C" int gsb_ipca_chain_persistent_supported(int d, int c) { return gsb::subspace_applicable(d, c) ? 1 : 0; }
-
-extern "C" size_t gsb_ipca_queue_bytes(int n_groups) { return gsb::chain_queue_bytes(n_groups); }
-
-extern "C" int gsb_ipca_queue_reset(void *d_queue, int n_groups, gsb_stream_t stream) {
-    GSB_CHECK_ARG(d_queue && n_groups > 0, "ipca_queue_reset: bad arguments");
-    return gsb::chain_queue_reset(d_queue, n_groups, (cudaStream_t)stream);
-}
-
-extern "C" int gsb_ipca_queue_publish(void *d_queue, int n_groups, int k0, int count, const double *d_mean_base,
-                                      const double *d_gram_base, int d, int round_first, int world, int per_rank, int flag,
-                                      gsb_stream_t stream) {
-    GSB_CHECK_ARG(d_queue && k0 >= 0 && count >= 1 && k0 + count <= n_groups && (flag == 1 || flag == 2) && world >= 1 && per_rank >= 1,
-                  "ipca_queue_publish: bad arguments (k0=%d count=%d groups=%d flag=%d)", k0, count, n_groups, flag);
-    GSB_CHECK_ARG(flag == 2 || (d_mean_base && d_gram_base), "ipca_queue_publish: null statistics");
-    return gsb::chain_queue_publish(d_queue, k0, count, d_mean_base, d_gram_base, d, round_first, world, per_rank, flag,
-                                    (cudaStream_t)stream);
-}
-
-extern "C" int gsb_ipca_chain_run(void *d_state, int d, int c, int64_t n_batch, void *d_queue, int n_groups, int k_begin, int k_end,
-                                  void *d_workspace, size_t workspace_bytes, gsb_stream_t stream) {
-    GSB_CHECK_ARG(d_state && d_queue && d_workspace, "ipca_chain_run: null pointer");
-    if (int r = gsb::check_dims(d, c)) return r;
-    GSB_CHECK_ARG(gsb::subspace_applicable(d, c), "ipca_chain_run: shape (d=%d, c=%d) has no persistent chain kernel", d, c);
-    GSB_CHECK_ARG(n_batch > 0 && k_begin >= 1 && k_begin <= k_end && k_end <= n_groups, "ipca_chain_run: bad step range [%d, %d) of %d",
-                  k_begin, k_end, n_groups);
-    gsb::Workspace w = gsb::carve(d_workspace, d, c);
-    size_t off = w.bytes;
-    if (gsb::lanczos_applicable(d, c)) off += gsb::carve_lanczos(nullptr, d, c).bytes;
-    gsb::SubspaceWs sw = gsb::carve_subspace(reinterpret_cast<char *>(d_workspace) + off, d, c);
-    if (workspace_bytes < off + sw.bytes) {
-        gsb::set_error("ipca_chain_run: workspace too small (%zu < %zu)", workspace_bytes, off + sw.bytes);
-        return GSB_ERR_WORKSPACE;
-    }
-    gsb::StateView s = gsb::state_view(d_state, d, c);
-    return gsb::subspace_run_persistent(s.hdr, s.mean, s.unnorm, s.H, s.Qbuf, sw, d, c, (double)n_batch, d_queue, n_groups, k_begin,
-                                        k_end, (cudaStream_t)stream);
 }
 
 extern "C" int gsb_ipca_export(const void *d_state, int d, int c, int64_t n_seen, double *d_components,

@@ -14,7 +14,6 @@ Workspace carve(void *base, int d, int c);
 // top-c eigenpairs (descending) of the symmetric matrix held in w.A (destroyed); evecs rows are sign-normalised
 int eig_top(const Workspace &w, int d, int c, double *evals, double *evecs, cudaStream_t st);
 
-int launch_cluster_orth(const double *lam, const double *dg, const double *e, int n, int c, double *Z, cudaStream_t st);
 // svd_flip sign rule on the rows of V[c,d]
 int sign_rows(double *V, int c, int d, cudaStream_t st);
 // sticky device-side status word of the chain kernels (bit1: a subspace step hit its iteration cap)
@@ -33,26 +32,8 @@ size_t subspace_smem_bytes(int d, int c);
 SubspaceWs carve_subspace(void *base, int d, int c);
 int subspace_step(double *hdr, double *mean, double *unnorm, double *H, double *Qbuf, const double *mean_b, const double *gram_b,
                   const SubspaceWs &w, int d, int c, double n_seen, double n_b, cudaStream_t st);
-// persistent form: the cluster stays resident for steps k_begin .. k_end-1 and takes (mean, Gram) pointers from a queue
-size_t chain_queue_bytes(int n_groups);
-int chain_queue_reset(void *queue, int n_groups, cudaStream_t st);
-int chain_queue_publish(void *queue, int k0, int count, const double *mean_base, const double *gram_base, int d, int round_first,
-                        int world, int per_rank, int flag, cudaStream_t st);
-int subspace_run_persistent(double *hdr, double *mean, double *unnorm, double *H, double *Qbuf, const SubspaceWs &w, int d, int c,
-                            double n_b, void *queue, int n_groups, int k_begin, int k_end, cudaStream_t st);
 int to_subspace_form(double *hdr, const double *S, const double *V, double *H, double *Qbuf, int d, int c, cudaStream_t st);
 int materialise_components(double *hdr, double *S, double *V, const double *H, const double *Qbuf, void *eig_ws, int d, int c,
                            cudaStream_t st);
-
-struct LanczosWs {
-    double *QbT, *RT, *T, *C, *Linv, *WT, *H, *U, *lamH;
-    void *eig_ws;
-    size_t bytes;
-};
-LanczosWs carve_lanczos(void *base, int d, int c);
-bool lanczos_applicable(int d, int c);
-// top-c eigenpairs of G[d,d] from the block Krylov space of the rows of Vprev[c,d]
-int eig_top_lanczos(const LanczosWs &lw, const double *G, const double *Vprev, int d, int c, double *evals, double *evecs,
-                    cudaStream_t st);
 
 }  // namespace gsb

@@ -42,9 +42,8 @@ struct SubspaceParams {
     double *Gt, *Part, *Red, *Slots;             // workspace: G tiles, per-CTA partial (H~, W), reduced (H~, W), scalars
     double *Prof;                                // [16] clocks per phase, accumulated by CTA 0 (profiling aid)
     int d, c;
-    double n_seen, n_b, tol;                     // n_seen < 0: read it from hdr[0] (persistent kernel)
+    double n_seen, n_b, tol;
     double dbl;                                  // residual > dbl * tol: two multiplications by G per orthonormalisation
-    int chol_blocked;                            // 1: panel-of-8 Cholesky (GANSPACE_B200_SUBSPACE_CHOL=blocked|columns)
     int maxit;
     int *status;
 };
@@ -119,80 +118,8 @@ __device__ __forceinline__ Grouping make_grouping(int mt, int nt) {
 
 
 // Cholesky of W[c,c] with the RPC rows of Y riding along (Y <- Y L^-T), all in REGISTERS: the (c + RPC) x c array is
-// spread over a 16 x 16 thread grid, thread (ry, cx) holds rows ry + 16 a (a < RA) and columns cx + 16 b (b < CB).
-// Per column ONE barrier: the owners of column j+1 publish its raw entries (pivot included) as soon as step j has updated
-// them, every thread scales what it needs by rsqrt(pivot) itself.  Only the Y rows are written back (L is not needed).
-template <int RA, int CB>
-__device__ __forceinline__ void chol_solve_regs(const double *__restrict__ Ws, double *__restrict__ Ys, int c, int cp, int RPC,
-                                                double *__restrict__ colbuf /* [2][16 * RA] */) {
-    const int tid = threadIdx.x, ry = tid >> 4, cx = tid & 15;
-    const int nrows = c + RPC, CL = 16 * RA;
-    double A[RA][CB];
-#pragma unroll
-    for (int a = 0; a < RA; ++a) {
-        const int r = ry + 16 * a;
-#pragma unroll
-        for (int b = 0; b < CB; ++b) {
-            const int q = cx + 16 * b;
-            double v = 0.0;
-            if (r < nrows && q < c) v = (r < c) ? Ws[(size_t)r * cp + q] : Ys[(size_t)(r - c) * cp + q];
-            A[a][b] = v;
-        }
-    }
-    // pivots below 1e-26 x the first (= largest-scale) diagonal entry are clamped: numerically dependent columns
-    const double floor_ = fmax(fabs(Ws[0]) * 1e-26, 1e-300);
-    __syncthreads();
-    if (cx == 0) {                                            // column 0, raw
-#pragma unroll
-        for (int a = 0; a < RA; ++a) colbuf[ry + 16 * a] = A[a][0];
-    }
-    __syncthreads();
-    for (int j = 0; j < c; ++j) {
-        const double *cb = colbuf + (size_t)(j & 1) * CL;
-        double piv = cb[j];
-        if (!(piv > floor_)) piv = floor_;
-        const double inv = fast_rsqrt(piv);
-        double xr[RA], lq[CB];
-#pragma unroll
-        for (int a = 0; a < RA; ++a) xr[a] = cb[ry + 16 * a] * inv;          // scaled column j by own rows
-#pragma unroll
-        for (int b = 0; b < CB; ++b) { const int q = cx + 16 * b; lq[b] = (q < c) ? cb[q] * inv : 0.0; }   // L[q][j] by own columns
-        const int jb = j >> 4;
-        if (cx == (j & 15)) {                                 // the owners keep the final (scaled) column j
-#pragma unroll
-            for (int b = 0; b < CB; ++b) if (b == jb) {
-#pragma unroll
-                for (int a = 0; a < RA; ++a) A[a][b] = xr[a];
-            }
-        }
-        double *nb_ = colbuf + (size_t)((j + 1) & 1) * CL;
-        const int j1 = j + 1, j1b = j1 >> 4;
-#pragma unroll
-        for (int b = 0; b < CB; ++b) {
-            const int q = cx + 16 * b;
-            if (q > j) {
-#pragma unroll
-                for (int a = 0; a < RA; ++a) A[a][b] = fma(-xr[a], lq[b], A[a][b]);
-            }
-            if (b == j1b && cx == (j1 & 15) && j1 < c) {      // column j+1 is final up to its own scaling: publish it
-#pragma unroll
-                for (int a = 0; a < RA; ++a) nb_[ry + 16 * a] = A[a][b];
-            }
-        }
-        __syncthreads();
-    }
-#pragma unroll
-    for (int a = 0; a < RA; ++a) {
-        const int r = ry + 16 * a;
-        if (r >= c && r < nrows) {
-#pragma unroll
-            for (int b = 0; b < CB; ++b) { const int q = cx + 16 * b; if (q < c) Ys[(size_t)(r - c) * cp + q] = A[a][b]; }
-        }
-    }
-    __syncthreads();
-}
-
-// Blocked form of the above (panels of 8 columns): the per-column barrier + rsqrt + broadcast of the unblocked loop cost 0.59 us per
+// spread over a 16 x 16 thread grid, thread (ry, cx) holds rows ry + 16 a (a < RA) and columns cx + 16 b (b < CB).  Only the Y
+// rows are written back (L is not needed).  Panels of 8 columns: a per-column barrier + rsqrt + broadcast costs 0.59 us per
 // column (47 us for c = 80) although the arithmetic is 0.07 us.  Per panel: (1) the owners publish the panel's 8 columns; (2) warp 0
 // factors the 8 x 8 diagonal block with shuffles (lane l owns row l), then one thread per remaining row solves X = P L^-T (the Y
 // rows of the panel are final here and go straight to Ys); (3) every thread applies the rank-8 update to its registers.
@@ -215,6 +142,7 @@ __device__ __forceinline__ void chol_solve_blocked(const double *__restrict__ Ws
             A[a][b] = v;
         }
     }
+    // pivots below 1e-26 x the first (= largest-scale) diagonal entry are clamped: numerically dependent columns
     const double floor_ = fmax(fabs(Ws[0]) * 1e-26, 1e-300);
     __syncthreads();
     for (int p = 0; p < c / 8; ++p) {
@@ -302,11 +230,11 @@ __device__ __forceinline__ void chol_solve_blocked(const double *__restrict__ Ws
     __syncthreads();
 }
 
-// One chain step by the whole cluster (every thread of every CTA calls it with the same p).  All data written by one CTA and
-// read by another travels through L2 (.cg loads / cp.async.cg) or after a cluster barrier, so the function can be called
-// repeatedly from a persistent kernel.
+// One chain step by the whole cluster.  All data written by one CTA and read by another travels through L2 (.cg loads /
+// cp.async.cg) or after a cluster barrier.
 template <int RA, int CB>
-__device__ __forceinline__ void subspace_step_body(const SubspaceParams &p) {
+__global__ void __launch_bounds__(SC_THREADS, 1)
+subspace_step_kernel(const SubspaceParams p) {
     extern __shared__ __align__(16) double sc_smem[];
     const int d = p.d, c = p.c, cp = c + 4, RPC = d / SC_CL, RT = RPC / 8, CT = c / 8, nkt = d / SC_KT;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, fg = lane >> 2, ft = lane & 3;
@@ -321,12 +249,12 @@ __device__ __forceinline__ void subspace_step_body(const SubspaceParams &p) {
     double *Ws = Qq + (size_t)RPC * cp;                     // [c][cp]     H, then W -> L
     double *mv = Ws + (size_t)c * cp;                       // [d]         mean-correction vector m
     double *red = mv + d;                                   // [64]
-    double *colbuf = red + 64;                              // [2][16 * RA]
+    double *cholbuf = red + 64;                             // [2 * 16 * RA * 9 + 80]  Cholesky panels
     long long tprev = clock64();
     double prof[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 #define PROF(k) do { const long long tn_ = clock64(); prof[k] += (double)(tn_ - tprev); tprev = tn_; } while (0)
 
-    const double n_seen = (p.n_seen >= 0.0) ? p.n_seen : __ldcg(p.hdr), n_b = p.n_b, n_tot = n_seen + n_b;   // persistent: from the state
+    const double n_seen = p.n_seen, n_b = p.n_b, n_tot = n_seen + n_b;
     int cur = (int)__ldcg(p.hdr + 3);
     double *Qc = p.Qbuf + (size_t)cur * d * cp, *Qn = p.Qbuf + (size_t)(cur ^ 1) * d * cp;
     const size_t tileA = (size_t)RPC * SC_LDA, tileB = (size_t)SC_KT * cp;
@@ -578,8 +506,7 @@ __device__ __forceinline__ void subspace_step_body(const SubspaceParams &p) {
         // ---- W = L L^T in shared memory; the rows of Y_q (Z_q) ride along:  Q_q <- Y_q L^-T
         for (int i = tid; i < c * c; i += SC_THREADS) Ws[(i / c) * cp + i % c] = __ldcg(p.Red + (size_t)c * c + i);
         __syncthreads();
-        if (p.chol_blocked) chol_solve_blocked<RA, CB>(Ws, Ys, c, cp, RPC, colbuf);
-        else chol_solve_regs<RA, CB>(Ws, Ys, c, cp, RPC, colbuf);
+        chol_solve_blocked<RA, CB>(Ws, Ys, c, cp, RPC, cholbuf);
         PROF(6);
         // ---- publish the new rows of Q
         {
@@ -632,73 +559,6 @@ __device__ __forceinline__ void subspace_step_body(const SubspaceParams &p) {
     sc_cluster_sync();
 }
 #undef PROF
-
-template <int RA, int CB>
-__global__ void __launch_bounds__(SC_THREADS, 1)
-subspace_step_kernel(const SubspaceParams p) {
-    subspace_step_body<RA, CB>(p);
-}
-
-// ---- persistent form: the cluster stays resident and takes the groups' statistics from a queue ---------------------------------
-// A step per launch needs 16 free SMs of one GPC at every launch; next to the producers' long-running CTAs (RNG sub-streams,
-// persistent GEMM CTAs) each launch waited up to a millisecond.  The persistent kernel occupies its 16 SMs once, for steps
-// k_begin .. k_end-1, and waits for entry k of the queue (pointers to the group's mean / centred Gram, then a flag) which a
-// one-warp kernel on the producers' stream publishes behind the statistics kernels.
-struct ChainQueueEntry {
-    const double *mean, *gram;
-    int flag;                // 0 = not published, 1 = ready, 2 = stop before this step
-    int pad;
-};
-
-__global__ void chain_publish_kernel(ChainQueueEntry *q, int k0, int count, const double *mean_base, const double *gram_base, int d,
-                                     int round_first, int world, int per_rank, int flag) {
-    const int i = threadIdx.x + blockIdx.x * blockDim.x;
-    if (i >= count) return;
-    const int k = k0 + i;
-    // slot of group k inside the buffers: linear (world = 1), or the all-gather layout of a round (plan.rounds):
-    // rank (k mod world) contributed its (k - round_first) / world -th group
-    const size_t slot = (world <= 1) ? (size_t)i : (size_t)(k % world) * per_rank + (size_t)(k - round_first) / world;
-    q[k].mean = mean_base ? mean_base + slot * d : nullptr;
-    q[k].gram = gram_base ? gram_base + slot * (size_t)d * d : nullptr;
-    __threadfence();
-    *reinterpret_cast<volatile int *>(&q[k].flag) = flag;
-}
-
-template <int RA, int CB>
-__global__ void __launch_bounds__(SC_THREADS, 1)
-subspace_persistent_kernel(SubspaceParams p, ChainQueueEntry *queue, int *decision, int k_begin, int k_end, double timeout_ns) {
-    __shared__ int s_dec;
-    uint32_t me;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(me));
-    for (int k = k_begin; k < k_end; ++k) {
-        if (me == 0 && threadIdx.x == 0) {
-            // CTA 0 alone polls (the others sleep in the cluster barrier) and decides for the whole cluster
-            unsigned long long t0, t1;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-            int f;
-            unsigned ns = 64;
-            for (;;) {
-                f = *reinterpret_cast<volatile int *>(&queue[k].flag);
-                if (f != 0) break;
-                __nanosleep(ns);
-                if (ns < 2048) ns *= 2;
-                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-                if ((double)(t1 - t0) > timeout_ns) { f = 3; break; }          // producer never came: give up, flag the run
-            }
-            __threadfence();
-            *reinterpret_cast<volatile int *>(decision) = f;
-            if (f == 3) atomicOr(p.status, 8);
-        }
-        __syncthreads();
-        sc_cluster_sync();
-        if (threadIdx.x == 0) s_dec = *reinterpret_cast<volatile int *>(decision);
-        __syncthreads();
-        if (s_dec != 1) break;
-        p.mean_b = *reinterpret_cast<const double *volatile *>(&queue[k].mean);
-        p.gram_b = *reinterpret_cast<const double *volatile *>(&queue[k].gram);
-        subspace_step_body<RA, CB>(p);
-    }
-}
 
 // (V, S) of the direct first step -> (Q, H):  Q[i][t] = V[t][i], H = diag(S^2)
 __global__ void to_subspace_kernel(double *hdr, const double *__restrict__ S, const double *__restrict__ V, double *__restrict__ H,
@@ -782,7 +642,7 @@ bool subspace_applicable(int d, int c) {
     static int mode = -1;
     if (mode == -1) {
         const char *env = getenv("GANSPACE_B200_CHAIN");
-        mode = (env && (strcmp(env, "direct") == 0 || strcmp(env, "lanczos") == 0)) ? 0 : 1;
+        mode = (env && strcmp(env, "direct") == 0) ? 0 : 1;
     }
     return mode == 1 && d % 128 == 0 && d >= 128 && d <= 512 && c % 8 == 0 && c >= 8 && c <= 128 && 2 * c <= d + d / 4 &&
            subspace_smem_bytes(d, c) <= 227 * 1024;
@@ -811,15 +671,6 @@ SubspaceWs carve_subspace(void *base, int d, int c) {
 // residual / tolerance ratio above which an iteration multiplies by G twice before orthonormalising (GANSPACE_B200_SUBSPACE_DBL;
 // 0 = never).  One multiplication gains a factor lambda_{c+1}/lambda_c ~ 1/k at step k, so "more than 10x away" means at least
 // two more iterations early in a run and costs at most one spare GEMM late in it.
-static int chol_blocked_default() {
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("GANSPACE_B200_SUBSPACE_CHOL");
-        v = (e && strcmp(e, "columns") == 0) ? 0 : 1;          // measured: Cholesky phase 47 -> 17 us per iteration, same digits
-    }
-    return v;
-}
-
 static double double_step_factor() {
     static double f = -1.0;
     if (f < 0.0) {
@@ -860,7 +711,7 @@ int subspace_step(double *hdr, double *mean, double *unnorm, double *H, double *
     p.hdr = hdr; p.mean = mean; p.unnorm = unnorm; p.H = H; p.Qbuf = Qbuf;
     p.mean_b = mean_b; p.gram_b = gram_b;
     p.Gt = w.Gt; p.Part = w.Part; p.Red = w.Red; p.Slots = w.Slots; p.Prof = hdr + 8;
-    p.d = d; p.c = c; p.n_seen = n_seen; p.n_b = n_b; p.tol = tol; p.maxit = maxit; p.dbl = double_step_factor(); p.chol_blocked = chol_blocked_default();
+    p.d = d; p.c = c; p.n_seen = n_seen; p.n_b = n_b; p.tol = tol; p.maxit = maxit; p.dbl = double_step_factor();
     p.status = eig_status_device_ptr();
     GSB_CHECK_ARG(p.status, "subspace_step: no device status word");
     cudaLaunchConfig_t cfg{};
@@ -870,70 +721,6 @@ int subspace_step(double *hdr, double *mean, double *unnorm, double *H, double *
     at[0].val.clusterDim.x = SC_CL; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
     GSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, p));
-    return GSB_OK;
-}
-
-// ---- persistent chain: host side -------------------------------------------------------------------------------------------
-size_t chain_queue_bytes(int n_groups) { return align_up((size_t)n_groups * sizeof(ChainQueueEntry), 256) + 256; }
-
-int chain_queue_reset(void *queue, int n_groups, cudaStream_t st) {
-    GSB_CHECK_CUDA(cudaMemsetAsync(queue, 0, chain_queue_bytes(n_groups), st));
-    // an empty publish: with lazy module loading the kernel's first launch would otherwise block until the resident kernel exits
-    chain_publish_kernel<<<1, 32, 0, st>>>(reinterpret_cast<ChainQueueEntry *>(queue), 0, 0, nullptr, nullptr, 0, 0, 1, 1, 0);
-    GSB_CHECK_LAUNCH();
-    return GSB_OK;
-}
-
-int chain_queue_publish(void *queue, int k0, int count, const double *mean_base, const double *gram_base, int d, int round_first,
-                        int world, int per_rank, int flag, cudaStream_t st) {
-    chain_publish_kernel<<<(count + 31) / 32, 32, 0, st>>>(reinterpret_cast<ChainQueueEntry *>(queue), k0, count, mean_base, gram_base,
-                                                         d, round_first, world, per_rank, flag);
-    GSB_CHECK_LAUNCH();
-    return GSB_OK;
-}
-
-int subspace_run_persistent(double *hdr, double *mean, double *unnorm, double *H, double *Qbuf, const SubspaceWs &w, int d, int c,
-                            double n_b, void *queue, int n_groups, int k_begin, int k_end, cudaStream_t st) {
-    double tol;
-    int maxit;
-    {
-        const char *e1 = getenv("GANSPACE_B200_SUBSPACE_TOL"), *e2 = getenv("GANSPACE_B200_SUBSPACE_MAXIT");
-        tol = e1 ? atof(e1) : 1e-4;
-        if (!(tol > 0.0)) tol = 1e-4;
-        maxit = e2 ? atoi(e2) : 60;
-        if (maxit < 1) maxit = 60;
-    }
-    const char *et = getenv("GANSPACE_B200_CHAIN_TIMEOUT_S");
-    const double timeout_ns = 1e9 * (et ? atof(et) : 10.0);
-    const size_t smem = subspace_smem_bytes(d, c);
-    const bool small = (c <= 80 && c + d / SC_CL <= 112);
-    auto kern = small ? subspace_persistent_kernel<7, 5> : subspace_persistent_kernel<10, 8>;
-    static size_t smem_set[2] = {0, 0};
-    static bool cluster_set[2] = {false, false};
-    if (!cluster_set[small]) {
-        GSB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-        cluster_set[small] = true;
-    }
-    if (smem > smem_set[small]) {
-        GSB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        smem_set[small] = smem;
-    }
-    SubspaceParams p;
-    p.hdr = hdr; p.mean = mean; p.unnorm = unnorm; p.H = H; p.Qbuf = Qbuf;
-    p.mean_b = nullptr; p.gram_b = nullptr;
-    p.Gt = w.Gt; p.Part = w.Part; p.Red = w.Red; p.Slots = w.Slots; p.Prof = hdr + 8;
-    p.d = d; p.c = c; p.n_seen = -1.0; p.n_b = n_b; p.tol = tol; p.maxit = maxit; p.dbl = double_step_factor(); p.chol_blocked = chol_blocked_default();
-    p.status = eig_status_device_ptr();
-    GSB_CHECK_ARG(p.status, "subspace_run_persistent: no device status word");
-    ChainQueueEntry *q = reinterpret_cast<ChainQueueEntry *>(queue);
-    int *decision = reinterpret_cast<int *>(reinterpret_cast<char *>(queue) + align_up((size_t)n_groups * sizeof(ChainQueueEntry), 256));
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(SC_CL); cfg.blockDim = dim3(SC_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = SC_CL; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    GSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, p, q, decision, k_begin, k_end, timeout_ns));
     return GSB_OK;
 }
 

@@ -347,8 +347,6 @@ def compute_arrays(config, instrumented_model, state=None):
     k = 0
     stop = False                 # fit_partial returned False (e.g. n_components > first batch): the reference leaves the loop (:262-263)
     exchange = _StatsExchange(d, world) if (live and not large_d) else None
-    if not large_d and hasattr(tr, "begin_run"):
-        tr.begin_run(K, NB, d, device)           # groups 1 .. K-1 merge inside one resident chain kernel (csrc/subspace.cu)
 
     def group_rows(rows):
         """[n, d] activations of the hooked layer for latent rows ``rows`` (small-d engine; n is a multiple of NB)."""
@@ -462,10 +460,6 @@ def compute_arrays(config, instrumented_model, state=None):
             raise
         # the reference's `gi` of the interrupted group (:268-272) = the samples merged so far
         state["canceled_at"] = int(tr.n_samples_seen_)
-
-    finally:
-        if hasattr(tr, "end_run"):
-            tr.end_run()                                # a resident chain kernel never waits for groups that will not come
     tick("sampling + activations + IPCA chain")
     # host work that does not depend on the chain's result, done while the device still runs the last merge steps (the
     # export below is the first call that waits for them): get_random_dirs' host stream + upload, the lat_stdev latents

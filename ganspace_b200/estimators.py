@@ -115,30 +115,13 @@ class DeviceIncrementalPCA:
         mean, gram = _native.batch_stats(X)
         return int(X.shape[0]), mean, gram
 
-    def begin_run(self, n_groups, n_batch, d, device):
-        """Small-d engine: announce a run of ``n_groups`` partial_fit calls of ``n_batch`` rows each.  From the second group on
-        the merge chain then runs in ONE resident cluster kernel that takes the groups' statistics from a device queue
-        (csrc/subspace.cu) instead of one launch per group."""
-        if d > self.SMALL_D_MAX or self._chain is not None or self.n_components > min(d, n_batch):
-            return False
-        chain = self._ensure(int(d), device)
-        return chain.begin_run(int(n_groups), int(n_batch)) if hasattr(chain, "begin_run") else False
-
-    def end_run(self):
-        if self._chain is not None and hasattr(self._chain, "end_run"):
-            self._chain.end_run()
-
     def merge(self, n_batch, mean_b, gram_b):
         """One partial_fit step from precomputed batch statistics (must follow the reference's batch order)."""
         chain = self._ensure(int(mean_b.shape[0]), mean_b.device)
         if int(self.n_samples_seen_) == 0 and self.n_components > n_batch:
             raise ValueError(f"n_components={self.n_components} must be less or equal to the batch number of "
                              f"samples {n_batch} for the first partial_fit call.")
-        run = getattr(chain, "_run", None)
-        if run is not None and not run["closed"]:
-            chain.run_step(n_batch, mean_b, gram_b)
-        else:
-            chain.step(n_batch, mean_b, gram_b)
+        chain.step(n_batch, mean_b, gram_b)
         self.n_samples_seen_ = np.int64(chain.n_seen)
         self._host = None
 

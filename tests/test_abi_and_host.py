@@ -20,7 +20,7 @@ def test_library_exports_every_declared_symbol():
     lib = ctypes.CDLL(str(_native.lib_path()))
     for name in declared:
         assert hasattr(lib, name), name
-    assert _native.load().gsb_abi_version() == 1
+    assert _native.load().gsb_abi_version() == 2
 
 
 def test_ctypes_signatures_match_header_prototypes():

@@ -222,39 +222,6 @@ def test_ipca_chain_vs_oracle_gram_d512(nat, oracle, mapping_weights):
     assert np.max(np.abs(out["explained_variance_ratio"] - st.explained_variance_ratio)) < 1e-6
 
 
-def test_persistent_chain_equals_step_launches(nat, oracle, mapping_weights, monkeypatch):
-    """The resident chain kernel (one launch for steps 1..K-1, statistics handed over through the device queue) performs the
-    same arithmetic as one launch per step; an early end_run() stops it after the published groups."""
-    ws, bs = mapping_weights
-    stats = []
-    for k in range(6):
-        z = oracle.standard_normal_f32(2000 + k, 512 * 2500).reshape(2500, 512)
-        stats.append(nat.batch_stats(torch.tensor(oracle.mapping_forward(z, ws, bs)).cuda()))
-    ref = nat.IPCAChain(512, 80, "cuda")
-    for m, G in stats:
-        ref.step(2500, m, G)
-    ref_out = {k: v.cpu().numpy() for k, v in ref.export().items()}
-    monkeypatch.setenv("GANSPACE_B200_CHAIN_PERSISTENT", "1")          # opt-in feature
-    run = nat.IPCAChain(512, 80, "cuda")
-    assert run.begin_run(6, 2500)
-    for m, G in stats:
-        run.run_step(2500, m, G)
-    out = {k: v.cpu().numpy() for k, v in run.export().items()}
-    for k in ref_out:
-        assert np.array_equal(out[k], ref_out[k]), k
-    # early stop: 4 of 6 groups published, then end_run
-    part = nat.IPCAChain(512, 80, "cuda")
-    assert part.begin_run(6, 2500)
-    for m, G in stats[:4]:
-        part.run_step(2500, m, G)
-    part.end_run()
-    ref4 = nat.IPCAChain(512, 80, "cuda")
-    for m, G in stats[:4]:
-        ref4.step(2500, m, G)
-    a, b = part.export(), ref4.export()
-    assert part.n_seen == 10000 and torch.equal(a["components"], b["components"]) and torch.equal(a["mean"], b["mean"])
-
-
 def test_project_std(nat):
     rng = np.random.RandomState(5)
     X = rng.standard_normal((5000, 512)).astype(np.float32) * 2 + 1

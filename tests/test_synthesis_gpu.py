@@ -150,7 +150,7 @@ def test_gram_tc_matches_fp64(monkeypatch):
 @pytest.mark.parametrize("d,nb,c,k", [(4096, 300, 12, 4), (2048, 1100, 16, 3)])
 def test_large_d_chain_vs_sklearn_form(oracle, monkeypatch, d, nb, c, k, gram):
     """IPCAEstimator with d > 1024 (small-side engine) against the oracle's restatement of IncrementalPCA.partial_fit.
-    (2048, 1100, 16): small side 1117 -> 1120 > 1024 exercises the L2 eigensolver on step 0 and the Lanczos steps after."""
+    (2048, 1100, 16): small side 1117 -> 1120 > 1024 exercises the L2 eigensolver on every step."""
     from ganspace_b200.estimators import get_estimator
     monkeypatch.setenv("GANSPACE_B200_BIGD_GRAM", gram)
     Xs = _synthetic_batches(d, nb, k, seed=d + nb)
