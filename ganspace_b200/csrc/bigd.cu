@@ -16,14 +16,10 @@
 // followed by sklearn's svd_flip sign rule on the rows and the Chan mean / variance merge per feature
 // (extmath._incremental_mean_and_var).  Nothing of size d x d or n_b x d ever leaves the device.
 #include "ipca_internal.cuh"
+#include "tc_common.cuh"
 #include <math.h>
 
 namespace gsb {
-
-// tensor-core small-side Gram (gram_tc.cu)
-size_t gram_tc_workspace_bytes(int n_pad, int64_t d);
-bool gram_tc_supported(int64_t d);
-int gram_tc(const float *M, int n_rows, int n_pad, int64_t d, void *ws, double *T, cudaStream_t st);
 
 constexpr int BD_HDR = 4;
 constexpr int BD_KCHUNK = 8192;

@@ -1,24 +1,31 @@
-// Small-side Gram  T = M M^T  of the large-d IPCA engine on the Hopper tensor cores (wgmma + TMA), with a PROMOTED
-// accumulator.
+// Gram matrices on the Hopper tensor cores (wgmma + TMA) with a PROMOTED accumulator: the centred per-group Grams of the
+// batch statistics (stats_tc.cu) and the small-side Gram  T = M M^T  of the large-d IPCA engine.
 //
 // Part of the replacement of sklearn IncrementalPCA.partial_fit (_incremental_pca.py:254-380) for conv feature maps
 // (bigd.cu): M is sklearn's stacked matrix [S*Vt; X - mean_b; correction] ([n_s <= 4096, d ~ 5e5] fp32 in HBM).
 //
 // Precision.  As in mapping_tc.cu every fp32 operand is split x 2^e = hi + lo into two fp16 numbers (22 significant
-// bits; e = a per-row power-of-two exponent that puts the row maximum into [8192, 16384)), and a product is three MMAs
-// (hi hi, lo hi, hi lo) accumulated in fp32.  Tensor-core accumulation TRUNCATES when aligning addends, which is harmless
-// over K = 512 but not over K = 524288.  So the MMAs accumulate only FLUSH_KB * 64 = 256 values of K (48 MMA steps) into
-// the wgmma accumulator; that partial is then added into a second set of fp32 REGISTERS with round-to-nearest, and after
-// a chunk of 4096 columns the sums are scaled by 2^-(e_i + e_j) and added into the fp64 matrix T (RED.ADD.F64), mirrored
-// across the diagonal.  Error budget per entry: <= 48 x 2^-24 truncation inside a flush, round-to-nearest fp32 across the
-// 16 flushes of a chunk, fp64 across chunks.
+// bits; e = a power-of-two exponent per row of M, or per group of centred samples, chosen so that hi keeps 11 bits and
+// lo stays a normal fp16), and a product is three MMAs (hi hi, lo hi, hi lo) accumulated in fp32.  Tensor-core accumulation
+// TRUNCATES when aligning addends, which is harmless over K = 512 but not over K = 524288.  So the MMAs accumulate only
+// FLUSH_KB * 64 = 256 values of K (48 MMA steps) into the wgmma accumulator; that partial is then added into a second set
+// of fp32 REGISTERS with round-to-nearest.  At the end of a work item the sums are scaled back by the exact power of two
+// and written in fp64, mirrored across the diagonal:
+//     Store       (batch statistics) one work item covers a whole group: plain stores of each group's Gram
+//     Accumulate  (large-d) one work item covers a chunk of 4096 columns: RED.ADD.F64 into T.  Error budget per entry:
+//                 <= 48 x 2^-24 truncation inside a flush, round-to-nearest fp32 across the 16 flushes of a chunk, fp64
+//                 across chunks.
 //
 // Kernel: persistent, one CTA per SM, 128 x 128 x 64 tiles (upper tile pairs only), 3 smem stages x 64 KB (A_hi, A_lo,
-// B_hi, B_lo; both operands are row blocks of the same two fp16 matrices), SWIZZLE_128B K-major:
+// B_hi, B_lo; both operands are row blocks of the same two fp16 matrices; diagonal tiles load B too: reading B from A's slot
+// instead made the kernel 3 % slower for the large-d Gram and 10 % slower for the d = 512 statistics on an H100 80GB HBM3 at
+// 700 W), SWIZZLE_128B K-major, 3-D TMA boxes {64 columns of K, 128 rows, 1 group}; columns past K are zero-filled by the
+// TMA unit:
 //     warp 8     TMA producer
-//     warps 0-7  two warpgroups of 64 output rows each: wgmma m64n128k16, promotion, fp64 reduction into T
-// Work items are (chunk of d, tile pair) in chunk-major order, so the CTAs running at the same time read the same
-// 2112 x 4096 slab of M (35 MB as hi+lo) out of the 50 MB L2.
+//     warps 0-7  two warpgroups of 64 output rows each: wgmma m64n128k16, promotion, epilogue
+// Work items are (group, chunk of K, tile pair) with the tile pair fastest and then the chunk: group-major for the
+// statistics, chunk-major for the large-d Gram, so the CTAs running at the same time read the same 2112 x 4096 slab of M
+// (35 MB as hi+lo) out of the 50 MB L2.
 #include "tc_common.cuh"
 #include <math.h>
 
@@ -28,26 +35,36 @@ namespace gtc {
 constexpr int BM = 128, BN = 128, BK = 64;
 constexpr int STAGES = 3;
 constexpr int FLUSH_KB = 4;                 // K-blocks (of 64) accumulated by the MMAs before the promotion into registers
-constexpr int CHUNK_KB = 64;                // K-blocks per work item (4096 columns of d)
+constexpr int CHUNK_KB = 64;                // K-blocks per work item of the Accumulate epilogue (4096 columns of d)
 constexpr uint32_t TILE_BYTES = BM * BK * 2;               // 16 KB
 constexpr uint32_t STAGE_BYTES = 4 * TILE_BYTES;           // 64 KB
 constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
 
 struct Params {
-    double *T;
-    const int *rexp;        // [n_pad] per-row scale exponents of the split operands
-    int ldt, n_rows;
-    int npairs, nt;         // upper tile pairs of the nt x nt grid of 128-row blocks
-    int total_kb;           // d / 64
-    int nchunks;
+    double *out;            // Store: [n_groups][ld][ld];  Accumulate: [ld][ld], summed into
+    const int *exps;        // scale exponents of the split operands: Store: [n_groups];  Accumulate: [ld], one per row
+    int ld, n_rows;         // output leading dimension; rows (and columns) of the Gram
+    int nt, npairs;         // upper tile pairs of the nt x nt grid of 128-row blocks
+    int n_groups, n_chunks;
+    int total_kb, chunk_kb; // K-blocks per group, per work item
 };
 
-__device__ __forceinline__ void decode_pair(int pair, int nt, int &ti, int &tj) {
-    ti = 0;
-    while (pair >= nt - ti) { pair -= nt - ti; ++ti; }
-    tj = ti + pair;
+struct Item { int g, m0, n0, kb0, kb1; };
+
+__device__ __forceinline__ Item decode_item(int item, const Params &p) {
+    const int outer = item / p.npairs;
+    int pair = item % p.npairs, ti = 0;
+    while (pair >= p.nt - ti) { pair -= p.nt - ti; ++ti; }
+    Item w;
+    w.g = outer / p.n_chunks;
+    w.kb0 = (outer % p.n_chunks) * p.chunk_kb;
+    w.kb1 = (w.kb0 + p.chunk_kb < p.total_kb) ? w.kb0 + p.chunk_kb : p.total_kb;
+    w.m0 = ti * BM;
+    w.n0 = (ti + pair) * BN;
+    return w;
 }
 
+template <GramEpilogue EPI>
 __global__ void __launch_bounds__(tc::THREADS, 1)
 gram_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, const Params p) {
     using namespace tc;
@@ -58,7 +75,7 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
     uint64_t *empty_bar = bars + STAGES;           // [STAGES]: one arrival per consumer warp
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int num_items = p.nchunks * p.npairs;
+    const int num_items = p.n_groups * p.n_chunks * p.npairs;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CONSUMER_THREADS / 32); }
@@ -72,25 +89,21 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
         if (lane == 0) {
             int stage = 0; uint32_t phase = 0;
             for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-                const int chunk = item / p.npairs;
-                int ti, tj;
-                decode_pair(item % p.npairs, p.nt, ti, tj);
-                const int m0 = ti * BM, n0 = tj * BN;
-                const int kb0 = chunk * CHUNK_KB, kb1 = (kb0 + CHUNK_KB < p.total_kb) ? kb0 + CHUNK_KB : p.total_kb;
-                for (int kb = kb0; kb < kb1; ++kb) {
+                const Item w = decode_item(item, p);
+                for (int kb = w.kb0; kb < w.kb1; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1);
                     uint8_t *st = smem + stage * STAGE_BYTES;
                     mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES);
-                    tma_load_2d(&tm_hi, &full_bar[stage], st, kb * BK, m0);
-                    tma_load_2d(&tm_lo, &full_bar[stage], st + TILE_BYTES, kb * BK, m0);
-                    tma_load_2d(&tm_hi, &full_bar[stage], st + 2 * TILE_BYTES, kb * BK, n0);
-                    tma_load_2d(&tm_lo, &full_bar[stage], st + 3 * TILE_BYTES, kb * BK, n0);
+                    tma_load_3d(&tm_hi, &full_bar[stage], st, kb * BK, w.m0, w.g);
+                    tma_load_3d(&tm_lo, &full_bar[stage], st + TILE_BYTES, kb * BK, w.m0, w.g);
+                    tma_load_3d(&tm_hi, &full_bar[stage], st + 2 * TILE_BYTES, kb * BK, w.n0, w.g);
+                    tma_load_3d(&tm_lo, &full_bar[stage], st + 3 * TILE_BYTES, kb * BK, w.n0, w.g);
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
         }
     } else {
-        // ===================== MMA + promoted accumulation + reduction into T =====================
+        // ===================== MMA + promoted accumulation + epilogue =====================
         const int wg = warp >> 2;                       // 64-row half of the 128-row tile
         const int row_frag = wg * 64 + (warp & 3) * 16 + (lane >> 2), col_frag = 2 * (lane & 3);
         int stage = 0; uint32_t phase = 0;
@@ -98,21 +111,17 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
 #pragma unroll
         for (int j = 0; j < 64; ++j) { acc[j] = 0.f; r[j] = 0.f; }
         for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-            const int chunk = item / p.npairs;
-            int ti, tj;
-            decode_pair(item % p.npairs, p.nt, ti, tj);
-            const int m0 = ti * BM, n0 = tj * BN;
-            const int kb0 = chunk * CHUNK_KB, kb1 = (kb0 + CHUNK_KB < p.total_kb) ? kb0 + CHUNK_KB : p.total_kb;
-            const int nkb = kb1 - kb0;
+            const Item w = decode_item(item, p);
+            const int nkb = w.kb1 - w.kb0;
             for (int g0 = 0; g0 < nkb; g0 += FLUSH_KB) {
                 const int g1 = (g0 + FLUSH_KB < nkb) ? g0 + FLUSH_KB : nkb;
-                for (int kbl = g0; kbl < g1; ++kbl) {
+                for (int kb = g0; kb < g1; ++kb) {
                     mbar_wait(&full_bar[stage], phase);
                     const uint32_t st = smem_u32(smem + stage * STAGE_BYTES);
                     const uint32_t sa = st + (uint32_t)wg * (TILE_BYTES / 2);
                     wgmma_fence();
                     split_kblock_m64n128(acc, sw128_kmajor_desc(sa), sw128_kmajor_desc(sa + TILE_BYTES),
-                                         sw128_kmajor_desc(st + 2 * TILE_BYTES), sw128_kmajor_desc(st + 3 * TILE_BYTES), kbl > g0);
+                                         sw128_kmajor_desc(st + 2 * TILE_BYTES), sw128_kmajor_desc(st + 3 * TILE_BYTES), kb > g0);
                     wgmma_commit();
                     wgmma_wait_all();
                     if (lane == 0) mbar_arrive(&empty_bar[stage]);
@@ -121,17 +130,38 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
 #pragma unroll
                 for (int j = 0; j < 64; ++j) r[j] = __fadd_rn(r[j], acc[j]);
             }
-            const int gm0 = m0 + row_frag, gm1 = gm0 + 8;
-            const int em0 = gm0 < p.n_rows ? __ldg(&p.rexp[gm0]) : 0, em1 = gm1 < p.n_rows ? __ldg(&p.rexp[gm1]) : 0;
+            if constexpr (EPI == GramEpilogue::Store) {
+                const double unscale = ldexp(1.0, -2 * __ldg(p.exps + w.g));
+                double *G = p.out + (size_t)w.g * p.ld * p.ld;
+                const bool diag = (w.m0 == w.n0);
 #pragma unroll
-            for (int j = 0; j < 64; ++j) {
-                const int gm = ((j >> 1) & 1) ? gm1 : gm0, gn = n0 + 8 * (j >> 2) + col_frag + (j & 1);
-                if (gm < p.n_rows && gn < p.n_rows && gn >= gm) {
-                    // 2^-(e_i + e_j) as an fp64 bit pattern: exact, |e_i + e_j| stays far inside the normal range
-                    const int e = ((j >> 1) & 1 ? em1 : em0) + __ldg(&p.rexp[gn]);
-                    const double val = (double)r[j] * __hiloint2double((1023 - e) << 20, 0);
-                    atomicAdd(&p.T[(size_t)gm * p.ldt + gn], val);
-                    if (gn > gm) atomicAdd(&p.T[(size_t)gn * p.ldt + gm], val);
+                for (int j = 0; j < 64; j += 2) {
+                    const int gm = w.m0 + row_frag + 8 * ((j >> 1) & 1), gn = w.n0 + 8 * (j >> 2) + col_frag;
+                    const double v0 = (double)r[j] * unscale, v1 = (double)r[j + 1] * unscale;
+                    if (!diag) {
+                        *reinterpret_cast<double2 *>(G + (size_t)gm * p.ld + gn) = make_double2(v0, v1);
+                        G[(size_t)gn * p.ld + gm] = v0;
+                        G[(size_t)(gn + 1) * p.ld + gm] = v1;
+                    } else {
+                        // diagonal tile: (i,j) and (j,i) come out of differently ordered MMA sums; keep the upper triangle
+                        // and mirror it, so the chain reads an exactly symmetric matrix
+                        if (gn >= gm) { G[(size_t)gm * p.ld + gn] = v0; G[(size_t)gn * p.ld + gm] = v0; }
+                        if (gn + 1 >= gm) { G[(size_t)gm * p.ld + gn + 1] = v1; G[(size_t)(gn + 1) * p.ld + gm] = v1; }
+                    }
+                }
+            } else {
+                const int gm0 = w.m0 + row_frag, gm1 = gm0 + 8;
+                const int em0 = gm0 < p.n_rows ? __ldg(&p.exps[gm0]) : 0, em1 = gm1 < p.n_rows ? __ldg(&p.exps[gm1]) : 0;
+#pragma unroll
+                for (int j = 0; j < 64; ++j) {
+                    const int gm = ((j >> 1) & 1) ? gm1 : gm0, gn = w.n0 + 8 * (j >> 2) + col_frag + (j & 1);
+                    if (gm < p.n_rows && gn < p.n_rows && gn >= gm) {
+                        // 2^-(e_i + e_j) as an fp64 bit pattern: exact, |e_i + e_j| stays far inside the normal range
+                        const int e = ((j >> 1) & 1 ? em1 : em0) + __ldg(&p.exps[gn]);
+                        const double val = (double)r[j] * __hiloint2double((1023 - e) << 20, 0);
+                        atomicAdd(&p.out[(size_t)gm * p.ld + gn], val);
+                        if (gn > gm) atomicAdd(&p.out[(size_t)gn * p.ld + gm], val);
+                    }
                 }
             }
 #pragma unroll
@@ -177,29 +207,49 @@ row_split_kernel(const float *__restrict__ M, int64_t d, int n_rows, const int *
     if (r < n_rows) v = reinterpret_cast<const float4 *>(M + (size_t)r * d)[q];
     const float sc = ldexpf(1.f, rexp[r]);
     const float f[4] = {v.x * sc, v.y * sc, v.z * sc, v.w * sc};              // power-of-two scale: exact
-    __half h[4], l[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        h[k] = __float2half_rn(f[k]);
-        l[k] = __float2half_rn(f[k] - __half2float(h[k]));
-    }
     uint2 ph, pl;
-    ph.x = (uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16);
-    ph.y = (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16);
-    pl.x = (uint32_t)__half_as_ushort(l[0]) | ((uint32_t)__half_as_ushort(l[1]) << 16);
-    pl.y = (uint32_t)__half_as_ushort(l[2]) | ((uint32_t)__half_as_ushort(l[3]) << 16);
+    tc::split4(f, ph, pl);
     reinterpret_cast<uint2 *>(hi + (size_t)r * d)[q] = ph;
     reinterpret_cast<uint2 *>(lo + (size_t)r * d)[q] = pl;
 }
 
-static int make_tmap(CUtensorMap *map, const void *base, uint64_t rows, uint64_t cols) {
-    const uint64_t dims[2] = {cols, rows};
-    const uint64_t strides[1] = {cols * 2};
-    const uint32_t box[2] = {(uint32_t)BK, (uint32_t)BM};
-    return tc_make_tmap_f16(map, base, 2, dims, strides, box);
-}
-
 }  // namespace gtc
+
+int gram_tc_launch(GramEpilogue epi, const __half *hi, const __half *lo, int64_t k, int64_t k_pitch, int n_groups, int n_pad,
+                   int n_rows, const int *exps, double *out, cudaStream_t st) {
+    using namespace gtc;
+    static bool attr_set = false;
+    if (!attr_set) {
+        GSB_CHECK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<GramEpilogue::Store>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            (int)SMEM_BYTES));
+        GSB_CHECK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<GramEpilogue::Accumulate>,
+                                            cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+        attr_set = true;
+    }
+    CUtensorMap tm_hi, tm_lo;
+    const uint64_t dims[3] = {(uint64_t)k, (uint64_t)n_pad, (uint64_t)n_groups};
+    const uint64_t strides[2] = {(uint64_t)k_pitch * 2, (uint64_t)n_pad * k_pitch * 2};
+    const uint32_t box[3] = {(uint32_t)BK, (uint32_t)BM, 1};
+    if (int r = tc_make_tmap(&tm_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, hi, 3, dims, strides, box)) return r;
+    if (int r = tc_make_tmap(&tm_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, lo, 3, dims, strides, box)) return r;
+    Params p;
+    p.out = out; p.exps = exps; p.ld = n_pad; p.n_rows = n_rows;
+    p.nt = (n_rows + BM - 1) / BM;
+    p.npairs = p.nt * (p.nt + 1) / 2;
+    p.n_groups = n_groups;
+    p.total_kb = (int)((k + BK - 1) / BK);
+    // a stored Gram has to be complete in one work item; an accumulated one is split into chunks of K that share the L2
+    p.chunk_kb = (epi == GramEpilogue::Store) ? p.total_kb : CHUNK_KB;
+    p.n_chunks = (p.total_kb + p.chunk_kb - 1) / p.chunk_kb;
+    const int items = p.n_groups * p.n_chunks * p.npairs;
+    const int grid = items < num_sms() ? items : num_sms();
+    if (epi == GramEpilogue::Store)
+        gram_tc_kernel<GramEpilogue::Store><<<grid, tc::THREADS, SMEM_BYTES, st>>>(tm_hi, tm_lo, p);
+    else
+        gram_tc_kernel<GramEpilogue::Accumulate><<<grid, tc::THREADS, SMEM_BYTES, st>>>(tm_hi, tm_lo, p);
+    GSB_CHECK_LAUNCH();
+    return GSB_OK;
+}
 
 size_t gram_tc_workspace_bytes(int n_pad, int64_t d) {
     return 2 * align_up((size_t)n_pad * d * 2, 256) + align_up((size_t)n_pad * sizeof(int), 256);
@@ -214,30 +264,12 @@ int gram_tc(const float *M, int n_rows, int n_pad, int64_t d, void *ws, double *
     __half *hi = reinterpret_cast<__half *>(ws);
     __half *lo = reinterpret_cast<__half *>(reinterpret_cast<char *>(ws) + hb);
     int *rexp = reinterpret_cast<int *>(reinterpret_cast<char *>(ws) + 2 * hb);
-    static bool attr_set = false;
-    if (!attr_set) {
-        GSB_CHECK_CUDA(cudaFuncSetAttribute(gram_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-        attr_set = true;
-    }
     row_exponent_kernel<<<n_pad, 1024, 0, st>>>(M, d, n_rows, rexp);
     GSB_CHECK_LAUNCH();
     dim3 sg((unsigned)((d / 4 + 255) / 256), (unsigned)n_pad);
     row_split_kernel<<<sg, 256, 0, st>>>(M, d, n_rows, rexp, hi, lo);
     GSB_CHECK_LAUNCH();
-    CUtensorMap tm_hi, tm_lo;
-    if (int r = make_tmap(&tm_hi, hi, (uint64_t)n_pad, (uint64_t)d)) return r;
-    if (int r = make_tmap(&tm_lo, lo, (uint64_t)n_pad, (uint64_t)d)) return r;
-    Params p;
-    p.T = T; p.rexp = rexp; p.ldt = n_pad; p.n_rows = n_rows;
-    p.nt = (n_rows + BM - 1) / BM;
-    p.npairs = p.nt * (p.nt + 1) / 2;
-    p.total_kb = (int)(d / BK);
-    p.nchunks = (p.total_kb + CHUNK_KB - 1) / CHUNK_KB;
-    const int items = p.nchunks * p.npairs;
-    const int grid = items < num_sms() ? items : num_sms();
-    gram_tc_kernel<<<grid, tc::THREADS, SMEM_BYTES, st>>>(tm_hi, tm_lo, p);
-    GSB_CHECK_LAUNCH();
-    return GSB_OK;
+    return gram_tc_launch(GramEpilogue::Accumulate, hi, lo, d, d, 1, n_pad, n_rows, rexp, T, st);
 }
 
 }  // namespace gsb

@@ -10,20 +10,9 @@
 //
 // Packed layout produced by gsb_mapping_pack:  [n_layers][dim*dim] fp32 of (weight*scale) row-major
 // (out,in), followed by [n_layers][dim] fp32 of (bias*lr_mul).
-#include "common.cuh"
+#include "tc_common.cuh"
 
 namespace gsb {
-
-// tensor-core path (mapping_tc.cu)
-size_t mapping_tc_packed_bytes(int n_layers, int dim);
-int mapping_tc_pack(const float *pw, int n_layers, int dim, void *tc_base, cudaStream_t st);
-int mapping_forward_tc(const float *pb, void *tc_base, int n_layers, int dim, const float *d_z, float *d_w,
-                       int64_t n, bool pixelnorm, void *ws, int leave_free_sms, cudaStream_t st);
-size_t mapping_tc_workspace_bytes(int64_t n, int dim);
-size_t tc_linear_workspace_bytes(int64_t n, int N, int K);
-int tc_linear(const float *x, const float *w, const float *bias, float *y, int64_t n, int N, int K, bool lrelu, void *ws,
-              cudaStream_t st);
-unsigned *mapping_tc_overflow_flag(void *tc_base, int n_layers, int dim);
 
 static inline size_t simt_packed_bytes(int n_layers, int dim) {
     return align_up(((size_t)n_layers * dim * dim + (size_t)n_layers * dim) * sizeof(float), 256);

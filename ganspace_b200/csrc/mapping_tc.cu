@@ -252,19 +252,9 @@ __global__ void pixelnorm_split_kernel(const float *__restrict__ x, __half *__re
     bool ovf = false;
     for (int i = lane; i < dim / 4; i += 32) {
         float4 v = xr[i];
-        float f[4] = {v.x * r, v.y * r, v.z * r, v.w * r};
-        __half h[4], l[4];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            h[q] = __float2half_rn(f[q]);
-            l[q] = __float2half_rn(f[q] - __half2float(h[q]));
-            ovf |= fabsf(f[q]) > 60000.f;
-        }
+        const float f[4] = {v.x * r, v.y * r, v.z * r, v.w * r};
         uint2 ph, pl;
-        ph.x = (uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16);
-        ph.y = (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16);
-        pl.x = (uint32_t)__half_as_ushort(l[0]) | ((uint32_t)__half_as_ushort(l[1]) << 16);
-        pl.y = (uint32_t)__half_as_ushort(l[2]) | ((uint32_t)__half_as_ushort(l[3]) << 16);
+        ovf |= tc::split4(f, ph, pl);
         reinterpret_cast<uint2 *>(hi + row * dim)[i] = ph;
         reinterpret_cast<uint2 *>(lo + row * dim)[i] = pl;
     }
@@ -289,10 +279,7 @@ __global__ void weight_split_kernel(const float *__restrict__ pw, int64_t count,
                                     __half *__restrict__ hi, __half *__restrict__ lo) {
     const float wscale = *wscale_p;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x) {
-        float w = pw[i] * wscale;          // power-of-two scale: exact
-        __half h = __float2half_rn(w);
-        hi[i] = h;
-        lo[i] = __float2half_rn(w - __half2float(h));
+        tc::split1(pw[i] * wscale, hi[i], lo[i]);          // power-of-two scale: exact
     }
 }
 
@@ -305,28 +292,15 @@ __global__ void absmax_kernel(const float *__restrict__ x, int64_t count, float 
 }
 
 // ---- host side ------------------------------------------------------------------------------------------
-// 2-D fp16 row-major [rows, cols] tensor, box = box_rows x 64 columns, 128B swizzle (rows / cols smaller than the box are fine:
-// the TMA unit fills the rest of the box with zeros)
-static int make_tmap_f16(CUtensorMap *map, const void *base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+// 2-D row-major [rows, cols] fp16 or fp32 tensor, box = box_rows x 128 bytes of a row, 128B swizzle (rows / cols smaller than
+// the box are fine: the TMA unit fills the rest of the box with zeros)
+static int make_tmap(CUtensorMap *map, const void *base, uint64_t rows, uint64_t cols, uint32_t box_rows,
+                     CUtensorMapDataType type = CU_TENSOR_MAP_DATA_TYPE_FLOAT16) {
+    const uint32_t esize = (type == CU_TENSOR_MAP_DATA_TYPE_FLOAT32) ? 4 : 2;
     const uint64_t dims[2] = {cols, rows};
-    const uint64_t strides[1] = {cols * 2};
-    const uint32_t box[2] = {(uint32_t)TC_BLOCK_K, box_rows};
-    return tc_make_tmap_f16(map, base, 2, dims, strides, box);
-}
-
-// 2-D fp32 row-major [rows, cols] tensor, box = 64 rows x 32 columns (128 bytes), 128B swizzle (epilogue output boxes)
-static int make_tmap_f32_out(CUtensorMap *map, const void *base, uint64_t rows, uint64_t cols) {
-    TcEncodeTiledFn enc = tc_encode_fn();
-    if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return GSB_ERR_CUDA; }
-    cuuint64_t gdim[2] = {cols, rows};
-    cuuint64_t gstride[1] = {cols * 4};
-    cuuint32_t box[2] = {32, (cuuint32_t)TC_FRAG_ROWS};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void *>(base), gdim, gstride, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (fp32 output) failed (%d)", (int)r); return GSB_ERR_CUDA; }
-    return GSB_OK;
+    const uint64_t strides[1] = {cols * esize};
+    const uint32_t box[2] = {128 / esize, box_rows};
+    return tc_make_tmap(map, type, base, 2, dims, strides, box);
 }
 
 // Tensor-core packed layout (appended after the fp32 SIMT pack inside the same allocation):
@@ -386,11 +360,13 @@ static int tc_launch_layer(const CUtensorMap &tm_ah, const CUtensorMap &tm_al, c
     // (the next layer's A operand) or fp32 [M, N]
     CUtensorMap tm_o0, tm_o1;
     if (p.out_f32) {
-        if (int r = make_tmap_f32_out(&tm_o0, p.out_f32, (uint64_t)p.M, (uint64_t)p.N_total)) return r;
+        if (int r = make_tmap(&tm_o0, p.out_f32, (uint64_t)p.M, (uint64_t)p.N_total, TC_FRAG_ROWS,
+                              CU_TENSOR_MAP_DATA_TYPE_FLOAT32))
+            return r;
         tm_o1 = tm_o0;
     } else {
-        if (int r = make_tmap_f16(&tm_o0, p.out_hi, (uint64_t)p.M, (uint64_t)p.N_total, TC_FRAG_ROWS)) return r;
-        if (int r = make_tmap_f16(&tm_o1, p.out_lo, (uint64_t)p.M, (uint64_t)p.N_total, TC_FRAG_ROWS)) return r;
+        if (int r = make_tmap(&tm_o0, p.out_hi, (uint64_t)p.M, (uint64_t)p.N_total, TC_FRAG_ROWS)) return r;
+        if (int r = make_tmap(&tm_o1, p.out_lo, (uint64_t)p.M, (uint64_t)p.N_total, TC_FRAG_ROWS)) return r;
     }
     const int m_tiles = (p.M + TC_BLOCK_M - 1) / TC_BLOCK_M, n_tiles = (p.N_total + TC_BLOCK_N - 1) / TC_BLOCK_N;
     int avail = num_sms() - leave_free_sms;
@@ -420,10 +396,10 @@ int tc_gemm_plain(const __half *a_hi, const __half *a_lo, int64_t M, int K, cons
                   "tc_gemm_plain: need N%%32==0, K%%8==0 (M=%lld N=%d K=%d)", (long long)M, N, K);
     if (int r = tc_ensure_attr()) return r;
     CUtensorMap tm_ah, tm_al, tm_wh, tm_wl;
-    if (int r = make_tmap_f16(&tm_ah, a_hi, (uint64_t)M, (uint64_t)K, TC_BLOCK_M)) return r;
-    if (int r = make_tmap_f16(&tm_al, a_lo, (uint64_t)M, (uint64_t)K, TC_BLOCK_M)) return r;
-    if (int r = make_tmap_f16(&tm_wh, w_hi, (uint64_t)N, (uint64_t)K, TC_BLOCK_N)) return r;
-    if (int r = make_tmap_f16(&tm_wl, w_lo, (uint64_t)N, (uint64_t)K, TC_BLOCK_N)) return r;
+    if (int r = make_tmap(&tm_ah, a_hi, (uint64_t)M, (uint64_t)K, TC_BLOCK_M)) return r;
+    if (int r = make_tmap(&tm_al, a_lo, (uint64_t)M, (uint64_t)K, TC_BLOCK_M)) return r;
+    if (int r = make_tmap(&tm_wh, w_hi, (uint64_t)N, (uint64_t)K, TC_BLOCK_N)) return r;
+    if (int r = make_tmap(&tm_wl, w_lo, (uint64_t)N, (uint64_t)K, TC_BLOCK_N)) return r;
     TcParams p;
     p.bias = nullptr; p.out_hi = nullptr; p.out_lo = nullptr; p.out_f32 = out; p.overflow = overflow;
     p.inv_wscale = inv_wscale; p.M = (int)M; p.N_total = N; p.K = K; p.mode = 1;
@@ -457,10 +433,10 @@ int tc_linear(const float *x, const float *w, const float *bias, float *y, int64
     pixelnorm_split_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(x, x_hi, x_lo, n, K, 0, overflow);
     GSB_CHECK_LAUNCH();
     CUtensorMap tm_ah, tm_al, tm_wh, tm_wl;
-    if (int r = make_tmap_f16(&tm_ah, x_hi, (uint64_t)n, (uint64_t)K, TC_BLOCK_M)) return r;
-    if (int r = make_tmap_f16(&tm_al, x_lo, (uint64_t)n, (uint64_t)K, TC_BLOCK_M)) return r;
-    if (int r = make_tmap_f16(&tm_wh, w_hi, (uint64_t)N, (uint64_t)K, TC_BLOCK_N)) return r;
-    if (int r = make_tmap_f16(&tm_wl, w_lo, (uint64_t)N, (uint64_t)K, TC_BLOCK_N)) return r;
+    if (int r = make_tmap(&tm_ah, x_hi, (uint64_t)n, (uint64_t)K, TC_BLOCK_M)) return r;
+    if (int r = make_tmap(&tm_al, x_lo, (uint64_t)n, (uint64_t)K, TC_BLOCK_M)) return r;
+    if (int r = make_tmap(&tm_wh, w_hi, (uint64_t)N, (uint64_t)K, TC_BLOCK_N)) return r;
+    if (int r = make_tmap(&tm_wl, w_lo, (uint64_t)N, (uint64_t)K, TC_BLOCK_N)) return r;
     TcParams p;
     p.bias = bias; p.out_hi = nullptr; p.out_lo = nullptr; p.out_f32 = y; p.overflow = overflow;
     p.inv_wscale = scal; p.M = (int)n; p.N_total = N; p.K = K; p.mode = lrelu ? 0 : 2;
@@ -488,10 +464,10 @@ int mapping_forward_tc(const float *pb, void *tc_base, int n_layers, int dim,
     for (int l = 0; l < n_layers; ++l) {
         const int src = l & 1, dst = src ^ 1;
         CUtensorMap tm_ah, tm_al, tm_wh, tm_wl;
-        if (int r = make_tmap_f16(&tm_ah, a_hi[src], (uint64_t)n, dim, TC_BLOCK_M)) return r;
-        if (int r = make_tmap_f16(&tm_al, a_lo[src], (uint64_t)n, dim, TC_BLOCK_M)) return r;
-        if (int r = make_tmap_f16(&tm_wh, v.w_hi + l * per, dim, dim, TC_BLOCK_N)) return r;
-        if (int r = make_tmap_f16(&tm_wl, v.w_lo + l * per, dim, dim, TC_BLOCK_N)) return r;
+        if (int r = make_tmap(&tm_ah, a_hi[src], (uint64_t)n, dim, TC_BLOCK_M)) return r;
+        if (int r = make_tmap(&tm_al, a_lo[src], (uint64_t)n, dim, TC_BLOCK_M)) return r;
+        if (int r = make_tmap(&tm_wh, v.w_hi + l * per, dim, dim, TC_BLOCK_N)) return r;
+        if (int r = make_tmap(&tm_wl, v.w_lo + l * per, dim, dim, TC_BLOCK_N)) return r;
         TcParams p;
         p.bias = pb + (int64_t)l * dim;
         const bool last = (l == n_layers - 1);

@@ -11,7 +11,7 @@
 // Kernels: column sums (coalesced, fp64 atomics), then a 64x64-tile SYRK over the upper triangle of
 // tile pairs, split over row chunks; each CTA adds its fp32 tile into the fp64 Gram with atomics and
 // mirrors off-diagonal tiles so the chain reads a full symmetric matrix.
-#include "common.cuh"
+#include "tc_common.cuh"
 
 namespace gsb {
 
@@ -117,11 +117,6 @@ gram_centered_kernel(const float *__restrict__ x, int64_t n, int d, int64_t ld, 
             if (ti != tj) atomicAdd(&gram[(int64_t)gj * d + gi], v);
         }
 }
-
-// tensor-core form (stats_tc.cu)
-bool stats_tc_supported(int64_t nb, int d);
-size_t stats_tc_workspace_bytes(int n_groups, int64_t nb, int d);
-int stats_tc(const float *x, int n_groups, int64_t nb, int d, int64_t ld, double *mean, double *gram, void *ws, cudaStream_t st);
 
 }  // namespace gsb
 

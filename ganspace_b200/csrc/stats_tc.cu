@@ -12,15 +12,10 @@
 //   center_split_t_kernel    xt[g][c][r] = fp16 hi/lo split of (x[g nb + r][c] - mean32[c]) * 2^e_g (e_g: per-group power of two
 //                            that puts 2 max|x| into [8192, 32768), so hi keeps 11 bits and nothing overflows), i.e. the centred samples
 //                            TRANSPOSED so that the sample index is the contiguous (K) dimension of both MMA operands
-//   gram_groups_tc_kernel    persistent, one CTA per SM, work items (group, upper tile pair) of 128 x 128 outputs:
-//                              warp 8     TMA producer   3-D boxes {64 samples, 128 features, 1 group}, SWIZZLE_128B; samples
-//                                                        beyond nb are zero-filled by the TMA unit (no padding is ever read)
-//                              warps 0-7  two warpgroups, 64 output rows each: wgmma m64n128k16 with 3 MMAs per product
-//                                         (hi hi, lo hi, hi lo) into an fp32 register accumulator.  Tensor-core accumulation
-//                                         truncates when aligning addends, so only 4 K-blocks (48 MMA steps) are summed there;
-//                                         each partial is then added into a second set of fp32 registers with round-to-nearest
-//                                         (as gram_tc.cu does), and the tile is finally scaled by 2^-2e and stored (with its
-//                                         mirror image) as fp64.
+//   gram_tc_kernel           (gram_tc.cu, Store epilogue) the centred Gram of every group: persistent wgmma kernel over
+//                            (group, upper 128 x 128 tile pair) work items, 3 MMAs per product, promoted accumulation;
+//                            samples beyond nb are zero-filled by the TMA unit (no padding is ever read); each tile is
+//                            scaled by 2^-2e and stored (with its mirror image) as fp64.
 // Algorithmic work: 2 d^2 FLOP per sample (x3 MMAs); HBM traffic: x read twice (4 B), xt written and read (4 + 4 B per element,
 // the re-reads of the 10 tile pairs come out of L2).
 #include "tc_common.cuh"
@@ -29,42 +24,7 @@
 
 namespace gsb {
 
-// ---- host: tensor maps (shared by the tensor-core kernels) ----------------------------------------------------------
-TcEncodeTiledFn tc_encode_fn() {
-    static TcEncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void *ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<TcEncodeTiledFn>(ptr);
-    }
-    return fn;
-}
-
-int tc_make_tmap_f16(CUtensorMap *map, const void *base, int rank, const uint64_t *dims, const uint64_t *strides_bytes,
-                     const uint32_t *box) {
-    TcEncodeTiledFn enc = tc_encode_fn();
-    if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return GSB_ERR_CUDA; }
-    cuuint64_t gdim[5], gstride[4];
-    cuuint32_t bx[5], estr[5];
-    for (int i = 0; i < rank; ++i) { gdim[i] = dims[i]; bx[i] = box[i]; estr[i] = 1; }
-    for (int i = 0; i + 1 < rank; ++i) gstride[i] = strides_bytes[i];
-    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void *>(base), gdim, gstride, bx, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d)", (int)r); return GSB_ERR_CUDA; }
-    return GSB_OK;
-}
-
 namespace stc {
-
-constexpr int BM = 128, BN = 128, BK = 64;
-constexpr int STAGES = 3;
-constexpr int FLUSH_KB = 4;                 // K-blocks (of 64 samples) accumulated by the MMAs before the promotion
-constexpr uint32_t TILE_BYTES = BM * BK * 2;               // 16 KB
-constexpr uint32_t STAGE_BYTES = 4 * TILE_BYTES;           // 64 KB  (A_hi, A_lo, B_hi, B_lo)
-constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
 
 // ---- column sums per group ----------------------------------------------------------------------------------------
 constexpr int SUM_ROWS = 256;               // rows per column-sum slice
@@ -154,116 +114,6 @@ center_split_t_kernel(const float *__restrict__ x, int64_t nb, int d, int64_t ld
     }
 }
 
-// ---- Gram of every group ---------------------------------------------------------------------------------------------
-struct Params {
-    double *gram;           // [G][d][d]
-    const int *exps;        // [G] scale exponents of the split operands
-    int d, nt, npairs;      // nt = d / 128 row blocks, npairs = nt (nt + 1) / 2
-    int n_groups, nkb;      // nkb = ceil(nb / 64)
-};
-
-__device__ __forceinline__ void decode_pair(int pair, int nt, int &ti, int &tj) {
-    ti = 0;
-    while (pair >= nt - ti) { pair -= nt - ti; ++ti; }
-    tj = ti + pair;
-}
-
-__global__ void __launch_bounds__(tc::THREADS, 1)
-gram_groups_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, const Params p) {
-    using namespace tc;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + STAGES * STAGE_BYTES);
-    uint64_t *full_bar = bars;                     // [STAGES]
-    uint64_t *empty_bar = bars + STAGES;           // [STAGES]: one arrival per consumer warp
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int num_items = p.n_groups * p.npairs;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CONSUMER_THREADS / 32); }
-        mbar_fence_init();
-    }
-    if (warp == PRODUCER_WARP && lane == 0) { tma_prefetch_desc(&tm_hi); tma_prefetch_desc(&tm_lo); }
-    __syncthreads();
-
-    if (warp == PRODUCER_WARP) {
-        // ===================== TMA producer =====================
-        if (lane == 0) {
-            int stage = 0; uint32_t phase = 0;
-            for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-                const int g = item / p.npairs;
-                int ti, tj;
-                decode_pair(item % p.npairs, p.nt, ti, tj);
-                const bool diag = (ti == tj);
-                for (int kb = 0; kb < p.nkb; ++kb) {
-                    mbar_wait(&empty_bar[stage], phase ^ 1);
-                    uint8_t *st = smem + stage * STAGE_BYTES;
-                    mbar_arrive_expect_tx(&full_bar[stage], diag ? 2 * TILE_BYTES : 4 * TILE_BYTES);
-                    tma_load_3d(&tm_hi, &full_bar[stage], st, kb * BK, ti * BM, g);
-                    tma_load_3d(&tm_lo, &full_bar[stage], st + TILE_BYTES, kb * BK, ti * BM, g);
-                    if (!diag) {
-                        tma_load_3d(&tm_hi, &full_bar[stage], st + 2 * TILE_BYTES, kb * BK, tj * BN, g);
-                        tma_load_3d(&tm_lo, &full_bar[stage], st + 3 * TILE_BYTES, kb * BK, tj * BN, g);
-                    }
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else {
-        // ===================== MMA + promoted accumulation + store =====================
-        const int wg = warp >> 2;                       // 64-row half of the 128-row tile
-        const int row_frag = wg * 64 + (warp & 3) * 16 + (lane >> 2), col_frag = 2 * (lane & 3);
-        int stage = 0; uint32_t phase = 0;
-        float acc[64], r[64];
-#pragma unroll
-        for (int j = 0; j < 64; ++j) { acc[j] = 0.f; r[j] = 0.f; }
-        for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-            const int g = item / p.npairs;
-            const double unscale = ldexp(1.0, -2 * __ldg(p.exps + g));
-            int ti, tj;
-            decode_pair(item % p.npairs, p.nt, ti, tj);
-            const uint32_t boff = (ti == tj) ? 0u : 2 * TILE_BYTES;      // diagonal tile: B is A
-            for (int g0 = 0; g0 < p.nkb; g0 += FLUSH_KB) {
-                const int g1 = (g0 + FLUSH_KB < p.nkb) ? g0 + FLUSH_KB : p.nkb;
-                for (int kb = g0; kb < g1; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    const uint32_t st = smem_u32(smem + stage * STAGE_BYTES);
-                    const uint32_t sa = st + (uint32_t)wg * (TILE_BYTES / 2);
-                    wgmma_fence();
-                    split_kblock_m64n128(acc, sw128_kmajor_desc(sa), sw128_kmajor_desc(sa + TILE_BYTES),
-                                         sw128_kmajor_desc(st + boff), sw128_kmajor_desc(st + boff + TILE_BYTES), kb > g0);
-                    wgmma_commit();
-                    wgmma_wait_all();
-                    if (lane == 0) mbar_arrive(&empty_bar[stage]);
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-#pragma unroll
-                for (int j = 0; j < 64; ++j) r[j] = __fadd_rn(r[j], acc[j]);
-            }
-            double *G = p.gram + (size_t)g * p.d * p.d;
-            const bool diag = (ti == tj);
-#pragma unroll
-            for (int j = 0; j < 64; j += 2) {
-                const int gm = ti * BM + row_frag + 8 * ((j >> 1) & 1), gn = tj * BN + 8 * (j >> 2) + col_frag;
-                const double v0 = (double)r[j] * unscale, v1 = (double)r[j + 1] * unscale;
-                if (!diag) {
-                    *reinterpret_cast<double2 *>(G + (size_t)gm * p.d + gn) = make_double2(v0, v1);
-                    G[(size_t)gn * p.d + gm] = v0;
-                    G[(size_t)(gn + 1) * p.d + gm] = v1;
-                } else {
-                    // diagonal tile: (i,j) and (j,i) come out of differently ordered MMA sums; keep the upper triangle and
-                    // mirror it, so the chain reads an exactly symmetric matrix
-                    if (gn >= gm) { G[(size_t)gm * p.d + gn] = v0; G[(size_t)gn * p.d + gm] = v0; }
-                    if (gn + 1 >= gm) { G[(size_t)gm * p.d + gn + 1] = v1; G[(size_t)(gn + 1) * p.d + gm] = v1; }
-                }
-            }
-#pragma unroll
-            for (int j = 0; j < 64; ++j) r[j] = 0.f;
-        }
-    }
-}
-
 struct WsView {
     double *sum;
     float *mean32;
@@ -307,11 +157,6 @@ int stats_tc(const float *x, int n_groups, int64_t nb, int d, int64_t ld, double
     using namespace stc;
     WsView w = carve(ws, n_groups, nb, d);
     const int64_t nbp = (nb + 63) / 64 * 64;
-    static bool attr_set = false;
-    if (!attr_set) {
-        GSB_CHECK_CUDA(cudaFuncSetAttribute(gram_groups_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-        attr_set = true;
-    }
     GSB_CHECK_CUDA(cudaMemsetAsync(w.absmax, 0, (size_t)n_groups * sizeof(float), st));
     {
         const int ny = (int)((nb + SUM_ROWS - 1) / SUM_ROWS);
@@ -326,20 +171,7 @@ int stats_tc(const float *x, int n_groups, int64_t nb, int d, int64_t ld, double
         center_split_t_kernel<<<grid, 256, 0, st>>>(x, nb, d, ld, nbp, w.mean32, w.exps, w.xt_hi, w.xt_lo);
         GSB_CHECK_LAUNCH();
     }
-    CUtensorMap tm_hi, tm_lo;
-    const uint64_t dims[3] = {(uint64_t)nb, (uint64_t)d, (uint64_t)n_groups};
-    const uint64_t strides[2] = {(uint64_t)nbp * 2, (uint64_t)d * nbp * 2};
-    const uint32_t box[3] = {(uint32_t)BK, (uint32_t)BM, 1};
-    if (int r = tc_make_tmap_f16(&tm_hi, w.xt_hi, 3, dims, strides, box)) return r;
-    if (int r = tc_make_tmap_f16(&tm_lo, w.xt_lo, 3, dims, strides, box)) return r;
-    Params p;
-    p.gram = gram; p.exps = w.exps; p.d = d; p.nt = d / BM; p.npairs = p.nt * (p.nt + 1) / 2;
-    p.n_groups = n_groups; p.nkb = (int)(nbp / BK);
-    const int items = p.n_groups * p.npairs;
-    const int grid = items < num_sms() ? items : num_sms();
-    gram_groups_tc_kernel<<<grid, tc::THREADS, SMEM_BYTES, st>>>(tm_hi, tm_lo, p);
-    GSB_CHECK_LAUNCH();
-    return GSB_OK;
+    return gram_tc_launch(GramEpilogue::Store, w.xt_hi, w.xt_lo, nb, nbp, n_groups, d, d, w.exps, gram, st);
 }
 
 }  // namespace gsb

@@ -20,14 +20,10 @@
 // over channels; between layers they travel as fp16 hi/lo pairs already multiplied by the NEXT layer's style.
 // The hooked layer's activation is written as fp32 NHWC rows of length res*res*co with a caller-given row stride
 // (directly into the large-d IPCA batch buffer).  Samples are processed in chunks whose tap planes (Y) fit the L2.
-#include "common.cuh"
-#include <cuda_fp16.h>
+#include "tc_common.cuh"
 #include <math.h>
 
 namespace gsb {
-
-int tc_gemm_plain(const __half *a_hi, const __half *a_lo, int64_t M, int K, const __half *w_hi, const __half *w_lo, int N,
-                  const float *inv_wscale, float *out, unsigned *overflow, int leave_free_sms, cudaStream_t st);
 
 constexpr int SY_MAX_LAYERS = 24;
 constexpr int SY_CHUNK_ROWS = 2048;       // GEMM rows per launch: 2048 x 9*512 fp32 tap planes = 38 MB (fits the 50 MB L2)
@@ -120,11 +116,8 @@ __global__ void sy_weight_pack_kernel(const float *__restrict__ W, int cout, int
         for (int tap = 0; tap < 9; ++tap) {
             const float w = W[idx * 9 + tap] * scale;
             sq = fmaf(w, w, sq);
-            const float ww = w * ws;
-            const __half h = __float2half_rn(ww);
             const int64_t o = ((int64_t)tap * cout + co) * cin + ci;
-            hi[o] = h;
-            lo[o] = __float2half_rn(ww - __half2float(h));
+            tc::split1(w * ws, hi[o], lo[o]);
         }
         wsq[idx] = sq;
     }
@@ -152,18 +145,8 @@ __global__ void sy_rsqrt_eps_kernel(float *__restrict__ x, int64_t count) {
 }
 
 __device__ __forceinline__ void store_split4(const float (&f)[4], __half *hi, __half *lo, int64_t off, bool &ovf) {
-    __half h[4], l[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-        h[q] = __float2half_rn(f[q]);
-        l[q] = __float2half_rn(f[q] - __half2float(h[q]));
-        ovf |= fabsf(f[q]) > 60000.f;
-    }
     uint2 ph, pl;
-    ph.x = (uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16);
-    ph.y = (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16);
-    pl.x = (uint32_t)__half_as_ushort(l[0]) | ((uint32_t)__half_as_ushort(l[1]) << 16);
-    pl.y = (uint32_t)__half_as_ushort(l[2]) | ((uint32_t)__half_as_ushort(l[3]) << 16);
+    ovf |= tc::split4(f, ph, pl);
     *reinterpret_cast<uint2 *>(hi + off) = ph;
     *reinterpret_cast<uint2 *>(lo + off) = pl;
 }

@@ -1,9 +1,11 @@
-// wgmma / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (stats_tc.cu, gram_tc.cu, mapping_tc.cu).
-// sm_90a (Hopper).  The shared-memory descriptor encoding follows cute::GMMA::GmmaDescriptor.
+// wgmma / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (gram_tc.cu, mapping_tc.cu), the fp32 -> fp16 hi/lo
+// operand split, and the declarations of the tensor-core entry points that other files call.  sm_90a (Hopper).  The
+// shared-memory descriptor encoding follows cute::GMMA::GmmaDescriptor.
 //
 // Warp layout: warpgroups 0 and 1 (warps 0-7) are the MMA consumers and keep their accumulators in registers; warp 8 holds
-// the TMA producer (one elected thread).  In stats_tc.cu and gram_tc.cu each consumer warpgroup owns 64 rows of a 128-row
-// tile; mapping_tc.cu gives each whole 128 x 128 tiles in turns and makes warps 8-11 a producer warpgroup (setmaxnreg).
+// the TMA producer (one elected thread).  In the Gram kernel (gram_tc.cu: the batch statistics of stats_tc.cu and the
+// large-d small side of bigd.cu) each consumer warpgroup owns 64 rows of a 128-row tile; mapping_tc.cu gives each whole
+// 128 x 128 tiles in turns and makes warps 8-11 a producer warpgroup (setmaxnreg).
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
@@ -121,23 +123,65 @@ __device__ __forceinline__ void split_kblock_m64n128(float (&d)[64], uint64_t ah
     }
 }
 
-// ---- fp32 -> fp16 hi/lo split (22 significant bits) -----------------------------------------------------------------
+// ---- fp32 -> fp16 hi/lo split (22 significant bits): x = hi + lo, hi = fp16(x), lo = fp16(x - hi) -----------------------
+__device__ __forceinline__ void split1(float x, __half &hi, __half &lo) {
+    hi = __float2half_rn(x);
+    lo = __float2half_rn(x - __half2float(hi));
+}
+// two values, packed as half2 bit patterns (a in the low half)
 __device__ __forceinline__ void split2(float a, float b, uint32_t &hi, uint32_t &lo) {
-    const __half h0 = __float2half_rn(a), h1 = __float2half_rn(b);
-    const __half l0 = __float2half_rn(a - __half2float(h0)), l1 = __float2half_rn(b - __half2float(h1));
+    __half h0, h1, l0, l1;
+    split1(a, h0, l0);
+    split1(b, h1, l1);
     hi = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
     lo = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
+}
+// four values, packed as 4 x fp16 (8 bytes); returns whether any |f| exceeds 60000 (hi would be at or near fp16's range end)
+__device__ __forceinline__ bool split4(const float (&f)[4], uint2 &hi, uint2 &lo) {
+    split2(f[0], f[1], hi.x, lo.x);
+    split2(f[2], f[3], hi.y, lo.y);
+    return (fabsf(f[0]) > 60000.f) | (fabsf(f[1]) > 60000.f) | (fabsf(f[2]) > 60000.f) | (fabsf(f[3]) > 60000.f);
 }
 
 }  // namespace tc
 
-// ---- host: tensor maps ---------------------------------------------------------------------------------------------
-typedef CUresult (*TcEncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                    const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-TcEncodeTiledFn tc_encode_fn();
-// fp16 tensor, innermost dimension contiguous, 128B swizzle; dims/box innermost first; strides (bytes) of dims 1..rank-1
-int tc_make_tmap_f16(CUtensorMap *map, const void *base, int rank, const uint64_t *dims, const uint64_t *strides_bytes,
-                     const uint32_t *box);
+// ---- host: tensor maps (core.cu) -------------------------------------------------------------------------------------
+// fp16 or fp32 tensor, innermost dimension contiguous, 128B swizzle, L2 promotion 256 B, out-of-bounds elements read as zero;
+// dims / box innermost first; strides (bytes) of dims 1..rank-1
+int tc_make_tmap(CUtensorMap *map, CUtensorMapDataType type, const void *base, int rank, const uint64_t *dims,
+                 const uint64_t *strides_bytes, const uint32_t *box);
+
+// ---- entry points used across files ----------------------------------------------------------------------------------
+// Gram kernel with promoted accumulation (gram_tc.cu).  Operands: n_groups fp16 hi/lo matrices of n_pad rows x k columns,
+// rows k_pitch elements apart, scaled by powers of two 2^e.
+//   Store:      out[g] = 2^-2e_g (x x^T)_g for each group (exps: [n_groups]; n_rows == n_pad, a multiple of 128); every
+//               entry is written, so out need not be zeroed
+//   Accumulate: out += 2^-(e_i + e_j) (x x^T)_ij for i, j < n_rows of the one group (exps: [n_pad], one per row); out is
+//               summed into with fp64 atomics over 4096-column chunks of k
+enum class GramEpilogue { Store, Accumulate };
+int gram_tc_launch(GramEpilogue epi, const __half *hi, const __half *lo, int64_t k, int64_t k_pitch, int n_groups, int n_pad,
+                   int n_rows, const int *exps, double *out, cudaStream_t st);
+// large-d small side T = M M^T (gram_tc.cu)
+size_t gram_tc_workspace_bytes(int n_pad, int64_t d);
+bool gram_tc_supported(int64_t d);
+int gram_tc(const float *M, int n_rows, int n_pad, int64_t d, void *ws, double *T, cudaStream_t st);
+
+// batch means and centred Grams of consecutive row groups (stats_tc.cu)
+bool stats_tc_supported(int64_t nb, int d);
+size_t stats_tc_workspace_bytes(int n_groups, int64_t nb, int d);
+int stats_tc(const float *x, int n_groups, int64_t nb, int d, int64_t ld, double *mean, double *gram, void *ws, cudaStream_t st);
+
+// mapping network, dense layers and the conv tap GEMM on the persistent layer kernel (mapping_tc.cu)
+size_t mapping_tc_packed_bytes(int n_layers, int dim);
+int mapping_tc_pack(const float *pw, int n_layers, int dim, void *tc_base, cudaStream_t st);
+int mapping_forward_tc(const float *pb, void *tc_base, int n_layers, int dim, const float *d_z, float *d_w,
+                       int64_t n, bool pixelnorm, void *ws, int leave_free_sms, cudaStream_t st);
+size_t mapping_tc_workspace_bytes(int64_t n, int dim);
+unsigned *mapping_tc_overflow_flag(void *tc_base, int n_layers, int dim);
+size_t tc_linear_workspace_bytes(int64_t n, int N, int K);
+int tc_linear(const float *x, const float *w, const float *bias, float *y, int64_t n, int N, int K, bool lrelu, void *ws,
+              cudaStream_t st);
+int tc_gemm_plain(const __half *a_hi, const __half *a_lo, int64_t M, int K, const __half *w_hi, const __half *w_lo, int N,
+                  const float *inv_wscale, float *out, unsigned *overflow, int leave_free_sms, cudaStream_t st);
 
 }  // namespace gsb
