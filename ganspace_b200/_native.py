@@ -75,6 +75,13 @@ SIGNATURES = {
     "gsb_bigd_step_gram": (_I, [_P, _P, _L, _I, _I, _L, _I, _I, _P, _P, _Z, _P]),
     "gsb_bigd_step_solve": (_I, [_P, _P, _L, _I, _I, _L, _I, _I, _P, _P, _Z, _P]),
     "gsb_bigd_step_commit": (_I, [_P, _P, _L, _I, _I, _L, _I, _I, _P, _P, _Z, _P]),
+    "gsb_fbpca_state_bytes": (_Z, [_I]),
+    "gsb_fbpca_reset": (_I, [_P, _I, _P]),
+    "gsb_fbpca_accumulate": (_I, [_P, _I, _I, _L, _P, _P, _P]),
+    "gsb_fbpca_add_zero_rows": (_I, [_P, _I, _L, _P]),
+    "gsb_fbpca_workspace_bytes": (_Z, [_I, _I, _I]),
+    "gsb_fbpca_solve": (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _Z, _P]),
+    "gsb_fbpca_status": (_I, [_P, _I, _P, _P]),
 }
 
 
@@ -912,3 +919,64 @@ class BigIPCA:
         full = torch.empty((W * n, dl), dtype=local.dtype, device=local.device)
         dist.all_gather_into_tensor(full, local)
         return full.view(W, n, dl).permute(1, 0, 2).reshape(n, W * dl).contiguous()
+
+
+class FBPCARankError(NativeError):
+    """fbpca's range finder needs data of numerical rank >= l = 2 n_components; the solve met a non-positive pivot."""
+
+
+class FBPCAPool:
+    """Pooled (n, mean, centred scatter) of a sample matrix built from per-group statistics, and the fbpca solve on it
+    (csrc/rsvd.cu; small-d engine, 32 <= d <= 1024, d % 32 == 0).  Groups are folded in the order they are passed."""
+
+    def __init__(self, d: int, device):
+        lib = load()
+        self.dev = require_cuda(device)
+        self.d = int(d)
+        self.n = 0
+        self.state = torch.empty(lib.gsb_fbpca_state_bytes(self.d), dtype=torch.uint8, device=self.dev)
+        with torch.cuda.device(self.dev):
+            _check(lib.gsb_fbpca_reset(_ptr(self.state), self.d, _stream()), "gsb_fbpca_reset")
+
+    def accumulate(self, rows_per_group: int, means: torch.Tensor, grams: torch.Tensor):
+        """Fold G groups: means [G, d], grams [G, d, d] (fp64, device), rows_per_group rows each."""
+        means = means.reshape(-1, self.d)
+        assert means.dtype == grams.dtype == torch.float64 and grams.numel() == means.shape[0] * self.d * self.d
+        assert means.is_contiguous() and grams.is_contiguous()
+        g = means.shape[0]
+        with torch.cuda.device(self.dev), instrument.section("fbpca_pool"):
+            _check(load().gsb_fbpca_accumulate(_ptr(self.state), self.d, g, int(rows_per_group), _ptr(means), _ptr(grams),
+                                               _stream()), "gsb_fbpca_accumulate")
+        instrument.count(2)
+        self.n += g * int(rows_per_group)
+
+    def add_zero_rows(self, n_zero: int):
+        if n_zero <= 0:
+            return
+        with torch.cuda.device(self.dev), instrument.section("fbpca_pool"):
+            _check(load().gsb_fbpca_add_zero_rows(_ptr(self.state), self.d, int(n_zero), _stream()), "gsb_fbpca_add_zero_rows")
+        instrument.count(2)
+        self.n += int(n_zero)
+
+    def solve(self, c: int, l: int, omega: torch.Tensor = None, raw: bool = False):
+        """-> dict(components [c, d], stdev [c], var_ratio [c], mean [d]) as fp64 device tensors.  ``omega`` [d, l] selects the
+        randomized branch (None: exact).  Raises FBPCARankError when the data's numerical rank is below l."""
+        lib = load()
+        f64 = dict(dtype=torch.float64, device=self.dev)
+        out = {"components": torch.empty((c, self.d), **f64), "stdev": torch.empty(c, **f64),
+               "var_ratio": torch.empty(c, **f64), "mean": torch.empty(self.d, **f64)}
+        if omega is not None:
+            omega = omega.to(self.dev, torch.float64).contiguous()
+            assert omega.shape == (self.d, l)
+        ws = scratch.get("fbpca", lib.gsb_fbpca_workspace_bytes(self.d, int(c), int(l)), self.dev)
+        with torch.cuda.device(self.dev):
+            with instrument.section("fbpca_solve"):
+                _check(lib.gsb_fbpca_solve(_ptr(self.state), self.d, int(c), int(l), 1 if raw else 0, _ptr(omega),
+                                           _ptr(out["components"]), _ptr(out["stdev"]), _ptr(out["var_ratio"]), _ptr(out["mean"]),
+                                           _ptr(ws), ws.numel(), _stream()), "gsb_fbpca_solve")
+            flags = C.c_uint(0)
+            _check(lib.gsb_fbpca_status(_ptr(self.state), self.d, C.byref(flags), _stream()), "gsb_fbpca_status")
+        if flags.value & 1:
+            raise FBPCARankError(f"fbpca: the samples have numerical rank below l = {l} (a Cholesky pivot of the range finder "
+                                 "was not positive); use fewer components or more varied samples")
+        return out

@@ -298,13 +298,21 @@ def compute_arrays(config, instrumented_model, state=None):
     if affine is not None and config.components > affine.rank:
         raise NotImplementedError(f"components={config.components} exceeds the rank {affine.rank} of layer {layer_key}")
     transformer = get_estimator(config.estimator, config.components, config.sparsity, device=device)
-    if not transformer.batch_support:
-        raise RuntimeError("only batched estimators run on the device path")
+    # fbpca (the one non-batched estimator on the device path) pools the per-group statistics instead of merging them into a
+    # chain, and solves once at the end (estimators.FacebookPCAEstimator, csrc/rsvd.cu)
+    pooled = not transformer.batch_support
     samples_are_latents = layer_key in ["g_mapping", "style"] and inst.model.latent_space_name() == "W"
+    if pooled and affine is not None:
+        raise NotImplementedError(f"--est {config.estimator} is not available for layer {layer_key} (an affine layer: the "
+                                  "test matrix would have to be projected through its isometry); use --est ipca")
     # conv feature maps (d up to ~10^6): the large-d IPCA engine keeps sklearn's stacked matrix in HBM and the model's
     # producer kernels write each batch into it in the device feature order (NHWC); the fixed NHWC->NCHW permutation
     # is applied once to the exported components (PCA is equivariant under it)
-    large_d = affine is None and not samples_are_latents and sample_dims > transformer.transformer.SMALL_D_MAX
+    small_d_max = transformer.SMALL_D_MAX if pooled else transformer.transformer.SMALL_D_MAX
+    large_d = affine is None and not samples_are_latents and sample_dims > small_d_max
+    if pooled and large_d:
+        raise NotImplementedError(f"--est {config.estimator} is not available for conv feature maps (d = {sample_dims} > "
+                                  f"{small_d_max}); use --est ipca")
     layout = model.feature_layout(layer_key) if (large_d and hasattr(model, "feature_layout")) else None
     if large_d and live:
         # row-parallel generation + feature-sharded chain (SURVEY.md section 8e): rank r synthesises rows
@@ -330,6 +338,9 @@ def compute_arrays(config, instrumented_model, state=None):
 
     # ---- Phase A: the seeds of every sample_latent(B) call the reference makes (:232-236) ----------
     seeds = _draw_seeds(pl.n_calls)
+    # fbpca draws its test matrix from the global state when it fits, after the collection (:284) and before the W-space
+    # lat_stdev seed (:327); nothing in between draws, so it is the next draw here
+    omega = transformer.draw_omega(N + NB, sample_dims) if pooled else None
     # W-space runs end with model.sample_latent(5000) for lat_stdev (:325-329).  Without a regression pass nothing touches the
     # global NumPy state in between, so its seed is the next draw; its latent stream (one sequential MT19937 stream, ~6 ms on
     # one SM) is generated on a side stream while the run proceeds instead of at the tail of the critical path.
@@ -347,6 +358,9 @@ def compute_arrays(config, instrumented_model, state=None):
     k = 0
     stop = False                 # fit_partial returned False (e.g. n_components > first batch): the reference leaves the loop (:262-263)
     exchange = _StatsExchange(d, world) if (live and not large_d) else None
+    # fbpca's random_stdevs project the first rows of the whole sample matrix (:313-316): rows [0, K NB) hold group data, the
+    # rest of the first min(5000, N + NB) rows stay zero.  Each row is written by the rank that owns its group.
+    first = torch.zeros((min(5000, N + NB), d), dtype=torch.float32, device=device) if pooled else None
 
     def group_rows(rows):
         """[n, d] activations of the hooked layer for latent rows ``rows`` (small-d engine; n is a multiple of NB)."""
@@ -429,6 +443,9 @@ def compute_arrays(config, instrumented_model, state=None):
                             _native.batch_stats_multi(Xb, len(span), NB, mean_out=means[i0:i0 + len(span)],
                                                       gram_out=grams[i0:i0 + len(span)])
                             i0 += len(span)
+                            if first is not None and span[0] * NB < first.shape[0]:
+                                cnt = min(first.shape[0] - span[0] * NB, len(span) * NB)
+                                first[span[0] * NB:span[0] * NB + cnt] = Xb[:cnt]
                         X = Xb[(len(span) - 1) * NB:]
                     if (K - 1) in rnd and _plan.owner(K - 1, world) != rank:
                         r0 = where[K - 1]                                # every rank keeps the final group's sample buffer
@@ -458,8 +475,16 @@ def compute_arrays(config, instrumented_model, state=None):
     except KeyboardInterrupt:
         if live:
             raise
+        if pooled:
+            sys.exit(1)          # nothing fitted yet, and the reference writes nothing (:269-270)
         # the reference's `gi` of the interrupted group (:268-272) = the samples merged so far
         state["canceled_at"] = int(tr.n_samples_seen_)
+    if pooled:
+        if live:
+            import torch.distributed as dist
+            dist.all_reduce(first)                               # each row is non-zero on exactly one rank
+        transformer.add_zero_rows(N + NB - K * NB)               # the unfilled tail of the sample matrix (:224)
+        transformer.fit_pooled(omega=omega)
     tick("sampling + activations + IPCA chain")
     # host work that does not depend on the chain's result, done while the device still runs the last merge steps (the
     # export below is the first call that waits for them): get_random_dirs' host stream + upload, the lat_stdev latents
@@ -469,9 +494,9 @@ def compute_arrays(config, instrumented_model, state=None):
     pre_lat = model.z_to_latent(lat_stdev_z()).reshape(5000, input_dims) if (config.use_w and lat_stdev_z is not None) else None
     X_comp, X_stdev, X_var_ratio = transformer.get_components()
     X_comp = np.array(X_comp, copy=True)
-    mean_dev = tr.device_attributes()["mean"]
+    mean_dev = transformer.device_outputs["mean"] if pooled else tr.device_attributes()["mean"]
     if affine is None:
-        X_global_mean = tr.mean_.reshape((1, sample_dims))
+        X_global_mean = (transformer.pooled_mean if pooled else tr.mean_).reshape((1, sample_dims))
         Y_comp, Y_mean = X_comp, X_global_mean              # device feature order (== the reference's unless `layout`)
     else:
         # lift through the isometry: components = components_y Q^T (svd_flip's sign rule is applied on the lifted
@@ -497,6 +522,8 @@ def compute_arrays(config, instrumented_model, state=None):
     Z_comp /= np.linalg.norm(Z_comp, axis=-1, keepdims=True)
 
     # random projections of the last group's buffer, centred on the global mean (:289-291,312-316)
+    if pooled:
+        X = first
     n_rand_samples = min(5000, NB if large_d else X.shape[0])
     if device_dirs:
         # get_random_dirs' stream (RandomState(2).normal) drawn by the device generator: 42M normals at convs.4

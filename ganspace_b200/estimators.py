@@ -10,11 +10,14 @@ reference API allows) or CUDA tensors (no copy: the samples never leave HBM).  F
 maps) the d x d Gram is out of reach and the small-side engine (csrc/bigd.cu) takes over behind the same
 interface; its stacked matrix lives in HBM and producers can write batches in place (``batch_buffer``).
 
-The other estimators of the reference (pca / fbpca / ica / spca, estimators.py:18-52,84-204) are not
-batched and appear in no BASELINE config; asking for them raises (SURVEY.md section 2 marks them out of
-scope).
+``FacebookPCAEstimator`` (estimators.py:120-160, fbpca.pca with raw=True) runs on the device from pooled batch statistics
+(csrc/rsvd.cu): its fit depends on the stacked samples only through their d x d Gram, so the driver never materialises them.
+The remaining estimators of the reference (pca / ica / spca, estimators.py:18-52,84-118,162-204) are not batched and appear
+in no BASELINE config; asking for them raises (SURVEY.md section 2 marks them out of scope).
 """
 from __future__ import annotations
+
+from types import SimpleNamespace
 
 import numpy as np
 import torch
@@ -240,10 +243,115 @@ class IPCAEstimator:
         return self.transformer.components_, stdev, var_ratio
 
 
+class FacebookPCAEstimator:
+    """fbpca.pca(X, k=c, n_iter=2, raw=True, l=2c) on the device (reference estimators.py:124-160).
+
+    ``fit(X)`` takes the whole sample matrix (host ndarray or CUDA tensor, d <= 1024).  The driver instead feeds per-group
+    statistics (``fit_partial_stats``, in the reference's row order), pads with the zero rows of its unfilled sample matrix
+    (``add_zero_rows``) and calls ``fit_pooled``; the samples are never stacked.  fbpca's test matrix Omega is drawn from
+    NumPy's global state (``draw_omega``), exactly as fbpca draws it, unless the caller passes one."""
+
+    SMALL_D_MAX = DeviceIncrementalPCA.SMALL_D_MAX
+
+    def __init__(self, n_components, device=None):
+        self.n_components = n_components
+        self.transformer = SimpleNamespace()
+        self.batch_support = False
+        self.n_iter = 2
+        self.l = 2 * self.n_components
+        self._device = device
+        self._pool = None
+        self.stdev = None
+        self.total_var = None
+        self.var_ratio = None
+        self.device_outputs = None
+
+    def get_param_str(self):
+        return "fbpca_c{}_it{}_l{}".format(self.n_components, self.n_iter, self.l)
+
+    def randomized(self, m, d):
+        """fbpca's branch choice for an [m, d] matrix: False = exact SVD (l >= m/1.25 or l >= d/1.25)."""
+        return not (self.l >= m / 1.25 or self.l >= d / 1.25)
+
+    def draw_omega(self, m, d):
+        """fbpca's test matrix for an [m, d] matrix (m >= d): np.random.uniform(-1, 1, (d, l)) cast to float32, drawn from the
+        global NumPy state -- or None for the exact branch, which draws nothing."""
+        if not self.randomized(m, d):
+            return None
+        return np.random.uniform(low=-1.0, high=1.0, size=(d, self.l)).astype(np.float32)
+
+    def _ensure(self, d, device):
+        if self._pool is None:
+            if not (32 <= d <= self.SMALL_D_MAX and d % 32 == 0):
+                raise NotImplementedError(f"fbpca runs on the device for 32 <= d <= {self.SMALL_D_MAX}, d % 32 == 0 (d={d})")
+            self._pool = _native.FBPCAPool(d, _native.require_cuda(device if device is not None else self._device))
+        elif self._pool.d != d:
+            raise ValueError(f"Number of input features has changed from {self._pool.d} to {d}")
+        return self._pool
+
+    def fit_partial_stats(self, n_batch, mean_b, gram_b):
+        """Pool one group's statistics (n, mean [d], centred Gram [d, d]; fp64 device tensors), in the reference's row order."""
+        pool = self._ensure(int(mean_b.shape[-1]), mean_b.device)
+        pool.accumulate(int(n_batch), mean_b.reshape(1, -1).contiguous(), gram_b.contiguous())
+        return True
+
+    def add_zero_rows(self, n_zero):
+        self._pool.add_zero_rows(int(n_zero))
+
+    def fit_pooled(self, omega=None, raw=False):
+        """fbpca.pca on the pooled samples: ``raw`` = False when they were centred (the driver: X = samples - mean, so
+        X^T X is the centred scatter), True for fbpca's raw=True on uncentred rows.  ``omega`` [d, l] (None = exact branch)."""
+        pool = self._pool
+        c, d = self.n_components, pool.d
+        if not (1 <= c <= min(pool.n, d)):
+            raise ValueError(f"n_components={c} must be in [1, min(n_samples, n_features)] = [1, {min(pool.n, d)}]")
+        if omega is not None:
+            omega = torch.as_tensor(np.asarray(omega, dtype=np.float64) if isinstance(omega, np.ndarray) else omega)
+        out = pool.solve(c, self.l, omega=omega, raw=raw)
+        self.device_outputs = out
+        flat = torch.cat([out["components"].reshape(-1), out["stdev"], out["var_ratio"], out["mean"]]).cpu().numpy()
+        comp, rest = flat[:c * d].reshape(c, d), flat[c * d:]
+        self.transformer.components_ = comp
+        self.stdev = rest[:c]
+        self.var_ratio = rest[c:2 * c]
+        self.total_var = float(self.stdev[0] ** 2 / self.var_ratio[0]) if self.var_ratio[0] > 0 else 0.0
+        mean = rest[2 * c:].reshape(1, d)
+        # X.mean(0) of the matrix fbpca saw: the raw rows' mean, or ~0 when the driver centred them
+        self.transformer.mean_ = mean if raw else np.zeros_like(mean)
+        self.pooled_mean = mean
+        dotps = comp @ comp.T - np.eye(c)
+        if not np.allclose(dotps, 0, atol=1e-4):
+            print("FBPCA components not orghogonal, max dot", np.abs(dotps).max())
+
+    def fit(self, X, omega=None):
+        """fbpca.pca(X, k=c, n_iter=2, raw=True, l=2c) for an [m, d] matrix with m >= d (host ndarray or CUDA tensor)."""
+        if isinstance(X, np.ndarray):
+            X = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float32)).to(_native.require_cuda(self._device))
+        if X.dim() != 2:
+            raise ValueError("Expected 2D array, got %dD" % X.dim())
+        m, d = int(X.shape[0]), int(X.shape[1])
+        if m < d:
+            raise NotImplementedError("fbpca on the device covers m >= n (more samples than features)")
+        self._pool = None
+        pool = self._ensure(d, X.device)
+        mean, gram = _native.batch_stats(X.float().contiguous())
+        pool.accumulate(m, mean.reshape(1, d), gram.reshape(1, d, d))
+        if omega is None:
+            omega = self.draw_omega(m, d)
+        elif not self.randomized(m, d):
+            omega = None
+        self.fit_pooled(omega=omega, raw=True)
+
+    def get_components(self):
+        return self.transformer.components_, self.stdev, self.var_ratio
+
+
 def get_estimator(name, n_components, alpha, device=None):
     if name == "ipca":
         return IPCAEstimator(n_components, device=device)
-    if name in ("pca", "fbpca", "ica", "spca"):
+    if name == "fbpca":
+        return FacebookPCAEstimator(n_components, device=device)
+    if name in ("pca", "ica", "spca"):
         raise RuntimeError(f"estimator '{name}' is not batched and outside the GPU hot path "
                            "(SURVEY.md section 2); use 'ipca'")
     raise RuntimeError("Unknown estimator")
