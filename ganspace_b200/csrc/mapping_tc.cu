@@ -15,16 +15,21 @@
 // Kernel (one launch per layer; activations travel between layers as fp16 hi/lo pairs = the same 4 B/element
 // as fp32): persistent, one CTA per SM, warp-specialised, ping-pong: each consumer warpgroup owns whole 128 x 128 output
 // tiles, and the two take turns on the tensor cores, so that one's epilogue runs under the other's MMAs:
-//     warps 8-11  producer warpgroup: one thread issues the TMA loads of the CTA's tiles in order (A_hi, A_lo, W_hi, W_lo:
-//                 128 x 64 boxes; SWIZZLE_128B, K-major); the warpgroup hands most of its registers to the consumers
-//                 (setmaxnreg)
+//     warps 8-11  producer warpgroup: one thread claims the CTA's tiles from the launch's queue and issues their TMA loads in
+//                 order (A_hi, A_lo, W_hi, W_lo: 128 x 64 boxes; SWIZZLE_128B, K-major); the warpgroup hands most of its
+//                 registers to the consumers (setmaxnreg)
 //     warps 0-7   two consumer warpgroups; tile i of the CTA belongs to warpgroup i & 1.  Main loop: wgmma m64n128k16 on
 //                 rows 0-63 and 64-127 of the tile, 6 per K step of 16 each (the accumulator, 128 fp32 per thread, lives in
 //                 registers), one wgmma group kept in flight.  A warpgroup starts its main loop when the other has issued
 //                 all of its own (an mbarrier hand-over per tile), then runs the epilogue (2^-s, +bias, leaky-ReLU, *sqrt2
 //                 -> split to fp16 hi/lo for the next layer, or fp32 for the last layer) through a swizzled shared-memory
 //                 staging box and TMA stores while the other warpgroup's MMAs run
-// smem: 3 stages x 64 KB (A_hi, A_lo, W_hi, W_lo: 16 KB each) with mbarrier full/empty pairs, + 2 x 16 KB staging.
+// smem: 3 stages x 64 KB (A_hi, A_lo, W_hi, W_lo: 16 KB each) with mbarrier full/empty pairs, + 2 x 16 KB staging, + one
+// tile slot per consumer warpgroup with its own full/empty mbarrier pair.
+// Tiles are claimed in order (n fastest) with an atomicAdd on a per-launch counter, one at a time as the producer issues the
+// last k-block of its current tile.  The launch shares the GPU with other streams (the RNG's launch groups take SMs as a
+// layer launch drains), and a CTA that starts late simply takes fewer tiles, where a static split (CTA b: tiles b, b + grid,
+// ...) would make the whole layer wait for its share.  Results do not depend on which CTA computes a tile.
 #include "tc_common.cuh"
 #include <stdlib.h>
 
@@ -44,7 +49,7 @@ constexpr uint32_t TC_STAGING_BYTES = 2 * 2 * TC_BOX_BYTES;     // per warpgroup
 // sub-partition's three warps fits its 16K registers (with 9 warps and no redistribution the cap is 168 and the 128-float
 // accumulator spills)
 constexpr int TC_THREADS = tc::CONSUMER_THREADS + 128;
-constexpr uint32_t TC_SMEM_BYTES = TC_STAGES * TC_STAGE_BYTES + TC_STAGING_BYTES + 64 /*barriers*/ + 1024 /*align slack*/;
+constexpr uint32_t TC_SMEM_BYTES = TC_STAGES * TC_STAGE_BYTES + TC_STAGING_BYTES + 128 /*barriers, tile slots*/ + 1024 /*align slack*/;
 static_assert(TC_SMEM_BYTES <= 232448, "mapping_layer_tc_kernel: shared memory exceeds the H100's 227 KB per block");
 
 struct TcParams {
@@ -53,6 +58,7 @@ struct TcParams {
     __half *out_lo;
     float *out_f32;         // fp32 output [M, N_total] (last layer)
     unsigned *overflow;     // set to 1 when an activation leaves fp16's range
+    unsigned *queue;        // tile claim counter, zeroed before the launch
     const float *inv_wscale;   // device pointer to 2^-s of this layer
     int M, N_total, K;
     int mode;               // 0: (acc 2^-s + bias) -> leaky-ReLU * sqrt2 (EqualLinear);  1: plain acc 2^-s (tc_gemm_plain);  2: acc 2^-s + bias
@@ -72,6 +78,9 @@ mapping_layer_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __gri
     uint64_t *full_bar = bars;                         // [TC_STAGES]
     uint64_t *empty_bar = bars + TC_STAGES;            // [TC_STAGES]: one arrival per warp of the consuming warpgroup
     uint64_t *turn_bar = bars + 2 * TC_STAGES;         // [2]: warpgroup wg may start its next main loop (arrivals: the other's warps)
+    uint64_t *tile_full = bars + 2 * TC_STAGES + 2;    // [2]: tile_slot[wg] holds warpgroup wg's next tile (arrival: the producer)
+    uint64_t *tile_empty = bars + 2 * TC_STAGES + 4;   // [2]: warpgroup wg has read tile_slot[wg] (arrivals: its warps)
+    volatile int *tile_slot = reinterpret_cast<volatile int *>(bars + 2 * TC_STAGES + 6);   // [2]: tile number, -1 = no more
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int num_m_tiles = (p.M + TC_BLOCK_M - 1) / TC_BLOCK_M;
@@ -79,13 +88,13 @@ mapping_layer_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __gri
     // clips stores (the 128/64/32-channel StyledConv blocks: N = 9 cout = 1152 / 576 / 288, K = cin down to 32)
     const int num_n_tiles = (p.N_total + TC_BLOCK_N - 1) / TC_BLOCK_N;
     const int num_k_blocks = (p.K + TC_BLOCK_K - 1) / TC_BLOCK_K;
-    // work unit = one 128 x 128 output tile, N fastest: neighbouring CTAs read the same A rows while they are in L2.  CTA b
-    // takes units b, b + grid, b + 2 grid, ...; its i-th unit belongs to consumer warpgroup i & 1.
+    // work unit = one 128 x 128 output tile, N fastest: neighbouring claims read the same A rows while they are in L2.  The
+    // CTA's i-th claimed unit belongs to consumer warpgroup i & 1.
     const int num_units = num_m_tiles * num_n_tiles;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < TC_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 4); }
-        mbar_init(&turn_bar[0], 4); mbar_init(&turn_bar[1], 4);
+        for (int w = 0; w < 2; ++w) { mbar_init(&turn_bar[w], 4); mbar_init(&tile_full[w], 1); mbar_init(&tile_empty[w], 4); }
         mbar_fence_init();
     }
     if (warp == PRODUCER_WARP && lane == 0) {
@@ -100,9 +109,25 @@ mapping_layer_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __gri
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
         if (warp == PRODUCER_WARP && lane == 0) {
             int stage = 0; uint32_t phase = 0;
-            for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
+            int u = (int)atomicAdd(p.queue, 1u);
+            for (int i = 0;; ++i) {
+                const int wg = i & 1;
+                mbar_wait(&tile_empty[wg], ((uint32_t)(i >> 1) & 1) ^ 1);   // warpgroup wg has taken its previous tile
+                if (u >= num_units) {                                      // no more tiles: tell both warpgroups
+                    tile_slot[wg] = -1;
+                    mbar_arrive(&tile_full[wg]);
+                    mbar_wait(&tile_empty[wg ^ 1], ((uint32_t)((i + 1) >> 1) & 1) ^ 1);
+                    tile_slot[wg ^ 1] = -1;
+                    mbar_arrive(&tile_full[wg ^ 1]);
+                    break;
+                }
+                tile_slot[wg] = u;
+                mbar_arrive(&tile_full[wg]);
                 const int m0 = (u / num_n_tiles) * TC_BLOCK_M, n0 = (u % num_n_tiles) * TC_BLOCK_N;
                 for (int kb = 0; kb < num_k_blocks; ++kb) {
+                    // the next tile is claimed with this one's last k-block: the atomic's round trip runs under the wait for a
+                    // free stage, and a CTA claims no more than one tile ahead of the loads it has issued
+                    if (kb == num_k_blocks - 1) u = (int)atomicAdd(p.queue, 1u);
                     mbar_wait(&empty_bar[stage], phase ^ 1);              // the warpgroup that consumed this stage has left it
                     uint8_t *st = smem + stage * TC_STAGE_BYTES;
                     mbar_arrive_expect_tx(&full_bar[stage], ((p.dbg & 4) ? 0u : 2 * TC_A_BYTES) + ((p.dbg & 2) ? 0u : 2 * TC_W_BYTES));
@@ -192,8 +217,11 @@ mapping_layer_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __gri
         // the CTA's i-th unit (i = 2 j + wg) is this warpgroup's j-th tile; the producer fills the ring with the CTA's k-blocks
         // in order, so k-block kb of unit i is the CTA's k-block i num_k_blocks + kb, which fixes its stage and phase
         for (int i = wg;; i += 2) {
-            const int u = blockIdx.x + i * gridDim.x;
-            if (u >= num_units) break;
+            mbar_wait(&tile_full[wg], (uint32_t)(i >> 1) & 1);
+            const int u = tile_slot[wg];
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&tile_empty[wg]);
+            if (u < 0) break;
             const int m0 = (u / num_n_tiles) * TC_BLOCK_M, n0 = (u % num_n_tiles) * TC_BLOCK_N;
             const int g0 = i * num_k_blocks;
             int stage = g0 % TC_STAGES, prev = stage;
@@ -354,8 +382,9 @@ static int tc_ensure_attr() {
 }
 
 // one launch of the layer kernel over all output tiles; A and W tensor maps must have been built with box rows 128
+// `queue`: one unsigned of device memory, zeroed here (stream-ordered), that no concurrent launch uses
 static int tc_launch_layer(const CUtensorMap &tm_ah, const CUtensorMap &tm_al, const CUtensorMap &tm_wh, const CUtensorMap &tm_wl,
-                           TcParams p, int leave_free_sms, cudaStream_t st) {
+                           TcParams p, unsigned *queue, int leave_free_sms, cudaStream_t st) {
     // output boxes of the epilogue's TMA stores (64 rows: one accumulator fragment, half of the tile): fp16 hi / lo [M, N]
     // (the next layer's A operand) or fp32 [M, N]
     CUtensorMap tm_o0, tm_o1;
@@ -377,9 +406,11 @@ static int tc_launch_layer(const CUtensorMap &tm_ah, const CUtensorMap &tm_al, c
         if (dbg < 0) { const char *e = getenv("GANSPACE_B200_MAPPING_DBG"); dbg = e ? atoi(e) : 0; }
         p.dbg = dbg;
     }
-    // work units: single 128 x 128 tiles, two consumer warpgroups per CTA -- a 70k-row chunk (2,188 tiles) on 100 CTAs wastes
-    // about 1 % in the last round
+    // work units: single 128 x 128 tiles, two consumer warpgroups per CTA
     const int64_t units = (int64_t)m_tiles * n_tiles;
+    GSB_CHECK_ARG(units < (1ll << 31) - 1024, "mapping_layer_tc: too many tiles");
+    GSB_CHECK_CUDA(cudaMemsetAsync(queue, 0, sizeof(unsigned), st));
+    p.queue = queue;
     const int grid = units < avail ? (int)units : avail;
     mapping_layer_tc_kernel<<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(tm_ah, tm_al, tm_wh, tm_wl, tm_o0, tm_o1, p);
     GSB_CHECK_LAUNCH();
@@ -391,8 +422,8 @@ static int tc_launch_layer(const CUtensorMap &tm_ah, const CUtensorMap &tm_al, c
 // unit zero-fills the operand boxes of a ragged last N or K tile and clips its stores).
 // Used by the modulated-convolution path (synthesis.cu): one dense contraction per 3x3 tap.
 int tc_gemm_plain(const __half *a_hi, const __half *a_lo, int64_t M, int K, const __half *w_hi, const __half *w_lo, int N,
-                  const float *inv_wscale, float *out, unsigned *overflow, int leave_free_sms, cudaStream_t st) {
-    GSB_CHECK_ARG(N % 32 == 0 && N >= 32 && K % 8 == 0 && K >= 8 && M > 0 && M < (1ll << 31),
+                  const float *inv_wscale, float *out, unsigned *overflow, unsigned *queue, int leave_free_sms, cudaStream_t st) {
+    GSB_CHECK_ARG(N % 32 == 0 && N >= 32 && K % 8 == 0 && K >= 8 && M > 0 && M < (1ll << 31) && queue,
                   "tc_gemm_plain: need N%%32==0, K%%8==0 (M=%lld N=%d K=%d)", (long long)M, N, K);
     if (int r = tc_ensure_attr()) return r;
     CUtensorMap tm_ah, tm_al, tm_wh, tm_wl;
@@ -403,13 +434,13 @@ int tc_gemm_plain(const __half *a_hi, const __half *a_lo, int64_t M, int K, cons
     TcParams p;
     p.bias = nullptr; p.out_hi = nullptr; p.out_lo = nullptr; p.out_f32 = out; p.overflow = overflow;
     p.inv_wscale = inv_wscale; p.M = (int)M; p.N_total = N; p.K = K; p.mode = 1;
-    return tc_launch_layer(tm_ah, tm_al, tm_wh, tm_wl, p, leave_free_sms, st);
+    return tc_launch_layer(tm_ah, tm_al, tm_wh, tm_wl, p, queue, leave_free_sms, st);
 }
 
 // y[n, N] = x[n, K] W[N, K]^T + bias (optionally sqrt2 * lrelu) on the tensor cores, fp32-grade (hi/lo split of both operands
 // done here: W per call -- N*K elements, negligible next to the n*N*K product for n >= 128).  N % 256 == 0, K % 64 == 0.
 // Used for BigGAN's generator.gen_z (biggan model.py:211-212,232): [B, 256] x [256, 32768].
-// ws layout: x_hi, x_lo [n*K] fp16 | w_hi, w_lo [N*K] fp16 | {inv_wscale, wscale, absmax} | overflow flag
+// ws layout: x_hi, x_lo [n*K] fp16 | w_hi, w_lo [N*K] fp16 | {inv_wscale, wscale, absmax} | overflow flag, tile queue
 size_t tc_linear_workspace_bytes(int64_t n, int N, int K) {
     return 2 * align_up((size_t)n * K * 2, 256) + 2 * align_up((size_t)N * K * 2, 256) + 512;
 }
@@ -440,10 +471,10 @@ int tc_linear(const float *x, const float *w, const float *bias, float *y, int64
     TcParams p;
     p.bias = bias; p.out_hi = nullptr; p.out_lo = nullptr; p.out_f32 = y; p.overflow = overflow;
     p.inv_wscale = scal; p.M = (int)n; p.N_total = N; p.K = K; p.mode = lrelu ? 0 : 2;
-    return tc_launch_layer(tm_ah, tm_al, tm_wh, tm_wl, p, 0, st);
+    return tc_launch_layer(tm_ah, tm_al, tm_wh, tm_wl, p, overflow + 1, 0, st);
 }
 
-// Full mapping network on the tensor cores.  ws: 4 fp16 buffers of n*dim (two hi/lo ping-pong pairs).
+// Full mapping network on the tensor cores.  ws: 4 fp16 buffers of n*dim (two hi/lo ping-pong pairs) + the tile queue.
 int mapping_forward_tc(const float *pb, void *tc_base, int n_layers, int dim,
                        const float *d_z, float *d_w, int64_t n, bool pixelnorm, void *ws, int leave_free_sms,
                        cudaStream_t st) {
@@ -453,6 +484,7 @@ int mapping_forward_tc(const float *pb, void *tc_base, int n_layers, int dim,
     const size_t buf = align_up((size_t)n * dim * 2, 256);
     __half *a_hi[2] = {reinterpret_cast<__half *>(ws), reinterpret_cast<__half *>((char *)ws + 2 * buf)};
     __half *a_lo[2] = {reinterpret_cast<__half *>((char *)ws + buf), reinterpret_cast<__half *>((char *)ws + 3 * buf)};
+    unsigned *queue = reinterpret_cast<unsigned *>((char *)ws + 4 * buf);
 
     if (int r = tc_ensure_attr()) return r;
     pixelnorm_split_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(d_z, a_hi[0], a_lo[0], n, dim, pixelnorm ? 1 : 0,
@@ -477,12 +509,12 @@ int mapping_forward_tc(const float *pb, void *tc_base, int n_layers, int dim,
         p.overflow = v.overflow;
         p.inv_wscale = v.inv_wscale + l;
         p.M = (int)n; p.N_total = dim; p.K = dim; p.mode = 0;
-        if (int r = tc_launch_layer(tm_ah, tm_al, tm_wh, tm_wl, p, leave_free_sms, st)) return r;
+        if (int r = tc_launch_layer(tm_ah, tm_al, tm_wh, tm_wl, p, queue, leave_free_sms, st)) return r;
     }
     return GSB_OK;
 }
 
-size_t mapping_tc_workspace_bytes(int64_t n, int dim) { return 4 * align_up((size_t)n * dim * 2, 256); }
+size_t mapping_tc_workspace_bytes(int64_t n, int dim) { return 4 * align_up((size_t)n * dim * 2, 256) + 256; }
 
 unsigned *mapping_tc_overflow_flag(void *tc_base, int n_layers, int dim) {
     return tc_pack_view(tc_base, n_layers, dim).overflow;

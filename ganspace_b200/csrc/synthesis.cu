@@ -382,6 +382,7 @@ struct SynthWs {
     float *s2;
     __half *act[2][2];     // [ping-pong][hi/lo]
     float *Y, *T;
+    unsigned *queue;        // tile queue of the tap GEMM launches
     float *rgb[2], *rgb_s, *rgb_modw;      // render path: skip images (ping-pong), ToRGB style, scaled modulation weight
     size_t bytes;
 };
@@ -415,6 +416,7 @@ static SynthWs synth_ws(void *base, const gsb_styled_conv *layers, int n_run, in
         for (int h = 0; h < 2; ++h) w.act[a][h] = (__half *)take(act_elems * 2);
     w.Y = (float *)take(y_elems * 4);
     w.T = (float *)take((t_elems ? t_elems : 64) * 4);
+    w.queue = (unsigned *)take(sizeof(unsigned));
     w.rgb[0] = w.rgb[1] = w.rgb_s = w.rgb_modw = nullptr;
     if (with_rgb) {
         const int ro = res_out_of(layers[n_run - 1]);
@@ -545,7 +547,7 @@ static int synthesis_run(const void *d_packed, const gsb_styled_conv *layers, in
             const int64_t nb = (b0 + spc <= n) ? spc : (n - b0);
             const int64_t rows = nb * hw_in;
             if (int r = tc_gemm_plain(w.act[src][0] + b0 * hw_in * c.cin, w.act[src][1] + b0 * hw_in * c.cin, rows, c.cin, v.L[l].w_hi,
-                                      v.L[l].w_lo, 9 * c.cout, v.L[l].scal, w.Y, v.overflow, 0, st)) return r;
+                                      v.L[l].w_lo, 9 * c.cout, v.L[l].scal, w.Y, v.overflow, w.queue, 0, st)) return r;
             EpiParams e;
             e.demod = w.D[l] + b0 * c.cout;
             e.noise = v.L[l].noise;

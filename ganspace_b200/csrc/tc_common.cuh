@@ -182,6 +182,6 @@ size_t tc_linear_workspace_bytes(int64_t n, int N, int K);
 int tc_linear(const float *x, const float *w, const float *bias, float *y, int64_t n, int N, int K, bool lrelu, void *ws,
               cudaStream_t st);
 int tc_gemm_plain(const __half *a_hi, const __half *a_lo, int64_t M, int K, const __half *w_hi, const __half *w_lo, int N,
-                  const float *inv_wscale, float *out, unsigned *overflow, int leave_free_sms, cudaStream_t st);
+                  const float *inv_wscale, float *out, unsigned *overflow, unsigned *queue, int leave_free_sms, cudaStream_t st);
 
 }  // namespace gsb
