@@ -11,11 +11,11 @@
 //        T = M M^T  (n_s x n_s, n_s = c + n_b + 1 ~ 2100; fp32 products summed in fp32 over 8192-long chunks of d,
 //                    chunks accumulated in fp64)
 //        T = U diag(lambda) U^T  (top c; fp64 direct solver: L2-resident Householder tridiagonalisation, bisection,
-//                    inverse iteration (ipca.cu))
+//                    inverse iteration (eig.cu))
 //        S_new = sqrt(lambda),   (S * Vt)_new = U^T M      (one skinny GEMM over M; rows 0..c-1 of M for the next step)
 // followed by sklearn's svd_flip sign rule on the rows and the Chan mean / variance merge per feature
 // (extmath._incremental_mean_and_var).  Nothing of size d x d or n_b x d ever leaves the device.
-#include "ipca_internal.cuh"
+#include "eig.cuh"
 #include "tc_common.cuh"
 #include <math.h>
 
@@ -37,8 +37,8 @@ static BigState big_state(void *p, int64_t d, int c) {
 }
 
 struct BigWs {
-    Workspace ew;          // ew.A doubles as T
-    double *mean_b, *U, *lam;
+    Workspace ew;          // ew.A doubles as T; ew.evecs (U) and ew.lam carry the solve over to the commit
+    double *mean_b;
     float *Dnew, *rowmax;
     void *tc;              // operands of the tensor-core Gram (flags & GSB_BIGD_GRAM_TC)
     size_t bytes;
@@ -52,8 +52,6 @@ static BigWs big_ws(void *base, int64_t d, int c, int nb_max, int flags) {
     const size_t eb = carve(nullptr, np, c).bytes;
     w.ew = carve(take(eb), np, c);
     w.mean_b = (double *)take((size_t)d * 8);
-    w.U = (double *)take((size_t)c * np * 8);
-    w.lam = (double *)take((size_t)c * 8);
     w.Dnew = (float *)take((size_t)c * d * 4);
     w.rowmax = (float *)take((size_t)2 * c * 4);
     w.tc = ((flags & GSB_BIGD_GRAM_TC) && gram_tc_supported(d)) ? take(gram_tc_workspace_bytes(np, d)) : nullptr;
@@ -259,20 +257,12 @@ bigd_rowmax_kernel(const float *__restrict__ Dnew, int64_t d, float *__restrict_
         const float v = row[i], av = fabsf(v);
         if (av > best) { best = av; bval = v; bi = i; }
     }
-    for (int o = 16; o > 0; o >>= 1) {
-        const float ob = __shfl_xor_sync(0xffffffffu, best, o), ov = __shfl_xor_sync(0xffffffffu, bval, o);
-        const long long oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ob > best || (ob == best && oi < bi)) { best = ob; bval = ov; bi = oi; }
-    }
+    warp_argmax_abs(best, bi, bval);
     if (lane == 0) { s_best[warp] = best; s_val[warp] = bval; s_idx[warp] = bi; }
     __syncthreads();
     if (warp == 0) {
         best = s_best[lane]; bval = s_val[lane]; bi = s_idx[lane];
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o), ov = __shfl_xor_sync(0xffffffffu, bval, o);
-            const long long oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (ob > best || (ob == best && oi < bi)) { best = ob; bval = ov; bi = oi; }
-        }
+        warp_argmax_abs(best, bi, bval);
         if (lane == 0) { rowmax[2 * t] = best; rowmax[2 * t + 1] = bval; }
     }
 }
@@ -398,8 +388,8 @@ extern "C" int gsb_bigd_step_solve(void *d_state, float *d_M, int64_t d, int c, 
     using namespace gsb;
     StepCtx x;
     if (int r = step_ctx(x, d_state, d_M, d, c, nb_max, n_seen, nb, flags, d_workspace, workspace_bytes, stream)) return r;
-    if (int r = eig_top(x.w.ew, x.np, c, x.w.lam, x.w.U, x.st)) return r;      // ew.A holds T (and is destroyed)
-    bigd_project_kernel<<<(unsigned)((d + PJ_COLS - 1) / PJ_COLS), 256, 0, x.st>>>(x.w.U, x.np, d_M, x.n_rows, d, c, x.w.Dnew);
+    if (int r = eig_top(x.w.ew, x.np, c, x.w.ew.lam, x.w.ew.evecs, x.st)) return r;      // ew.A holds T (and is destroyed)
+    bigd_project_kernel<<<(unsigned)((d + PJ_COLS - 1) / PJ_COLS), 256, 0, x.st>>>(x.w.ew.evecs, x.np, d_M, x.n_rows, d, c, x.w.Dnew);
     GSB_CHECK_LAUNCH();
     bigd_rowmax_kernel<<<c, 1024, 0, x.st>>>(x.w.Dnew, d, x.w.rowmax);
     GSB_CHECK_LAUNCH();
@@ -413,7 +403,7 @@ extern "C" int gsb_bigd_step_commit(void *d_state, float *d_M, int64_t d, int c,
     using namespace gsb;
     StepCtx x;
     if (int r = step_ctx(x, d_state, d_M, d, c, nb_max, n_seen, nb, flags, d_workspace, workspace_bytes, stream)) return r;
-    bigd_commit_kernel<<<c, 1024, 0, x.st>>>(x.w.Dnew, d, x.w.lam, x.w.rowmax, d_signs, d_M, x.s.S, x.s.hdr, (double)(n_seen + nb));
+    bigd_commit_kernel<<<c, 1024, 0, x.st>>>(x.w.Dnew, d, x.w.ew.lam, x.w.rowmax, d_signs, d_M, x.s.S, x.s.hdr, (double)(n_seen + nb));
     GSB_CHECK_LAUNCH();
     return GSB_OK;
 }

@@ -54,6 +54,23 @@ __device__ __forceinline__ double block_sum(double v, double *red) {
     return t;
 }
 
+// Warp-wide argmax of |x| (svd_flip's sign rule): each lane holds a candidate (best = |x|, idx, val = x); every lane gets
+// the winner.  Ties go to the lower index, as np.argmax's first occurrence.
+template <class T, class I>
+__device__ __forceinline__ void warp_argmax_abs(T &best, I &idx, T &val) {
+    for (int o = 16; o > 0; o >>= 1) {
+        const T ob = __shfl_xor_sync(0xffffffffu, best, o), ov = __shfl_xor_sync(0xffffffffu, val, o);
+        const I oi = __shfl_xor_sync(0xffffffffu, idx, o);
+        if (ob > best || (ob == best && oi < idx)) { best = ob; idx = oi; val = ov; }
+    }
+}
+
 int num_sms();
+
+// Raises `kernel`'s dynamic shared-memory limit to `bytes` unless an earlier call already set at least that much (the
+// largest size set so far is remembered per kernel, process-wide).
+int raise_dyn_smem(const void *kernel, size_t bytes);
+template <class F>
+int raise_dyn_smem(F *kernel, size_t bytes) { return raise_dyn_smem(reinterpret_cast<const void *>(kernel), bytes); }
 
 }  // namespace gsb

@@ -1,6 +1,8 @@
 // Error reporting, device queries and tensor-map encoding shared by all entry points.
 #include "tc_common.cuh"
 #include <stdarg.h>
+#include <mutex>
+#include <unordered_map>
 
 namespace gsb {
 
@@ -22,6 +24,18 @@ int num_sms() {
             sms = 132;
     }
     return sms;
+}
+
+int raise_dyn_smem(const void *kernel, size_t bytes) {
+    static std::mutex mu;
+    static std::unordered_map<const void *, size_t> largest;
+    std::lock_guard<std::mutex> lock(mu);
+    size_t &set = largest[kernel];
+    if (bytes > set) {
+        GSB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+        set = bytes;
+    }
+    return GSB_OK;
 }
 
 // cuTensorMapEncodeTiled through the runtime's driver entry point, so that the library does not link libcuda

@@ -218,14 +218,8 @@ row_split_kernel(const float *__restrict__ M, int64_t d, int n_rows, const int *
 int gram_tc_launch(GramEpilogue epi, const __half *hi, const __half *lo, int64_t k, int64_t k_pitch, int n_groups, int n_pad,
                    int n_rows, const int *exps, double *out, cudaStream_t st) {
     using namespace gtc;
-    static bool attr_set = false;
-    if (!attr_set) {
-        GSB_CHECK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<GramEpilogue::Store>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                            (int)SMEM_BYTES));
-        GSB_CHECK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<GramEpilogue::Accumulate>,
-                                            cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-        attr_set = true;
-    }
+    if (int r = raise_dyn_smem(gram_tc_kernel<GramEpilogue::Store>, SMEM_BYTES)) return r;
+    if (int r = raise_dyn_smem(gram_tc_kernel<GramEpilogue::Accumulate>, SMEM_BYTES)) return r;
     CUtensorMap tm_hi, tm_lo;
     const uint64_t dims[3] = {(uint64_t)k, (uint64_t)n_pad, (uint64_t)n_groups};
     const uint64_t strides[2] = {(uint64_t)k_pitch * 2, (uint64_t)n_pad * k_pitch * 2};

@@ -1,21 +1,9 @@
-// Internal interfaces of the fp64 symmetric eigensolver (ipca.cu), shared with the large-d engine (bigd.cu).
+// Internal interfaces of the small-d chain, shared by ipca.cu and subspace.cu.
 #pragma once
-#include "common.cuh"
+#include "eig.cuh"
 
 namespace gsb {
 
-struct Workspace {
-    double *A, *dg, *e, *beta, *Vh, *lam, *Z, *lu, *xch, *evecs, *qx;
-    unsigned *counter;
-    unsigned char *swp;
-    size_t bytes;
-};
-Workspace carve(void *base, int d, int c);
-// top-c eigenpairs (descending) of the symmetric matrix held in w.A (destroyed); evecs rows are sign-normalised
-int eig_top(const Workspace &w, int d, int c, double *evals, double *evecs, cudaStream_t st);
-
-// svd_flip sign rule on the rows of V[c,d]
-int sign_rows(double *V, int c, int d, cudaStream_t st);
 // sticky device-side status word of the chain kernels (bit1: a subspace step hit its iteration cap)
 int *eig_status_device_ptr();
 

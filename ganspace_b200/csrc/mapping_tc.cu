@@ -372,15 +372,6 @@ int mapping_tc_pack(const float *pw, int n_layers, int dim, void *tc_base, cudaS
     return GSB_OK;
 }
 
-static int tc_ensure_attr() {
-    static bool attr_set = false;
-    if (!attr_set) {
-        GSB_CHECK_CUDA(cudaFuncSetAttribute(mapping_layer_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_BYTES));
-        attr_set = true;
-    }
-    return GSB_OK;
-}
-
 // one launch of the layer kernel over all output tiles; A and W tensor maps must have been built with box rows 128
 // `queue`: one unsigned of device memory, zeroed here (stream-ordered), that no concurrent launch uses
 static int tc_launch_layer(const CUtensorMap &tm_ah, const CUtensorMap &tm_al, const CUtensorMap &tm_wh, const CUtensorMap &tm_wl,
@@ -425,7 +416,7 @@ int tc_gemm_plain(const __half *a_hi, const __half *a_lo, int64_t M, int K, cons
                   const float *inv_wscale, float *out, unsigned *overflow, unsigned *queue, int leave_free_sms, cudaStream_t st) {
     GSB_CHECK_ARG(N % 32 == 0 && N >= 32 && K % 8 == 0 && K >= 8 && M > 0 && M < (1ll << 31) && queue,
                   "tc_gemm_plain: need N%%32==0, K%%8==0 (M=%lld N=%d K=%d)", (long long)M, N, K);
-    if (int r = tc_ensure_attr()) return r;
+    if (int r = raise_dyn_smem(mapping_layer_tc_kernel, TC_SMEM_BYTES)) return r;
     CUtensorMap tm_ah, tm_al, tm_wh, tm_wl;
     if (int r = make_tmap(&tm_ah, a_hi, (uint64_t)M, (uint64_t)K, TC_BLOCK_M)) return r;
     if (int r = make_tmap(&tm_al, a_lo, (uint64_t)M, (uint64_t)K, TC_BLOCK_M)) return r;
@@ -448,7 +439,7 @@ size_t tc_linear_workspace_bytes(int64_t n, int N, int K) {
 int tc_linear(const float *x, const float *w, const float *bias, float *y, int64_t n, int N, int K, bool lrelu, void *ws,
               cudaStream_t st) {
     GSB_CHECK_ARG(N % 256 == 0 && K % TC_BLOCK_K == 0 && n > 0 && n < (1ll << 31) && bias, "tc_linear: need N%%256==0, K%%64==0, bias");
-    if (int r = tc_ensure_attr()) return r;
+    if (int r = raise_dyn_smem(mapping_layer_tc_kernel, TC_SMEM_BYTES)) return r;
     char *p0 = reinterpret_cast<char *>(ws);
     const size_t xb = align_up((size_t)n * K * 2, 256), wb = align_up((size_t)N * K * 2, 256);
     __half *x_hi = (__half *)p0, *x_lo = (__half *)(p0 + xb), *w_hi = (__half *)(p0 + 2 * xb), *w_lo = (__half *)(p0 + 2 * xb + wb);
@@ -486,7 +477,7 @@ int mapping_forward_tc(const float *pb, void *tc_base, int n_layers, int dim,
     __half *a_lo[2] = {reinterpret_cast<__half *>((char *)ws + buf), reinterpret_cast<__half *>((char *)ws + 3 * buf)};
     unsigned *queue = reinterpret_cast<unsigned *>((char *)ws + 4 * buf);
 
-    if (int r = tc_ensure_attr()) return r;
+    if (int r = raise_dyn_smem(mapping_layer_tc_kernel, TC_SMEM_BYTES)) return r;
     pixelnorm_split_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(d_z, a_hi[0], a_lo[0], n, dim, pixelnorm ? 1 : 0,
                                                                   v.overflow);
     GSB_CHECK_LAUNCH();

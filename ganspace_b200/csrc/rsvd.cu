@@ -12,7 +12,7 @@
 //
 // Products are fp64 on the tensor cores (mma.sync m8n8k4, as subspace.cu); the range basis is orthonormalised by CholQR2
 // between the products.  Everything is deterministic: no atomics on values, fixed reduction orders.
-#include "ipca_internal.cuh"
+#include "eig.cuh"
 #include <math.h>
 
 namespace gsb {
@@ -43,8 +43,8 @@ FbState fb_state(void *base, int d) {
 int lpad(int l) { return (l + 31) / 32 * 32; }
 
 struct FbWs {
-    double *G, *Y, *P, *Sm, *evals, *evecs, *comp, *T;
-    Workspace eig;
+    double *G, *Y, *P, *Sm, *comp, *T;
+    Workspace eig;         // eig.lam / eig.evecs: the eigenpairs of F^T F
     size_t bytes;
 };
 
@@ -58,8 +58,6 @@ FbWs fb_carve(void *base, int d, int c, int l) {
     w.Y = (double *)take((size_t)d * lp * 8);
     w.P = (double *)take((size_t)d * lp * 8);
     w.Sm = (double *)take((size_t)lp * lp * 8);
-    w.evals = (double *)take((size_t)c * 8);
-    w.evecs = (double *)take((size_t)c * de * 8);
     w.comp = (double *)take((size_t)c * d * 8);
     w.T = (double *)take((size_t)d * c * 8);
     const size_t eig_off = off;
@@ -365,7 +363,7 @@ extern "C" int gsb_fbpca_solve(void *d_state, int d, int c, int l, int flags, co
         // exact branch: the top-c right singular vectors of X are the top-c eigenvectors of G
         fb_form_g_kernel<<<gd, 128, 0, st>>>(w.eig.A, s.S, s.mean, s.hdr, d, flags & GSB_FBPCA_RAW);
         GSB_CHECK_LAUNCH();
-        if (int r = eig_top(w.eig, d, c, w.evals, w.comp, st)) return r;
+        if (int r = eig_top(w.eig, d, c, w.eig.lam, w.comp, st)) return r;
     } else {
         GSB_CHECK_CUDA(cudaMemsetAsync(w.Y, 0, (size_t)d * lp * 8, st));
         GSB_CHECK_CUDA(cudaMemsetAsync(w.P, 0, (size_t)d * lp * 8, st));
@@ -395,11 +393,11 @@ extern "C" int gsb_fbpca_solve(void *d_state, int d, int c, int l, int flags, co
         if (int r = fb_trsm_rows(w.P, d, l, lp, w.Sm, lp, s.status, st)) return r;
         // F^T F (lp x lp, zero-padded so that the eigensolver sees a multiple of 32) -> top-c (s^2, W)
         if (int r = fb_gemm<true, false>(lp, lp, d, w.P, lp, w.P, lp, w.eig.A, lp, st)) return r;
-        if (int r = eig_top(w.eig, lp, c, w.evals, w.evecs, st)) return r;
+        if (int r = eig_top(w.eig, lp, c, w.eig.lam, w.eig.evecs, st)) return r;
         // Va = diag(1/s) W^T F^T  [c, d]
-        fb_scale_rows_kernel<<<c, 128, 0, st>>>(w.evecs, c, lp, w.evals);
+        fb_scale_rows_kernel<<<c, 128, 0, st>>>(w.eig.evecs, c, lp, w.eig.lam);
         GSB_CHECK_LAUNCH();
-        if (int r = fb_gemm<false, true>(c, d, lp, w.evecs, lp, w.P, lp, w.comp, d, st)) return r;
+        if (int r = fb_gemm<false, true>(c, d, lp, w.eig.evecs, lp, w.P, lp, w.comp, d, st)) return r;
     }
     // stdevs from the centred scatter, sort, sign rule (largest-|.| entry of each row positive)
     if (int r = fb_gemm<false, true>(d, c, d, s.S, d, w.comp, d, w.T, c, st)) return r;

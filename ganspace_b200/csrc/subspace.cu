@@ -697,16 +697,12 @@ int subspace_step(double *hdr, double *mean, double *unnorm, double *H, double *
     const size_t smem = subspace_smem_bytes(d, c);
     const bool small = (c <= 80 && c + d / SC_CL <= 112);   // register tile of the Cholesky: 7 x 5 or 10 x 8 per thread
     auto kern = small ? subspace_step_kernel<7, 5> : subspace_step_kernel<10, 8>;
-    static size_t smem_set[2] = {0, 0};
     static bool cluster_set[2] = {false, false};
     if (!cluster_set[small]) {
         GSB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
         cluster_set[small] = true;
     }
-    if (smem > smem_set[small]) {
-        GSB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        smem_set[small] = smem;
-    }
+    if (int r = raise_dyn_smem(kern, smem)) return r;
     SubspaceParams p;
     p.hdr = hdr; p.mean = mean; p.unnorm = unnorm; p.H = H; p.Qbuf = Qbuf;
     p.mean_b = mean_b; p.gram_b = gram_b;

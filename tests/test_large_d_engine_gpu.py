@@ -1,4 +1,4 @@
-"""The large-d IPCA engine (csrc/bigd.cu, the small-side eigensolver ``eig_top`` in csrc/ipca.cu and the tensor-core Gram in
+"""The large-d IPCA engine (csrc/bigd.cu, the small-side eigensolver ``eig_top`` in csrc/eig.cu and the tensor-core Gram in
 csrc/gram_tc.cu) against the fp64 restatement of sklearn's IncrementalPCA.partial_fit, at shapes up to config 5's small side
 (c = 80, b = 2000: 2081 rows padded to 2112) and at the 4096-row cap, for every tridiagonalisation branch of ``eig_top``.
 
@@ -20,10 +20,10 @@ RATIO_TOL = 1e-3
 TIGHT = dict(cos=1e-5, sv=2e-5, ev=4e-5, ratio=1e-6)      # 1 - cos, rtol, rtol, absolute
 N_TIGHT_POWER = 20     # leading components of the "power" spectrum held to the tight bars
 
-# np = roundup32(c + nb + 1) decides the eigensolver branch of eig_top (csrc/ipca.cu):
+# np = roundup32(c + nb + 1) decides the eigensolver branch of eig_top (csrc/eig.cu):
 #   np <= 512: tridiag_reg_kernel (256 threads for np <= 256); 512 < np <= 640 (the 16-CTA cluster's column blocks fit
-#   227 KiB): tridiag_kernel<true>; np <= 1024: tridiag_kernel<false> with P = np/8 CTAs (halved above 128);
-#   np > 1024: tridiag_l2_kernel.  Back-transform: <4> for np <= 128, <8> <= 256, <16> <= 512, <32> <= 1024, then
+#   227 KiB): tridiag_kernel<Cols::Cluster>; np <= 1024: tridiag_kernel<Cols::Grid> with P = np/8 CTAs;
+#   np > 1024: tridiag_kernel<Cols::L2>.  Back-transform: <4> for np <= 128, <8> <= 256, <16> <= 512, <32> <= 1024, then
 #   backtransform_big_kernel.  The branch of each case below was also seen in torch.profiler traces of its first step; the
 #   profiler drops kernel records now and then, so the suite does not assert on them.
 CASES = {
@@ -32,11 +32,11 @@ CASES = {
     "A":  (8,   100,  1040,   5),     # 128   tridiag_reg_kernel (256 threads), <4>; d % 64 != 0: the tc Gram falls back to FMA
     "B":  (16,  239,  2048,   5),     # 256   tridiag_reg_kernel (256 threads), <8>; n_rows = 2 x 128
     "C":  (24,  300,  18496,  4),     # 352   tridiag_reg_kernel, <16>; d = 289 x 64: ragged K-chunks in both Gram kernels
-    "D":  (80,  559,  8192,   4),     # 640   tridiag_kernel<true> (cluster, 230,912 B of shared memory), <32>
-    "D2": (80,  591,  8192,   4),     # 672   tridiag_kernel<false> (grid barrier, P = 84), <32>
-    "E":  (80,  900,  8192,   4),     # 992   tridiag_kernel<false> (grid barrier, P = 124), <32>
-    "F":  (80,  2000, 8192,   25),    # 2112  tridiag_l2_kernel, backtransform_big_kernel; config 5's c, b and np
-    "G":  (128, 3967, 4096,   2),     # 4096  tridiag_l2_kernel, backtransform_big_kernel; the cap, c = PJ_CMAX
+    "D":  (80,  559,  8192,   4),     # 640   tridiag_kernel<Cols::Cluster> (230,912 B of shared memory), <32>
+    "D2": (80,  591,  8192,   4),     # 672   tridiag_kernel<Cols::Grid> (P = 84), <32>
+    "E":  (80,  900,  8192,   4),     # 992   tridiag_kernel<Cols::Grid> (P = 124), <32>
+    "F":  (80,  2000, 8192,   25),    # 2112  tridiag_kernel<Cols::L2>, backtransform_big_kernel; config 5's c, b and np
+    "G":  (128, 3967, 4096,   2),     # 4096  tridiag_kernel<Cols::L2>, backtransform_big_kernel; the cap, c = PJ_CMAX
 }
 # case F's basis has components whose largest entry lies in the last quarter of the features and whose largest entry in the
 # first quarter has the opposite sign, so a feature-sharded step must overrule shard 0's own svd_flip choice for them
