@@ -519,9 +519,7 @@ class IPCAChain:
                        "gsb_ipca_chain_step")
         # kernels per step: first step = direct solve (8) + seeding of the subspace form (1); later steps = one cluster
         # launch (orthogonal iteration, csrc/subspace.cu).  Shapes outside the subspace kernel's range: direct solve (8).
-        subspace = (self.d % 128 == 0 and 128 <= self.d <= 512 and self.c % 8 == 0 and 8 <= self.c <= 128
-                    and os.environ.get("GANSPACE_B200_CHAIN", "") != "direct" and not _chain_forced_direct)
-        instrument.count((1 if self.n_seen > 0 else 9) if subspace else 8)
+        instrument.count((1 if self.n_seen > 0 else 9) if chain_iterates(self.d, self.c) else 8)
         self.n_seen += int(n_batch)
 
     def join(self):
@@ -548,6 +546,20 @@ class IPCAChain:
             check_eig_status("IPCAChain.export")
         instrument.count(1)
         return out
+
+
+def chain_iterates(d: int, c: int) -> bool:
+    """Whether chain steps after the first enqueued now run the orthogonal iteration of csrc/subspace.cu rather than the direct
+    solve.  The library reserves (H, Q) and an export workspace in the state exactly then, so the state is larger than its eigen
+    form: header, mean, unnormalised variance, S and V (csrc/ipca.cu, ``state_view``), in fp64 and rounded up to 256 bytes."""
+    key = (int(d), int(c), _chain_forced_direct)      # GANSPACE_B200_CHAIN is read once by the library
+    if key not in _chain_iterates:
+        eigen_form = (8 * (24 + 2 * d + c + c * d) + 255) // 256 * 256
+        _chain_iterates[key] = load().gsb_ipca_state_bytes(d, c) > eigen_form
+    return _chain_iterates[key]
+
+
+_chain_iterates = {}
 
 
 class ChainNotConverged(NativeError):

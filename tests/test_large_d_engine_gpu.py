@@ -12,6 +12,7 @@ import time
 import numpy as np
 import pytest
 import torch
+from ipca_rows import Data
 
 pytestmark = pytest.mark.gpu
 
@@ -43,43 +44,10 @@ CASES = {
 F_SPIKES = (2, 5, 9)
 
 
-class _Data:
-    """Batches with a known spectrum ("gapped": sigma_k^2 = 0.97^k; "power": sigma_k^2 = 1/(k+1)), generated on the host
-    from fixed RandomState seeds so that the engine and the oracle see the same fp32 rows; batch i depends on (seed, i)."""
-
-    def __init__(self, d, c, nb, spectrum, seed, spikes=()):
-        rng = np.random.RandomState(seed)
-        self.d, self.seed, self.r = d, seed, c + 16
-        k = np.arange(self.r, dtype=np.float64)
-        self.sig2 = 0.97 ** k if spectrum == "gapped" else 1.0 / (k + 1.0)
-        G = rng.standard_normal((d, self.r)) / np.sqrt(d)
-        for i, col in enumerate(spikes):
-            G[d - 1 - 97 * i, col] = 0.25                 # global maximum: last feature quarter
-            G[11 + 97 * i, col] = -0.15                   # shard 0's maximum, opposite sign
-        self.B = np.linalg.qr(G)[0]
-        u = rng.standard_normal(d)
-        u -= self.B @ (self.B.T @ u)
-        self.u = u / np.linalg.norm(u)
-        self.shift = 2.0 * rng.standard_normal(d)
-        # a batch's noise eigenvalues (Marchenko-Pastur edge nu^2 (sqrt d + sqrt nb)^2) 10x below nb sigma_{r-1}^2
-        self.nu = np.sqrt(0.1 * self.sig2[-1] * nb / (np.sqrt(d) + np.sqrt(nb)) ** 2)
-        self.delta = np.sqrt(1.5 * self.sig2[0])
-
-    def batch(self, i, nb):
-        rng = np.random.RandomState([self.seed, i])
-        Z = rng.standard_normal((nb, self.r))
-        Z -= Z.mean(axis=0)
-        Z = np.linalg.qr(Z)[0] * np.sqrt(nb)              # centred, Z^T Z = nb I
-        X = (Z * np.sqrt(self.sig2)) @ self.B.T
-        X += self.nu * rng.standard_normal((nb, self.d))
-        X += self.shift + (1.0 if i % 2 == 0 else -1.0) * self.delta * self.u
-        return X.astype(np.float32)
-
-
 def _case_data(case, spectrum):
     c, nb, d = CASES[case][:3]
-    return _Data(d, c, nb, spectrum, seed=1000 + d + nb + (7 if spectrum == "power" else 0),
-                 spikes=F_SPIKES if case == "F" else ())
+    return Data(d, c, nb, spectrum, seed=1000 + d + nb + (7 if spectrum == "power" else 0),
+                spikes=F_SPIKES if case == "F" else ())
 
 
 def _oracle_state(st):
@@ -241,7 +209,7 @@ def test_batch_size_changes_public_api(oracle, monkeypatch, gram):
     from ganspace_b200.estimators import get_estimator
     monkeypatch.setenv("GANSPACE_B200_BIGD_GRAM", gram)
     d, c = 4096, 16
-    data = _Data(d, c, 700, "gapped", seed=77)
+    data = Data(d, c, 700, "gapped", seed=77)
     est = get_estimator("ipca", c, 1.0)
     st = oracle.IPCAState(c)
     worst = {}
