@@ -65,6 +65,11 @@ SIGNATURES = {
     "gsb_synthesis_status": (_I, [_P, _P, _I, _I, _P]),
     "gsb_synthesis_render_workspace_bytes": (_Z, [_P, _I, _L, _I]),
     "gsb_synthesis_render": (_I, [_P, _P, _I, _I, _I, _P, _I, _P, _I, _L, _P, _L, _P, _P, _Z, _P]),
+    "gsb_progan_packed_bytes": (_Z, [_P, _I]),
+    "gsb_progan_pack": (_I, [_P, _I, _P, _P, _P, _Z, _P]),
+    "gsb_progan_workspace_bytes": (_Z, [_P, _I, _L]),
+    "gsb_progan_forward": (_I, [_P, _P, _I, _I, _P, _L, _P, _L, _P, _P, _Z, _P]),
+    "gsb_progan_status": (_I, [_P, _P, _I, _P]),
     "gsb_bigd_rows": (_I, [_I, _I]),
     "gsb_bigd_state_bytes": (_Z, [_L, _I]),
     "gsb_bigd_workspace_bytes": (_Z, [_L, _I, _I, _I]),
@@ -96,6 +101,12 @@ class ToRGBDesc(C.Structure):
     """``gsb_to_rgb`` of include/ganspace_b200.h."""
     _fields_ = [("conv_weight", C.c_void_p), ("mod_weight", C.c_void_p), ("mod_bias", C.c_void_p), ("bias", C.c_void_p),
                 ("cin", C.c_int)]
+
+
+class ProGANBlockDesc(C.Structure):
+    """``gsb_progan_block`` of include/ganspace_b200.h."""
+    _fields_ = [("conv_weight", C.c_void_p), ("bias", C.c_void_p), ("cin", C.c_int), ("cout", C.c_int), ("upsample", C.c_int),
+                ("res_in", C.c_int), ("ksize", C.c_int)]
 
 
 class NativeError(RuntimeError):
@@ -218,6 +229,7 @@ SECTION_KERNELS = {
     "mapping": "mapping MLP: pixelnorm_split + 8 x mapping_layer_tc_kernel (wgmma, fp16 hi/lo x3)",
     "linear": "gen_z linear: mapping_layer_tc_kernel (wgmma, fp16 hi/lo x3, bias epilogue, TMA store) for n >= 128",
     "synthesis": "StyledConv chain: tap-GEMM tc_gemm_plain (wgmma) + gather/scatter/blur epilogues",
+    "progan": "ProGAN chain: tap-GEMM tc_gemm_plain (wgmma) + pg_gather_kernel (gather, bias, leaky-ReLU, PixelNorm, RGB)",
 }
 
 
@@ -793,6 +805,81 @@ class PackedSynthesis:
                    "gsb_synthesis_status")
         if flags.value & 1:
             raise NativeError("synthesis: an operand exceeded fp16 range in the tensor-core path; results are invalid")
+
+
+class PackedProGAN:
+    """ProGAN blocks layer1 .. layerK and the RGB output block packed for the tap-GEMM kernels (gsb_progan_pack).
+
+    ``blocks``: dicts with conv_weight [co,ci,k,k], bias [co] (fp32 tensors) and upsample (bool), in execution order;
+    ``out_weight`` [3,c,1,1] / ``out_bias`` [3]: the output block."""
+
+    def __init__(self, blocks, out_weight: torch.Tensor, out_bias: torch.Tensor):
+        lib = load()
+        self.device = require_cuda(out_weight.device)
+        self.n_blocks = len(blocks)
+        self.desc = (ProGANBlockDesc * self.n_blocks)()
+        self.shapes = []                        # (res_out, cout) per block
+        f32 = lambda t: t.detach().to(self.device, torch.float32).contiguous()
+        keep, res = [], 1
+        for i, L in enumerate(blocks):
+            w, b = f32(L["conv_weight"]), f32(L["bias"])
+            keep += [w, b]
+            co, ci, k = w.shape[0], w.shape[1], w.shape[2]
+            assert w.shape == (co, ci, k, k) and b.shape == (co,) and k == (4 if i == 0 else 3)
+            d = self.desc[i]
+            d.conv_weight, d.bias = w.data_ptr(), b.data_ptr()
+            d.cin, d.cout, d.upsample, d.res_in, d.ksize = ci, co, int(bool(L["upsample"])), res, k
+            res = 4 if i == 0 else (2 * res if L["upsample"] else res)
+            self.shapes.append((res, co))
+        self.z_dim = int(self.desc[0].cin)
+        ow, ob = f32(out_weight).reshape(3, -1), f32(out_bias).reshape(3)
+        assert ow.shape[1] == self.shapes[-1][1]
+        nbytes = lib.gsb_progan_packed_bytes(self.desc, self.n_blocks)
+        if nbytes == 0:
+            raise NativeError(f"gsb_progan_packed_bytes: {lib.gsb_last_error().decode()}")
+        self.packed = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            _check(lib.gsb_progan_pack(self.desc, self.n_blocks, _ptr(ow), _ptr(ob), _ptr(self.packed), self.packed.numel(),
+                                       _stream()), "gsb_progan_pack")
+            torch.cuda.current_stream().synchronize()      # the fp32 copies in `keep` may be freed after this returns
+
+    def out_dims(self, n_run: int) -> int:
+        r, co = self.shapes[n_run - 1]
+        return r * r * co
+
+    def forward(self, z: torch.Tensor, n_run: int, out: torch.Tensor = None, want_act: bool = True, want_rgb: bool = False):
+        """Blocks 0 .. n_run-1 on z [n, z_dim].  Returns (activation of block n_run-1 as fp32 NHWC rows [n, res*res*cout] or None,
+        image as fp32 NHWC [n, res, res, 3] or None; the image needs n_run == n_blocks).  ``out`` may be a row-strided 2-D view,
+        e.g. the batch rows of the large-d IPCA buffer."""
+        lib = load()
+        assert z.is_cuda and z.dtype == torch.float32 and z.dim() == 2 and z.shape[1] == self.z_dim
+        z = z.contiguous()
+        n, d = z.shape[0], self.out_dims(n_run)
+        act = rgb = None
+        if want_act:
+            act = torch.empty((n, d), dtype=torch.float32, device=z.device) if out is None else out
+            assert act.is_cuda and act.dtype == torch.float32 and act.shape == (n, d) and act.stride(1) == 1
+        if want_rgb:
+            res = self.shapes[-1][0]
+            rgb = torch.empty((n, res, res, 3), dtype=torch.float32, device=z.device)
+        if n == 0:
+            return act, rgb
+        ws_bytes = lib.gsb_progan_workspace_bytes(self.desc, n_run, n)
+        ws = scratch.get("progan", ws_bytes, z.device)
+        with torch.cuda.device(z.device), instrument.section("progan"):
+            _check(lib.gsb_progan_forward(_ptr(self.packed), self.desc, self.n_blocks, n_run, _ptr(z), n,
+                                          C.c_void_p(act.data_ptr() if act is not None else 0), act.stride(0) if act is not None else 0,
+                                          _ptr(rgb), _ptr(ws), ws.numel(), _stream()), "gsb_progan_forward")
+        instrument.count(1)
+        instrument.add_rows("progan", n)
+        return act, rgb
+
+    def check(self):
+        flags = C.c_uint(0)
+        with torch.cuda.device(self.device):
+            _check(load().gsb_progan_status(_ptr(self.packed), self.desc, self.n_blocks, C.byref(flags)), "gsb_progan_status")
+        if flags.value & 1:
+            raise NativeError("progan: an operand exceeded fp16 range in the tensor-core path; results are invalid")
 
 
 def pick_global_signs(rowmax_all: torch.Tensor) -> torch.Tensor:

@@ -397,6 +397,135 @@ class StyleGAN2(BaseModel):
                 self.noise.append(torch.randn(1, 1, 2 ** i, 2 ** i).to(self.device))
 
 
+class ProGAN(BaseModel):
+    """wrappers.py:469-522 on the fused chain of csrc/progan.cu.  Z space only; hookable layers are the blocks
+    ``layer1 .. layer14`` and ``output_256x256``.  Checkpoint: ``$GANCONTROL_CHECKPOINT_DIR/progan/<class>_lsun.pth`` (there is no
+    network to download it); without one, ``random_init=<seed>`` (or env GANSPACE_B200_RANDOM_INIT) builds
+    ``progan.random_init(seed)``."""
+
+    CLASSES = ["bedroom", "churchoutdoor", "conferenceroom", "diningroom", "kitchen", "livingroom", "restaurant"]
+    # deepest feature map get_or_compute decomposes (layer10, 128 x 64 x 64): the large-d engine's stacked matrix takes
+    # (components + max(B, 2000, 3 components) + 1) x d x 4 bytes -- 4.4 GB there, 17.5 GB at layer13/14 with its fp16 operand
+    # copies on top -- and has been run up to this size only
+    MAX_DECOMPOSITION_DIMS = 524_288
+
+    def __init__(self, device, lsun_class=None, random_init=None):
+        super().__init__("ProGAN", lsun_class)
+        self.device = _native.require_cuda(device)
+        assert self.outclass in self.CLASSES, f"Invalid LSUN class {self.outclass}, should be one of {self.CLASSES}"
+        self._random_init = random_init
+        self.load_model()
+        self.name = f"ProGAN-{self.outclass}"
+        self.has_latent_residual = False
+
+    def load_model(self):
+        from . import progan
+        root = os.environ.get("GANCONTROL_CHECKPOINT_DIR", Path(__file__).parent / "checkpoints")
+        checkpoint = Path(root) / f"progan/{self.outclass}_lsun.pth"
+        seed = self._random_init
+        if seed is None and os.environ.get("GANSPACE_B200_RANDOM_INIT"):
+            seed = int(os.environ["GANSPACE_B200_RANDOM_INIT"])
+        if checkpoint.is_file() and seed is None:
+            self.model = progan.from_state_dict(torch.load(checkpoint, map_location="cpu")).to(self.device)
+        elif seed is not None:
+            self.model = progan.random_init(seed).to(self.device)
+        else:
+            raise RuntimeError(f"ProGAN checkpoint {checkpoint} not found and no network access to download it; pass "
+                               "random_init=<seed> (or set GANSPACE_B200_RANDOM_INIT) for random-init weights")
+        self.z_dim = self.model.layer1.conv.in_channels
+
+    def get_latent_shape(self):
+        """As StyleGAN2.get_latent_shape: the reference's sample_latent(1) consumes one draw of the global NumPy stream."""
+        _global_seed()
+        return (1, self.z_dim, 1, 1)
+
+    def sample_latent(self, n_samples=1, seed=None, truncation=None):
+        """zdataset.py:26-40: ``RandomState(seed).standard_normal(n * z_dim)`` as float32 [n, z_dim, 1, 1], drawn on the device."""
+        if seed is None:
+            seed = _global_seed()
+        return _native.legacy_normal([seed], self.z_dim * n_samples, self.device).view(n_samples, self.z_dim, 1, 1)
+
+    def sample_latents_multi(self, n_samples, seeds, out=None):
+        """Several ``sample_latent(n_samples, seed=s)`` calls in one launch (the decomposition driver's producer)."""
+        z = _native.legacy_normal(list(seeds), self.z_dim * n_samples, self.device,
+                                  out=None if out is None else out.view(len(seeds), self.z_dim * n_samples),
+                                  parts=_native.split_parts(self.z_dim * n_samples))
+        return z.view(len(seeds) * n_samples, self.z_dim, 1, 1)
+
+    def set_output_class(self, new_class):
+        if self.outclass != new_class:
+            raise RuntimeError("ProGAN: cannot change output class without reloading")
+
+    def check_numerics(self):
+        """Raise if a kernel flagged an out-of-range operand since the weights were packed (synchronises)."""
+        self.model.packed().check()
+
+    @staticmethod
+    def _single(x):
+        if isinstance(x, list):
+            assert len(x) == 1, "ProGAN only supports a single global latent"
+            x = x[0]
+        return x.reshape(x.shape[0], -1).float()
+
+    def _run(self, x, target, want_rgb):
+        """The chain up to block ``target`` (index into layer1 .. layerK; K = the output block, which needs ``want_rgb``) with the
+        forward hooks of every block on the way: a hooked earlier block gets its own run of the chain."""
+        z = self._single(x)
+        names = self.model.block_names()
+        mods = list(self.model._modules.values())
+        packed = self.model.packed()
+        n_conv = len(mods) - 1
+        last = min(target, n_conv - 1)
+
+        def nchw(act, i):
+            res, co = packed.shapes[i]
+            return act.view(-1, res, res, co).permute(0, 3, 1, 2)                # NCHW view of NHWC storage
+
+        def hand(i, t):
+            if mods[i](_result=t) is not t and i < target:
+                raise NotImplementedError(f"an edit on layer '{names[i]}' cannot be propagated through the fused ProGAN chain")
+
+        for i in [i for i in range(last) if len(mods[i]._forward_hooks)]:
+            hand(i, nchw(packed.forward(z, i + 1)[0], i))
+        want_act = len(mods[last]._forward_hooks) > 0 or not want_rgb
+        act, rgb = packed.forward(z, last + 1, want_act=want_act, want_rgb=want_rgb)
+        if want_act:
+            hand(last, nchw(act, last))
+        if want_rgb:
+            img = rgb.permute(0, 3, 1, 2)
+            out = mods[n_conv](_result=img)
+            return out
+        return None
+
+    def forward(self, x):
+        return 0.5 * (self._run(x, len(self.model) - 1, True) + 1)
+
+    def partial_forward(self, x, layer_name):
+        names = self.model.block_names()
+        if layer_name not in names:
+            raise RuntimeError(f"Layer {layer_name} not encountered in partial_forward")
+        target = names.index(layer_name)
+        self._run(x, target, want_rgb=(target == len(names) - 1))
+
+    def feature_layout(self, layer_name):
+        """Device feature order of ``activations_into``: ('nhwc', (H, W, C)) for a conv block."""
+        names = self.model.block_names()
+        if layer_name not in names[:-1]:
+            return None
+        res, co = self.model.packed().shapes[names.index(layer_name)]
+        if res * res * co > self.MAX_DECOMPOSITION_DIMS:
+            raise NotImplementedError(
+                f"ProGAN {layer_name}: d = {res * res * co} exceeds {self.MAX_DECOMPOSITION_DIMS} (layer10), the largest feature map "
+                "the large-d IPCA engine is run at: its stacked matrix holds (components + batch + 1) rows of d floats in HBM")
+        return ("nhwc", (res, res, co))
+
+    def activations_into(self, x, layer_name, out):
+        """Activations of block ``layer_name`` for latents x [n, z_dim(,1,1)] written as fp32 NHWC rows into ``out`` [n, H*W*C]
+        (may be row-strided): the decomposition driver's producer."""
+        n_run = self.model.block_names().index(layer_name) + 1
+        return self.model.packed().forward(self._single(x), n_run, out=out)[0]
+
+
 # ---- factories (wrappers.py:651-735) ---------------------------------------------------------------
 @singledispatch
 def get_model(name, output_class, device, **kwargs):
@@ -416,7 +545,9 @@ def get_model(name, output_class, device, **kwargs):
         assert "-" in name, "Please specify BigGAN resolution, e.g. BigGAN-512"
         from .biggan import BigGAN
         model = BigGAN(device, name.split("-")[-1], class_name=output_class, random_init=kwargs.get("random_init"))
-    elif name in ("StyleGAN", "ProGAN", "DCGAN"):
+    elif name == "ProGAN":
+        model = ProGAN(device, lsun_class=output_class, random_init=kwargs.get("random_init"))
+    elif name in ("StyleGAN", "DCGAN"):
         raise RuntimeError(f"{name} is outside the GPU hot path (SURVEY.md section 2: not in any BASELINE config)")
     else:
         raise RuntimeError(f"Unknown model {name}")
