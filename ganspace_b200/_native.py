@@ -70,6 +70,11 @@ SIGNATURES = {
     "gsb_progan_workspace_bytes": (_Z, [_P, _I, _L]),
     "gsb_progan_forward": (_I, [_P, _P, _I, _I, _P, _L, _P, _L, _P, _P, _Z, _P]),
     "gsb_progan_status": (_I, [_P, _P, _I, _P]),
+    "gsb_biggan_conv_forward": (_I, [_P, _L, _P]),
+    "gsb_biggan_bn_table": (_I, [_P, _L, _I, _P, _P, _P, _F, _I, _P, _P, _P]),
+    "gsb_biggan_attn_pool": (_I, [_P, _L, _I, _I, _P, _P, _P]),
+    "gsb_biggan_softmax_rows": (_I, [_P, _L, _I, _P]),
+    "gsb_biggan_rgb": (_I, [_P, _L, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     "gsb_bigd_rows": (_I, [_I, _I]),
     "gsb_bigd_state_bytes": (_Z, [_L, _I]),
     "gsb_bigd_workspace_bytes": (_Z, [_L, _I, _I, _I]),
@@ -107,6 +112,15 @@ class ProGANBlockDesc(C.Structure):
     """``gsb_progan_block`` of include/ganspace_b200.h."""
     _fields_ = [("conv_weight", C.c_void_p), ("bias", C.c_void_p), ("cin", C.c_int), ("cout", C.c_int), ("upsample", C.c_int),
                 ("res_in", C.c_int), ("ksize", C.c_int)]
+
+
+class BigGANConvDesc(C.Structure):
+    """``gsb_biggan_conv`` of include/ganspace_b200.h."""
+    _fields_ = [("x", C.c_void_p), ("ldx", C.c_int64), ("cin", C.c_int), ("res_in", C.c_int), ("upsample", C.c_int),
+                ("ksize", C.c_int), ("bn_mean", C.c_void_p), ("bn_scale", C.c_void_p), ("bn_offset", C.c_void_p),
+                ("weight", C.c_void_p), ("w_sample_stride", C.c_int64), ("cout", C.c_int), ("bias", C.c_void_p),
+                ("alpha", C.c_float), ("res", C.c_void_p), ("ldres", C.c_int64), ("res_upsample", C.c_int), ("out", C.c_void_p),
+                ("ldo", C.c_int64)]
 
 
 class NativeError(RuntimeError):
@@ -230,6 +244,7 @@ SECTION_KERNELS = {
     "linear": "gen_z linear: mapping_layer_tc_kernel (wgmma, fp16 hi/lo x3, bias epilogue, TMA store) for n >= 128",
     "synthesis": "StyledConv chain: tap-GEMM tc_gemm_plain (wgmma) + gather/scatter/blur epilogues",
     "progan": "ProGAN chain: tap-GEMM tc_gemm_plain (wgmma) + pg_gather_kernel (gather, bias, leaky-ReLU, PixelNorm, RGB)",
+    "biggan": "BigGAN chain: bb_conv_kernel (fp32 implicit GEMM, BN+ReLU prologue, skip / residual epilogue), attention, RGB",
 }
 
 
@@ -880,6 +895,63 @@ class PackedProGAN:
             _check(load().gsb_progan_status(_ptr(self.packed), self.desc, self.n_blocks, C.byref(flags)), "gsb_progan_status")
         if flags.value & 1:
             raise NativeError("progan: an operand exceeded fp16 range in the tensor-core path; results are invalid")
+
+
+def _f32_dev(t, what):
+    assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous(), f"{what}: contiguous fp32 device tensor expected"
+    return C.c_void_p(t.data_ptr())
+
+
+def biggan_conv(x, n, cin, res_in, ksize, weight, cout, out, ldx=None, ldo=None, upsample=False, bn=None, w_sample_stride=0,
+                bias=None, alpha=1.0, res=None, ldres=None, res_upsample=False):
+    """One gsb_biggan_conv_forward launch (csrc/biggan.cu): implicit-GEMM conv of NHWC ``x`` (``n`` samples at res_in^2 pixels with
+    pixel stride ``ldx``) with ``weight`` [ksize^2 cin, cout] into ``out``; ``bn`` = (mean [cin], scale [n, cin], offset [n, cin])
+    is the BatchNorm + ReLU applied to the operand, ``res`` the residual added after ``alpha * (conv + bias)``."""
+    d = BigGANConvDesc()
+    d.x, d.ldx, d.cin, d.res_in, d.upsample, d.ksize = x.data_ptr(), ldx or cin, cin, res_in, int(upsample), ksize
+    if bn is not None:
+        d.bn_mean, d.bn_scale, d.bn_offset = (_f32_dev(t, "biggan_conv bn").value for t in bn)
+    d.weight, d.w_sample_stride, d.cout = _f32_dev(weight, "biggan_conv weight").value, w_sample_stride, cout
+    d.bias = _f32_dev(bias, "biggan_conv bias").value if bias is not None else None
+    d.alpha = alpha
+    if res is not None:
+        d.res, d.ldres, d.res_upsample = res.data_ptr(), ldres or cout, int(res_upsample)
+    d.out, d.ldo = out.data_ptr(), ldo or cout
+    for t in (x, out) + ((res,) if res is not None else ()):
+        assert t.is_cuda and t.dtype == torch.float32
+    with torch.cuda.device(out.device):
+        _check(load().gsb_biggan_conv_forward(C.byref(d), n, _stream()), "gsb_biggan_conv_forward")
+    instrument.count(1)
+
+
+def biggan_bn_table(cond, w_scale, w_offset, var, eps, scale_out, offset_out):
+    n, cdim = cond.shape
+    with torch.cuda.device(cond.device):
+        _check(load().gsb_biggan_bn_table(_f32_dev(cond, "cond"), n, cdim, _f32_dev(w_scale, "w_scale"), _f32_dev(w_offset, "w_offset"),
+                                          _f32_dev(var, "var"), float(eps), var.numel(), _f32_dev(scale_out, "scale"),
+                                          _f32_dev(offset_out, "offset"), _stream()), "gsb_biggan_bn_table")
+    instrument.count(1)
+
+
+def biggan_attn_pool(tpg, n, res, c, phi_t, g):
+    with torch.cuda.device(tpg.device):
+        _check(load().gsb_biggan_attn_pool(_f32_dev(tpg, "tpg"), n, res, c, _f32_dev(phi_t, "phi_t"), _f32_dev(g, "g"), _stream()),
+               "gsb_biggan_attn_pool")
+    instrument.count(1)
+
+
+def biggan_softmax_rows(s, rows, cols):
+    with torch.cuda.device(s.device):
+        _check(load().gsb_biggan_softmax_rows(_f32_dev(s, "s"), rows, cols, _stream()), "gsb_biggan_softmax_rows")
+    instrument.count(1)
+
+
+def biggan_rgb(x, n, res, c, mean, scale, offset, weight, bias, img):
+    with torch.cuda.device(x.device):
+        _check(load().gsb_biggan_rgb(_f32_dev(x, "x"), n, res, c, _f32_dev(mean, "mean"), _f32_dev(scale, "scale"),
+                                     _f32_dev(offset, "offset"), _f32_dev(weight, "weight"), _f32_dev(bias, "bias"),
+                                     _f32_dev(img, "img"), _stream()), "gsb_biggan_rgb")
+    instrument.count(1)
 
 
 def pick_global_signs(rowmax_all: torch.Tensor) -> torch.Tensor:

@@ -17,12 +17,15 @@ With the thin QR  A = Q R  every centred activation is  (z - zbar) R^T Q^T, so s
 factorisation; the decomposition driver then never materialises the [N, 32768] activations (131 GB at N=1e6)
 and reuses the small-d engine.  ``partial_forward`` still produces the full activation for API users.
 
-The synthesis blocks after gen_z (GenBlock / SelfAttn / BigGANBatchNorm) are outside the hot path
-(SURVEY.md section 2 row 8) and raise.
+Synthesis (``forward``, ``partial_forward`` to ``generator.layers.k``): the reference's module tree (GenBlock, SelfAttn,
+BigGANBatchNorm, generator.bn, conv_to_rgb; same names, shapes and creation order) holds the parameters, and ``_Chain`` runs
+them on the kernels of csrc/biggan.cu (DESIGN.md section 5i).  Decomposing a layer other than gen_z is not built and raises.
 """
 from __future__ import annotations
 
+import math
 import os
+import re
 from pathlib import Path
 
 import numpy as np
@@ -37,8 +40,16 @@ from .wrappers import BaseModel, _global_seed
 _CLASS_IDS = {"husky": 248, "siberian_husky": 250, "golden_retriever": 207, "lion": 291, "tiger": 292,
               "mushroom": 947, "barn": 425, "church": 497, "castle": 483, "volcano": 980, "lakeside": 975}
 
-# (up-sample, in, out) of biggan-deep-{128,256,512}: only len(layers) matters here (n_latents)
-_N_LAYERS = {128: 10, 256: 12, 512: 14}
+# (up-sample, in, out) per GenBlock, in units of channel_width.  128: the reference's BigGANConfig defaults; 512: its
+# biggan-deep-512 configuration; 256: the same pattern with six up-samplings (the published config is not available offline)
+_LAYERS = {
+    128: [(False, 16, 16), (True, 16, 16), (False, 16, 16), (True, 16, 8), (False, 8, 8), (True, 8, 4), (False, 4, 4),
+          (True, 4, 2), (False, 2, 2), (True, 2, 1)],
+    256: [(False, 16, 16), (True, 16, 16), (False, 16, 16), (True, 16, 8), (False, 8, 8), (True, 8, 8), (False, 8, 8),
+          (True, 8, 4), (False, 4, 4), (True, 4, 2), (False, 2, 2), (True, 2, 1)],
+    512: [(False, 16, 16), (True, 16, 16), (False, 16, 16), (True, 16, 8), (False, 8, 8), (True, 8, 8), (False, 8, 8),
+          (True, 8, 4), (False, 4, 4), (True, 4, 2), (False, 2, 2), (True, 2, 1), (False, 1, 1), (True, 1, 1)],
+}
 _CHANNEL_WIDTH = 128
 
 
@@ -49,19 +60,26 @@ class _Config:
         self.class_embed_dim = 128
         self.channel_width = _CHANNEL_WIDTH
         self.num_classes = 1000
-        self.layers = [None] * _N_LAYERS[resolution]
+        self.layers = list(_LAYERS[resolution])
+        self.attention_layer_position = 8
         self.eps = 1e-4
+        self.n_stats = 51
 
 
-class SNLinear(nn.Module):
-    """``spectral_norm(nn.Linear)`` in eval mode: y = x (W_orig / sigma)^T + b, sigma = u^T W_orig v."""
+class _SNParams(nn.Module):
+    """The tensors of a ``torch.nn.utils.spectral_norm`` module (``bias``, ``weight_orig``, ``weight_u``, ``weight_v``), copied from
+    one built with torch so that its random init (layer init, then the normal draws of u and v) is the reference's.  In eval mode
+    the effective weight is W_orig / sigma with sigma = u^T W_orig.view(out, -1) v: no power iteration."""
 
-    def __init__(self, lin_sn):
+    def __init__(self, sn):
         super().__init__()
-        self.weight_orig = nn.Parameter(lin_sn.weight_orig.detach().clone())
-        self.bias = nn.Parameter(lin_sn.bias.detach().clone())
-        self.register_buffer("weight_u", lin_sn.weight_u.detach().clone())
-        self.register_buffer("weight_v", lin_sn.weight_v.detach().clone())
+        if sn.bias is not None:
+            self.bias = nn.Parameter(sn.bias.detach().clone())
+        else:
+            self.register_parameter("bias", None)
+        self.weight_orig = nn.Parameter(sn.weight_orig.detach().clone())
+        self.register_buffer("weight_u", sn.weight_u.detach().clone())
+        self.register_buffer("weight_v", sn.weight_v.detach().clone())
         self._eff = None
         self._key = None
 
@@ -69,10 +87,14 @@ class SNLinear(nn.Module):
         key = (self.weight_orig._version, self.weight_orig.data_ptr(), self.weight_u._version, self.weight_v._version)
         if self._eff is None or self._key != key:
             w = self.weight_orig.detach()
-            sigma = torch.dot(self.weight_u, torch.mv(w, self.weight_v))      # torch spectral_norm, eval mode
+            sigma = torch.dot(self.weight_u, torch.mv(w.reshape(w.shape[0], -1), self.weight_v))      # torch spectral_norm, eval mode
             self._eff = (w / sigma).contiguous()
             self._key = key
         return self._eff
+
+
+class SNLinear(_SNParams):
+    """``spectral_norm(nn.Linear)`` in eval mode: y = x (W_orig / sigma)^T + b."""
 
     def forward(self, x):
         # latents are truncated normals in [-2, 2] * truncation and the class embedding is a fixed vector: inside fp16's range,
@@ -80,27 +102,185 @@ class SNLinear(nn.Module):
         return _native.linear(x, self.effective_weight(), self.bias.detach(), bounded=bool(x.abs().max() < 6e4) if x.shape[0] >= 128 else False)
 
 
+class SNConv2d(_SNParams):
+    """``spectral_norm(nn.Conv2d)`` in eval mode, parameters only: the convolution runs in csrc/biggan.cu."""
+
+    def __init__(self, in_channels, out_channels, kernel_size, padding=0, bias=True, eps=1e-12):
+        super().__init__(nn.utils.spectral_norm(nn.Conv2d(in_channels, out_channels, kernel_size, padding=padding, bias=bias), eps=eps))
+
+    def gemm_weight(self) -> torch.Tensor:
+        """W_eff as the GEMM operand of gsb_biggan_conv_forward: [ksize^2 cin, cout], row (ky ksize + kx) cin + ci."""
+        w = self.effective_weight()
+        return w.permute(2, 3, 1, 0).reshape(-1, w.shape[0]).contiguous()
+
+
+def _sn_linear(cin, cout, eps, bias=True):
+    return SNLinear(nn.utils.spectral_norm(nn.Linear(cin, cout, bias=bias), eps=eps))
+
+
+class _FusedModule(nn.Module):
+    """A module whose arithmetic runs in the BigGAN chain (BigGAN.forward / partial_forward): ``forward(_result=act)`` only hands
+    the chain's result to the forward hooks, the convention of stylegan2.StyledConv and progan.Block."""
+
+    def forward(self, *args, _result=None, **kwargs):
+        if _result is None:
+            raise NotImplementedError(f"{type(self).__name__} runs as part of the BigGAN chain (BigGAN.forward / partial_forward); "
+                                      "a stand-alone call is not built and there is no PyTorch fallback")
+        return _result
+
+
+class BigGANBatchNorm(_FusedModule):
+    """model.py:99-149: BatchNorm with the statistics interpolated from 51 per-truncation tables; conditional: weight
+    1 + scale(cond) and bias offset(cond), bias-free spectral-norm linears of the condition vector."""
+
+    def __init__(self, num_features, condition_vector_dim=None, n_stats=51, eps=1e-4, conditional=True):
+        super().__init__()
+        self.num_features = num_features
+        self.eps = eps
+        self.conditional = conditional
+        self.register_buffer("running_means", torch.zeros(n_stats, num_features))
+        self.register_buffer("running_vars", torch.ones(n_stats, num_features))
+        self.step_size = 1.0 / (n_stats - 1)
+        if conditional:
+            self.scale = _sn_linear(condition_vector_dim, num_features, eps, bias=False)
+            self.offset = _sn_linear(condition_vector_dim, num_features, eps, bias=False)
+        else:
+            self.weight = nn.Parameter(torch.empty(num_features))         # uninitialised in the reference (torch.Tensor(n))
+            self.bias = nn.Parameter(torch.empty(num_features))
+
+    def stats(self, truncation):
+        """(mean, var) at ``truncation``, interpolated exactly as the reference orders it (model.py:128-135)."""
+        coef, start = math.modf(truncation / self.step_size)
+        start = int(start)
+        rm, rv = self.running_means.detach(), self.running_vars.detach()
+        if coef != 0.0:
+            return rm[start] * coef + rm[start + 1] * (1 - coef), rv[start] * coef + rv[start + 1] * (1 - coef)
+        return rm[start], rv[start]
+
+
+class GenBlock(_FusedModule):
+    """model.py:152-202: bn_0 -> ReLU -> conv_0 (1x1) -> bn_1 -> ReLU -> [nearest x2] -> conv_1 (3x3) -> bn_2 -> ReLU -> conv_2 (3x3)
+    -> bn_3 -> ReLU -> conv_3 (1x1), plus the skip path (first in/2 channels when in != out, nearest x2 when up-sampling)."""
+
+    def __init__(self, in_size, out_size, condition_vector_dim, reduction_factor=4, up_sample=False, n_stats=51, eps=1e-12):
+        super().__init__()
+        self.up_sample = up_sample
+        self.drop_channels = in_size != out_size
+        mid = in_size // reduction_factor
+        self.bn_0 = BigGANBatchNorm(in_size, condition_vector_dim, n_stats=n_stats, eps=eps)
+        self.conv_0 = SNConv2d(in_size, mid, 1, eps=eps)
+        self.bn_1 = BigGANBatchNorm(mid, condition_vector_dim, n_stats=n_stats, eps=eps)
+        self.conv_1 = SNConv2d(mid, mid, 3, padding=1, eps=eps)
+        self.bn_2 = BigGANBatchNorm(mid, condition_vector_dim, n_stats=n_stats, eps=eps)
+        self.conv_2 = SNConv2d(mid, mid, 3, padding=1, eps=eps)
+        self.bn_3 = BigGANBatchNorm(mid, condition_vector_dim, n_stats=n_stats, eps=eps)
+        self.conv_3 = SNConv2d(mid, out_size, 1, eps=eps)
+
+
+class SelfAttn(_FusedModule):
+    """model.py:57-96: theta, phi, g 1x1 convs (C/8, C/8, C/2, no bias), 2x2 max-pool of phi and g, softmax over the keys,
+    o_conv (C/2 -> C), out = x + gamma o."""
+
+    def __init__(self, in_channels, eps=1e-12):
+        super().__init__()
+        self.in_channels = in_channels
+        self.snconv1x1_theta = SNConv2d(in_channels, in_channels // 8, 1, bias=False, eps=eps)
+        self.snconv1x1_phi = SNConv2d(in_channels, in_channels // 8, 1, bias=False, eps=eps)
+        self.snconv1x1_g = SNConv2d(in_channels, in_channels // 2, 1, bias=False, eps=eps)
+        self.snconv1x1_o_conv = SNConv2d(in_channels // 2, in_channels, 1, bias=False, eps=eps)
+        self.gamma = nn.Parameter(torch.zeros(1))
+
+
 class _Generator(nn.Module):
+    """model.py:204-229, modules created in the reference's order."""
+
     def __init__(self, gen_z, config):
         super().__init__()
         self.config = config
+        ch = config.channel_width
+        cdim = 2 * config.z_dim
         self.gen_z = gen_z
-        self.layers = nn.ModuleList()        # GenBlock / SelfAttn: outside the hot path
+        layers = []
+        for i, (up, cin, cout) in enumerate(config.layers):
+            if i == config.attention_layer_position:
+                layers.append(SelfAttn(ch * cin, eps=config.eps))
+            layers.append(GenBlock(ch * cin, ch * cout, cdim, up_sample=up, n_stats=config.n_stats, eps=config.eps))
+        self.layers = nn.ModuleList(layers)
+        self.bn = BigGANBatchNorm(ch, n_stats=config.n_stats, eps=config.eps, conditional=False)
+        self.conv_to_rgb = SNConv2d(ch, ch, 3, padding=1, eps=config.eps)
 
 
 class _BigGANNet(nn.Module):
-    """Parameter layout of pytorch_pretrained_biggan.BigGAN restricted to embeddings + generator.gen_z."""
+    """Module tree, parameter and buffer names of pytorch_pretrained_biggan.BigGAN (a pytorch_model.bin loads by key)."""
 
     def __init__(self, resolution):
         super().__init__()
         self.config = _Config(resolution)
-        # creation order == the reference's (embeddings, then Generator.gen_z first), so that
-        # torch.manual_seed(s) reproduces the reference's random init of these tensors bit-for-bit
+        # creation order == the reference's (embeddings, then Generator: gen_z, layers, bn, conv_to_rgb), so that
+        # torch.manual_seed(s) reproduces the reference's random init bit-for-bit (gen_z's is a prefix of it)
         self.embeddings = nn.Linear(self.config.num_classes, self.config.z_dim, bias=False)
-        lin = nn.utils.spectral_norm(nn.Linear(2 * self.config.z_dim, 4 * 4 * 16 * self.config.channel_width),
-                                     eps=self.config.eps)
-        self.generator = _Generator(SNLinear(lin), self.config)
+        self.generator = _Generator(_sn_linear(2 * self.config.z_dim, 4 * 4 * 16 * self.config.channel_width, self.config.eps),
+                                    self.config)
         self.n_latents = len(self.config.layers) + 1
+
+
+@torch.no_grad()
+def synthesis_fill(net, seed=0):
+    """Seeded values for what a random init leaves degenerate or undefined: the BatchNorm statistics tables (zeros and ones),
+    ``SelfAttn.gamma`` (zero) and ``generator.bn.weight`` / ``bias`` (uninitialised).  Works on this module tree and on the
+    reference's (same attribute names), so that both get the same weights.
+
+    Spectral normalisation with random u, v does not bound a random conv (sigma = u^T W v is not its norm), so a BatchNorm with
+    unit statistics would let the activations grow by orders of magnitude per conv.  The tables are therefore scaled to the
+    second moment each BatchNorm's input would have if every conv input were independent and zero-mean (propagated per channel
+    through the effective weights, in fp64), then perturbed per truncation row: every BatchNorm re-normalises and the 51 rows
+    differ, so the interpolation is visible.  The tail BatchNorm's weight is scaled so that ``conv_to_rgb`` stays out of tanh's
+    saturation."""
+    gen = torch.Generator().manual_seed(int(seed))
+    randn = lambda *s: torch.randn(*s, generator=gen, dtype=torch.float64)
+    rand = lambda *s: torch.rand(*s, generator=gen, dtype=torch.float64)
+    g = net.generator
+    cfg = net.config
+
+    def w_eff(m):
+        w = m.weight_orig.detach().double().cpu()
+        return w / torch.dot(m.weight_u.double().cpu(), torch.mv(w.reshape(w.shape[0], -1), m.weight_v.double().cpu()))
+
+    def conv_m2(m, m2):
+        out = w_eff(m).pow(2).flatten(2).sum(2) @ m2
+        return out if m.bias is None else out + m.bias.detach().double().cpu().pow(2)
+
+    cond_m2 = torch.cat([torch.ones(cfg.z_dim, dtype=torch.float64),
+                         net.embeddings.weight.detach().double().cpu().pow(2).mean(1)])
+
+    def fill_bn(bn, m2):
+        c = m2.numel()
+        sd = m2.clamp_min(1e-12).sqrt()
+        bn.running_means.copy_(0.3 * sd * randn(cfg.n_stats, c))
+        bn.running_vars.copy_(m2.clamp_min(1e-12) * (0.5 + rand(cfg.n_stats, c)))
+        if bn.conditional:                     # E[((1 + s) x^ + o)^2] with x^ of unit second moment, then ReLU halves it
+            return 0.5 * (1 + w_eff(bn.scale).pow(2) @ cond_m2 + w_eff(bn.offset).pow(2) @ cond_m2)
+        return None
+
+    wz = w_eff(g.gen_z)
+    m2 = (wz.pow(2) @ cond_m2 + g.gen_z.bias.detach().double().cpu().pow(2)).view(16, -1).mean(0)      # NHWC [4, 4, 16 ch]
+    for layer in g.layers:
+        if hasattr(layer, "snconv1x1_theta"):
+            # o_conv's output is not normalised: gamma brings it to the scale of its input, so that neither term drowns the other
+            o2 = conv_m2(layer.snconv1x1_o_conv, conv_m2(layer.snconv1x1_g, m2))
+            gamma = (0.5 + 0.5 * rand(1)) * torch.sqrt(m2.mean() / o2.mean())
+            layer.gamma.copy_(gamma)
+            m2 = m2 + gamma.pow(2) * o2
+            continue
+        h = m2
+        for bn, conv in ((layer.bn_0, layer.conv_0), (layer.bn_1, layer.conv_1), (layer.bn_2, layer.conv_2), (layer.bn_3, layer.conv_3)):
+            h = conv_m2(conv, fill_bn(bn, h))
+        m2 = h + m2[:h.numel()]
+    fill_bn(g.bn, m2)
+    kappa = 1.0 / torch.sqrt(0.5 * w_eff(g.conv_to_rgb)[:3].pow(2).flatten(1).sum(1).mean())
+    c = m2.numel()
+    g.bn.weight.copy_(kappa * (0.5 + rand(c)))
+    g.bn.bias.copy_(0.2 * kappa * randn(c))
 
 
 class AffineLayer:
@@ -124,6 +304,96 @@ class AffineLayer:
         return _native.linear(rows64.float().contiguous(), self.Q32).double()
 
 
+class _Chain:
+    """The synthesis weights folded at one truncation and uploaded for csrc/biggan.cu, and the launch sequence of each module.
+    Per GenBlock BatchNorm: the interpolated mean and variance and the effective scale / offset weights, whose products with the
+    samples' condition vectors become per-(sample, channel) affine tables at run time; per conv: W_eff as a [k^2 cin, cout]
+    GEMM operand; SelfAttn: theta | phi | g as one GEMM operand; tail: the BatchNorm as a per-channel affine and the first three
+    output channels of conv_to_rgb (the only ones the image keeps)."""
+
+    def __init__(self, net, truncation, device):
+        f = lambda t: t.detach().to(device=device, dtype=torch.float32).contiguous()
+        g = net.generator
+        self.device = device
+        self.steps = []
+        for layer in g.layers:
+            if isinstance(layer, SelfAttn):
+                w = torch.cat([m.gemm_weight() for m in (layer.snconv1x1_theta, layer.snconv1x1_phi, layer.snconv1x1_g)], dim=1)
+                self.steps.append(dict(w_tpg=f(w), w_o=f(layer.snconv1x1_o_conv.gemm_weight()), gamma=float(layer.gamma.detach())))
+                continue
+            bns = []
+            for bn in (layer.bn_0, layer.bn_1, layer.bn_2, layer.bn_3):
+                mean, var = bn.stats(truncation)
+                bns.append(dict(mean=f(mean), var=f(var), ws=f(bn.scale.effective_weight()), wo=f(bn.offset.effective_weight()),
+                                eps=bn.eps))
+            convs = [dict(w=f(c.gemm_weight()), b=f(c.bias)) for c in (layer.conv_0, layer.conv_1, layer.conv_2, layer.conv_3)]
+            cin, mid, cout = layer.conv_0.weight_orig.shape[1], layer.conv_0.weight_orig.shape[0], layer.conv_3.weight_orig.shape[0]
+            assert cout == cin or 2 * cout == cin
+            self.steps.append(dict(cin=cin, mid=mid, cout=cout, up=bool(layer.up_sample), bns=bns, convs=convs))
+        mean, var = g.bn.stats(truncation)
+        self.tail = dict(mean=f(mean), scale=f(g.bn.weight.detach() / torch.sqrt(var + g.bn.eps)), offset=f(g.bn.bias),
+                         w=f(g.conv_to_rgb.effective_weight()[:3]), b=f(g.conv_to_rgb.bias[:3]))
+
+    def _empty(self, *shape):
+        return torch.empty(shape, dtype=torch.float32, device=self.device)
+
+    def block(self, i, x, cond):
+        """GenBlock i on NHWC x [n, R, R, cin] with condition vectors cond [n, 256] -> [n, R', R', cout]."""
+        p = self.steps[i]
+        n, R = x.shape[0], x.shape[1]
+        R2 = 2 * R if p["up"] else R
+        mid, cin, cout = p["mid"], p["cin"], p["cout"]
+        with _native.instrument.section(f"biggan layers.{i}"):
+            tabs = []
+            for bn in p["bns"]:
+                c = bn["mean"].numel()
+                scale, offset = self._empty(n, c), self._empty(n, c)
+                _native.biggan_bn_table(cond, bn["ws"], bn["wo"], bn["var"], bn["eps"], scale, offset)
+                tabs.append((bn["mean"], scale, offset))
+            (w0, w1, w2, w3) = p["convs"]
+            t0 = self._empty(n, R, R, mid)
+            _native.biggan_conv(x, n, cin, R, 1, w0["w"], mid, t0, bn=tabs[0], bias=w0["b"])
+            t1 = self._empty(n, R2, R2, mid)
+            _native.biggan_conv(t0, n, mid, R, 3, w1["w"], mid, t1, upsample=p["up"], bn=tabs[1], bias=w1["b"])
+            t2 = self._empty(n, R2, R2, mid)
+            _native.biggan_conv(t1, n, mid, R2, 3, w2["w"], mid, t2, bn=tabs[2], bias=w2["b"])
+            out = self._empty(n, R2, R2, cout)
+            _native.biggan_conv(t2, n, mid, R2, 1, w3["w"], cout, out, bn=tabs[3], bias=w3["b"], res=x, ldres=cin,
+                                res_upsample=p["up"])
+        _native.instrument.add_rows("biggan", n if i == 0 else 0)
+        return out
+
+    def attn(self, i, x):
+        """SelfAttn i on NHWC x [n, R, R, C]: theta | phi | g in one GEMM, 2x2 max-pool, scores against the pooled keys, softmax
+        over the keys, the weighted sum of the pooled g, then o_conv with x + gamma o in its epilogue."""
+        p = self.steps[i]
+        n, R, C = x.shape[0], x.shape[1], x.shape[3]
+        c8, c2, hwp = C // 8, C // 2, R * R // 4
+        ct = 2 * c8 + c2
+        with _native.instrument.section(f"biggan layers.{i}"):
+            tpg = self._empty(n, R, R, ct)
+            _native.biggan_conv(x, n, C, R, 1, p["w_tpg"], ct, tpg)
+            phi_t, gp = self._empty(n, c8, hwp), self._empty(n, hwp, c2)
+            _native.biggan_attn_pool(tpg, n, R, C, phi_t, gp)
+            s = self._empty(n, R * R, hwp)
+            _native.biggan_conv(tpg, n, c8, R, 1, phi_t, hwp, s, ldx=ct, w_sample_stride=c8 * hwp)
+            _native.biggan_softmax_rows(s, n * R * R, hwp)
+            o = self._empty(n, R * R, c2)
+            _native.biggan_conv(s, n, hwp, R, 1, gp, c2, o, w_sample_stride=hwp * c2)
+            out = self._empty(n, R, R, C)
+            _native.biggan_conv(o, n, c2, R, 1, p["w_o"], C, out, alpha=p["gamma"], res=x)
+        return out
+
+    def rgb(self, x):
+        """Tail on NHWC x [n, R, R, ch]: image 0.5 (tanh(conv_to_rgb(ReLU(bn(x)))[:3]) + 1), NHWC [n, R, R, 3]."""
+        n, R, C = x.shape[0], x.shape[1], x.shape[3]
+        t = self.tail
+        img = self._empty(n, R, R, 3)
+        with _native.instrument.section("biggan rgb"):
+            _native.biggan_rgb(x, n, R, C, t["mean"], t["scale"], t["offset"], t["w"], t["b"], img)
+        return img
+
+
 class BigGAN(BaseModel):
     def __init__(self, device, resolution, class_name, truncation=1.0, random_init=None):
         super().__init__(f"BigGAN-{resolution}", class_name)
@@ -138,7 +408,7 @@ class BigGAN(BaseModel):
         self._affine = {}
 
     def load_model(self, name):
-        if self.resolution not in _N_LAYERS:
+        if self.resolution not in _LAYERS:
             raise RuntimeError("Unknown BigGAN model name", name)
         root = os.environ.get("GANCONTROL_CHECKPOINT_DIR", Path(__file__).parent / "checkpoints")
         weights = Path(root) / name / "pytorch_model.bin"
@@ -148,19 +418,19 @@ class BigGAN(BaseModel):
                 else int(os.environ["GANSPACE_B200_RANDOM_INIT"])
         if weights.is_file() and seed is None:
             net = _BigGANNet(self.resolution)
-            sd = torch.load(weights, map_location="cpu")
-            g = net.generator.gen_z
-            net.embeddings.weight.data.copy_(sd["embeddings.weight"])
-            g.weight_orig.data.copy_(sd["generator.gen_z.weight_orig"])
-            g.bias.data.copy_(sd["generator.gen_z.bias"])
-            g.weight_u.copy_(sd["generator.gen_z.weight_u"])
-            g.weight_v.copy_(sd["generator.gen_z.weight_v"])
+            net.load_state_dict(torch.load(weights, map_location="cpu"), strict=False)      # as BigGAN.from_pretrained
         elif seed is not None:
             torch.manual_seed(int(seed))
             net = _BigGANNet(self.resolution)
+            synthesis_fill(net, int(seed))
         else:
             raise RuntimeError(f"BigGAN weights {weights} not found and no network access; pass random_init=<seed>")
-        self.model = net.to(self.device)
+        # only the embedding and gen_z go to the device here: the synthesis weights are folded and uploaded on the first
+        # synthesis call (_chain), so that gen_z-only runs (decomposition of generator.gen_z) never touch them
+        net.embeddings.to(self.device)
+        net.generator.gen_z.to(self.device)
+        self.model = net
+        self._chain_cache = None
 
     # ---- latents ----------------------------------------------------------------------------------
     def sample_latent(self, n_samples=1, truncation=None, seed=None):
@@ -214,22 +484,86 @@ class BigGAN(BaseModel):
         """embeddings(one_hot) = column `idx` of the embedding matrix  -> [128] fp32."""
         return self.model.embeddings.weight.detach()[:, self._class_idx].contiguous()
 
+    # ---- synthesis: GenBlock / SelfAttn chain and the RGB tail (csrc/biggan.cu) --------------------------------------------
+    def _conds(self, x):
+        """cond[k] = cat(z[k], embed) for the n_latents latents (one z is used for all of them), model.py:295-309."""
+        n_lat = self.model.n_latents
+        zs = x if isinstance(x, list) else n_lat * [x]
+        assert len(zs) == n_lat, f"Expected {n_lat} latents, got {len(zs)}"
+        e = self._embed().unsqueeze(0)
+        return [torch.cat((z.reshape(z.shape[0], -1).float(), e.expand(z.shape[0], -1)), dim=1).contiguous() for z in zs]
+
+    def _chain(self):
+        """The synthesis weights folded and uploaded at the current truncation (again when a parameter or buffer changes)."""
+        g = self.model.generator
+        tensors = [t for m in (g.layers, g.bn, g.conv_to_rgb) for t in list(m.parameters()) + list(m.buffers())]
+        key = (float(self.truncation), tuple((t._version, t.data_ptr()) for t in tensors))
+        if self._chain_cache is None or self._chain_cache[0] != key:
+            self._chain_cache = (key, _Chain(self.model, float(self.truncation), self.device))
+        return self._chain_cache[1]
+
+    def _synthesize(self, x, n_modules, want_image):
+        """gen_z, then generator.layers[:n_modules] (and the tail when ``want_image``), firing the hooks of every layer on the
+        way.  A hook's result on gen_z is what the chain continues from; an edit on a later layer would have to be re-fed into the
+        chain, which is not built -- it raises instead of being silently ignored (except on the last layer of a partial run)."""
+        g = self.model.generator
+        layers = list(g.layers)[:n_modules]
+        inner = [(name, m) for i, l in enumerate(layers) for name, m in l.named_modules(prefix=f"generator.layers.{i}") if m is not l]
+        if want_image:
+            inner += [("generator.bn", g.bn), ("generator.conv_to_rgb", g.conv_to_rgb)]
+        for name, m in inner:
+            if len(m._forward_hooks):
+                raise NotImplementedError(f"a hook on '{name}': the BigGAN chain materialises the outputs of gen_z and of "
+                                          "generator.layers.k only")
+        conds = self._conds(x)
+        h = g.gen_z(conds[0])
+        chain = self._chain()
+        act = h.contiguous().view(h.shape[0], 4, 4, -1)                 # gen_z's output is NHWC [4, 4, 16 ch] already
+        ci = 1
+        for i, mod in enumerate(layers):
+            if isinstance(mod, GenBlock):
+                act = chain.block(i, act, conds[ci])
+                ci += 1
+            else:
+                act = chain.attn(i, act)
+            if len(mod._forward_hooks):
+                view = act.permute(0, 3, 1, 2)                             # NCHW view of NHWC storage
+                if mod(_result=view) is not view and (want_image or i < len(layers) - 1):
+                    raise NotImplementedError(f"an edit on layer 'generator.layers.{i}' cannot be propagated through the "
+                                              "BigGAN chain")
+        return chain.rgb(act).permute(0, 3, 1, 2) if want_image else None
+
     def forward(self, x):
-        raise NotImplementedError("BigGAN image synthesis (GenBlock / SelfAttn) is outside the GPU hot path "
-                                  "(SURVEY.md section 2 row 8)")
+        """wrappers.py:599-607: images 0.5 (G(z) + 1) in [0, 1], [n, 3, R, R] (an NCHW view of NHWC storage), from one latent or
+        a list of n_latents (one per layer)."""
+        return self._synthesize(x, len(self.model.generator.layers), True)
 
     def partial_forward(self, x, layer_name):
-        if layer_name not in ("embeddings", "generator.gen_z"):
-            raise NotImplementedError(f"BigGAN.partial_forward to '{layer_name}': only generator.gen_z is on the hot path")
-        z = x[0] if isinstance(x, list) else x
-        cond = torch.cat((z, self._embed().unsqueeze(0).expand(z.shape[0], -1)), dim=1).contiguous()
-        self.model.generator.gen_z(cond)             # hook retains [B, 4*4*16*ch]
+        """wrappers.py:611-648, including its quirks: 'generator.layers.k' runs layers[:k+1] of the ModuleList (SelfAttn is one of
+        them); any other name but embeddings / gen_z runs layers[:len(config.layers)], one module short of the ModuleList, and
+        never the tail.  Returns None; results reach the caller through hooks."""
+        if layer_name in ("embeddings", "generator.gen_z"):
+            z = x[0] if isinstance(x, list) else x
+            cond = torch.cat((z, self._embed().unsqueeze(0).expand(z.shape[0], -1)), dim=1).contiguous()
+            self.model.generator.gen_z(cond)             # hook retains [B, 4*4*16*ch]
+            return None
+        if "generator.layers" in layer_name:
+            m = re.match(r"^generator\.layers\.[0-9]+", layer_name)
+            if m is None:
+                raise RuntimeError(f"Unknown layer '{layer_name}'")
+            n_layers = int(m[0].split(".")[-1]) + 1
+        else:
+            n_layers = len(self.model.config.layers)
+        self._synthesize(x, n_layers, False)
         return None
 
     # ---- low-rank structure of gen_z ----------------------------------------------------------------
     def affine_layer(self, layer_name):
         # GANSPACE_B200_BIGGAN_AFFINE=0: no low-rank shortcut -- the activations are materialised and go through the general
         # large-d engine (csrc/bigd.cu), a cross-check of the shortcut
+        if layer_name.startswith("generator.") and layer_name != "generator.gen_z":
+            raise NotImplementedError(f"BigGAN: decomposing '{layer_name}' is not built; of the generator's layers only "
+                                      "generator.gen_z can be decomposed")
         if layer_name != "generator.gen_z" or os.environ.get("GANSPACE_B200_BIGGAN_AFFINE", "1") == "0":
             return None
         if layer_name not in self._affine:
