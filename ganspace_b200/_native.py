@@ -70,6 +70,11 @@ SIGNATURES = {
     "gsb_progan_workspace_bytes": (_Z, [_P, _I, _L]),
     "gsb_progan_forward": (_I, [_P, _P, _I, _I, _P, _L, _P, _L, _P, _P, _Z, _P]),
     "gsb_progan_status": (_I, [_P, _P, _I, _P]),
+    "gsb_stylegan_packed_bytes": (_Z, [_P, _I, _I]),
+    "gsb_stylegan_pack": (_I, [_P, _I, _I, _P, _P, _P, _P, _Z, _P]),
+    "gsb_stylegan_workspace_bytes": (_Z, [_P, _I, _L]),
+    "gsb_stylegan_forward": (_I, [_P, _P, _I, _I, _I, _P, _I, _L, _P, _L, _P, _P, _Z, _P]),
+    "gsb_stylegan_status": (_I, [_P, _P, _I, _I, _P]),
     "gsb_biggan_conv_forward": (_I, [_P, _L, _P]),
     "gsb_biggan_bn_table": (_I, [_P, _L, _I, _P, _P, _P, _F, _I, _P, _P, _P]),
     "gsb_biggan_attn_pool": (_I, [_P, _L, _I, _I, _P, _P, _P]),
@@ -112,6 +117,13 @@ class ProGANBlockDesc(C.Structure):
     """``gsb_progan_block`` of include/ganspace_b200.h."""
     _fields_ = [("conv_weight", C.c_void_p), ("bias", C.c_void_p), ("cin", C.c_int), ("cout", C.c_int), ("upsample", C.c_int),
                 ("res_in", C.c_int), ("ksize", C.c_int)]
+
+
+class StyleGANLayerDesc(C.Structure):
+    """``gsb_stylegan_layer`` of include/ganspace_b200.h."""
+    _fields_ = [("conv_weight", C.c_void_p), ("bias", C.c_void_p), ("noise", C.c_void_p), ("noise_weight", C.c_void_p),
+                ("style_weight", C.c_void_p), ("style_bias", C.c_void_p), ("cin", C.c_int), ("cout", C.c_int), ("upsample", C.c_int),
+                ("res_out", C.c_int)]
 
 
 class BigGANConvDesc(C.Structure):
@@ -244,6 +256,8 @@ SECTION_KERNELS = {
     "linear": "gen_z linear: mapping_layer_tc_kernel (wgmma, fp16 hi/lo x3, bias epilogue, TMA store) for n >= 128",
     "synthesis": "StyledConv chain: tap-GEMM tc_gemm_plain (wgmma) + gather/scatter/blur epilogues",
     "progan": "ProGAN chain: tap-GEMM tc_gemm_plain (wgmma) + pg_gather_kernel (gather, bias, leaky-ReLU, PixelNorm, RGB)",
+    "stylegan": "StyleGAN chain: tap-GEMM tc_gemm_plain (wgmma) + sg_epilogue_kernel (gather / blur, noise, leaky-ReLU, sums) + "
+                "sg_finish_kernel + sg_apply_kernel (InstanceNorm + StyleMod, torgb)",
     "biggan": "BigGAN chain: bb_conv_kernel (fp32 implicit GEMM, BN+ReLU prologue, skip / residual epilogue), attention, RGB",
 }
 
@@ -895,6 +909,88 @@ class PackedProGAN:
             _check(load().gsb_progan_status(_ptr(self.packed), self.desc, self.n_blocks, C.byref(flags)), "gsb_progan_status")
         if flags.value & 1:
             raise NativeError("progan: an operand exceeded fp16 range in the tensor-core path; results are invalid")
+
+
+class PackedStyleGAN:
+    """StyleGAN (v1) synthesis layers (two per block) and torgb packed for the tap-GEMM kernels (gsb_stylegan_pack).
+
+    ``layers``: dicts with conv_weight [co,ci,3,3] (None for the first layer), bias [co], noise [r,r], noise_weight [co],
+    style_weight [2co, dlatent], style_bias [2co] (fp32 tensors), upsample (bool) and res_out (int), in execution order;
+    ``const`` [c0,4,4]: the InputBlock's constant; ``rgb_weight`` [3,c,1,1] / ``rgb_bias`` [3]: torgb."""
+
+    def __init__(self, layers, const: torch.Tensor, rgb_weight: torch.Tensor, rgb_bias: torch.Tensor, dlatent: int = 512):
+        lib = load()
+        self.device = require_cuda(rgb_weight.device)
+        self.n_layers, self.dlatent = len(layers), int(dlatent)
+        self.desc = (StyleGANLayerDesc * self.n_layers)()
+        self.shapes = []                        # (res_out, cout) per layer
+        f32 = lambda t: t.detach().to(self.device, torch.float32).contiguous()
+        keep = []
+        for i, L in enumerate(layers):
+            ts = {k: f32(L[k]) for k in ("bias", "noise", "noise_weight", "style_weight", "style_bias")}
+            if L["conv_weight"] is not None:
+                ts["conv_weight"] = f32(L["conv_weight"])
+            keep.append(ts)
+            co, r = ts["bias"].shape[0], int(L["res_out"])
+            ci = ts["conv_weight"].shape[1] if "conv_weight" in ts else co
+            assert ("conv_weight" in ts) == (i > 0) and ts["noise"].numel() == r * r and ts["noise_weight"].shape == (co,)
+            assert ts["style_weight"].shape == (2 * co, self.dlatent) and ts["style_bias"].shape == (2 * co,)
+            d = self.desc[i]
+            for k, t in ts.items():
+                setattr(d, k, t.data_ptr())
+            d.cin, d.cout, d.upsample, d.res_out = ci, co, int(bool(L["upsample"])), r
+            self.shapes.append((r, co))
+        cst = f32(const).reshape(self.shapes[0][1], 4, 4)
+        rw, rb = f32(rgb_weight).reshape(3, -1), f32(rgb_bias).reshape(3)
+        assert rw.shape[1] == self.shapes[-1][1]
+        nbytes = lib.gsb_stylegan_packed_bytes(self.desc, self.n_layers, self.dlatent)
+        if nbytes == 0:
+            raise NativeError(f"gsb_stylegan_packed_bytes: {lib.gsb_last_error().decode()}")
+        self.packed = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            _check(lib.gsb_stylegan_pack(self.desc, self.n_layers, self.dlatent, _ptr(cst), _ptr(rw), _ptr(rb), _ptr(self.packed),
+                                         self.packed.numel(), _stream()), "gsb_stylegan_pack")
+            torch.cuda.current_stream().synchronize()      # the fp32 copies in `keep` may be freed after this returns
+
+    def out_dims(self, n_run: int) -> int:
+        r, co = self.shapes[n_run - 1]
+        return r * r * co
+
+    def forward(self, w: torch.Tensor, n_run: int, out: torch.Tensor = None, want_act: bool = True, want_rgb: bool = False):
+        """Layers 0 .. n_run-1 for dlatents ``w`` [n, dlatent] (one latent for every layer) or [Lw, n, dlatent] (layer l reads
+        latent l).  Returns (output of layer n_run-1 as fp32 NHWC rows [n, res*res*cout] or None, image as fp32 NHWC
+        [n, res, res, 3] or None; the image needs n_run == n_layers).  ``out`` may be a row-strided 2-D view, e.g. the batch rows
+        of the large-d IPCA buffer."""
+        lib = load()
+        assert w.is_cuda and w.dtype == torch.float32 and w.shape[-1] == self.dlatent and w.dim() in (2, 3)
+        w3 = (w[None] if w.dim() == 2 else w).contiguous()
+        Lw, n = int(w3.shape[0]), int(w3.shape[1])
+        d = self.out_dims(n_run)
+        act = rgb = None
+        if want_act:
+            act = torch.empty((n, d), dtype=torch.float32, device=w.device) if out is None else out
+            assert act.is_cuda and act.dtype == torch.float32 and act.shape == (n, d) and act.stride(1) == 1
+        if want_rgb:
+            res = self.shapes[-1][0]
+            rgb = torch.empty((n, res, res, 3), dtype=torch.float32, device=w.device)
+        if n == 0:
+            return act, rgb
+        ws = scratch.get("stylegan", lib.gsb_stylegan_workspace_bytes(self.desc, n_run, n), w.device)
+        with torch.cuda.device(w.device), instrument.section("stylegan"):
+            _check(lib.gsb_stylegan_forward(_ptr(self.packed), self.desc, self.n_layers, n_run, self.dlatent, _ptr(w3), Lw, n,
+                                            C.c_void_p(act.data_ptr() if act is not None else 0), act.stride(0) if act is not None else 0,
+                                            _ptr(rgb), _ptr(ws), ws.numel(), _stream()), "gsb_stylegan_forward")
+        instrument.count(1)
+        instrument.add_rows("stylegan", n)
+        return act, rgb
+
+    def check(self):
+        flags = C.c_uint(0)
+        with torch.cuda.device(self.device):
+            _check(load().gsb_stylegan_status(_ptr(self.packed), self.desc, self.n_layers, self.dlatent, C.byref(flags)),
+                   "gsb_stylegan_status")
+        if flags.value & 1:
+            raise NativeError("stylegan: an operand exceeded fp16 range in the tensor-core path; results are invalid")
 
 
 def _f32_dev(t, what):

@@ -1,0 +1,553 @@
+// StyleGAN (v1) synthesis network: g_synthesis.blocks.4x4 .. RxR and torgb.
+//
+// Replaces models/stylegan/model.py:270-376 (InputBlock, GSynthesisBlock, LayerEpilogue, G_synthesis.forward) as driven by
+// models/wrappers.py:330-417 (StyleGAN.forward, partial_forward).
+//
+// Layers run in execution order, two per block.  Layer l is
+//     x  ->  conv (l > 0)  ->  + bias  ->  + noise_weight[c] noise[y,x]  ->  leaky-ReLU 0.2  ->  InstanceNorm  ->  StyleMod(w_l)
+// with  layer 0 : x = const (the InputBlock's learned [C, 4, 4] tensor, shared by all samples)
+//       conv    : 3x3, padding 1, weight * sqrt2 / sqrt(9 cin)
+//       up-conv : nearest x2, 3x3 conv, then the [1,2,1] x [1,2,1] / 16 depthwise blur with zero padding of the conv OUTPUT.
+//                 From 128 px on the reference takes the conv_transpose2d branch (model.py:82-91) instead: that equals nearest x2
+//                 followed by a 3x3 correlation with the kernel flipped in both spatial axes, so those layers pack the flipped
+//                 kernel and share the rest of the path.
+// InstanceNorm is per sample and channel over H*W (biased variance, eps 1e-5); StyleMod is  x (s0 + 1) + s1  with
+// [s0 | s1] = w_l (A / sqrt(dlatent))^T + b.  Together:  y = (x - mean) * (rstd (s0 + 1)) + s1,  one affine per (sample, channel).
+//
+// Per layer and chunk of samples:
+//     tap GEMM      Y[b,p,tap,co] = sum_ci (scale W)[co,ci,tap] x[b,p,ci]    (tc_gemm_plain, fp16 hi/lo, wgmma), at the INPUT
+//                                 resolution: nearest x2 only replicates pixels (the formulation of progan.cu)
+//     up gather     U = the up-conv output (up-conv layers only; the blur reads it)
+//     epilogue      gather / blur, bias, noise, leaky-ReLU -> pre-norm activation A (fp32 NHWC) and per-(sample, tile, channel)
+//                   fp64 sums and sums of squares
+//     finish        one warp per (sample, channel): the tiles' sums in a fixed order -> mean and the affine
+//     apply         the affine -> the next layer's operand as fp16 hi/lo, and / or the hooked activation as fp32 NHWC rows with a
+//                   caller-given row stride, and / or (last layer) the 1x1 torgb conv
+// The StyleMod vectors of every layer come from one kernel before the first layer.  No float atomics; every reduction runs in
+// a fixed order inside one sample, so a sample's result does not depend on the batch it is part of.
+//
+// Channel counts: cin and cout are powers of two in [16, 512].  The 16-channel layers of the 1024-px generators run on the same
+// path: the GEMM needs only K % 8 == 0, and its N = 9 cout is padded with zero weight rows to a multiple of 32.
+#include "tc_common.cuh"
+#include <math.h>
+
+namespace gsb {
+
+constexpr int SG_MAX_LAYERS = 18;
+constexpr int64_t SG_CHUNK_ELEMS = (int64_t)2048 * 9 * 512;      // fp32 elements of the largest per-chunk buffer (38 MB)
+constexpr int SG_TILE_PASSES = 8;                                 // pixel passes of one epilogue block (the statistics tile)
+
+static int sg_np(const gsb_stylegan_layer &c) { return (9 * c.cout + 31) / 32 * 32; }           // GEMM N (padded)
+static int sg_res_in(const gsb_stylegan_layer &c) { return c.upsample ? c.res_out / 2 : c.res_out; }
+// up-conv layers from 128 px on run the reference's conv_transpose2d branch: the flipped kernel
+static bool sg_flipped(const gsb_stylegan_layer &c) { return c.upsample && c.res_out >= 128; }
+static int sg_tile_px(const gsb_stylegan_layer &c) {
+    const int hw = c.res_out * c.res_out, ppp = 1024 / c.cout;    // pixels per pass of a 256-thread block
+    return hw < ppp * SG_TILE_PASSES ? hw : ppp * SG_TILE_PASSES;
+}
+static int64_t sg_chunk_samples(const gsb_stylegan_layer &c) {
+    const int64_t hw_in = (int64_t)sg_res_in(c) * sg_res_in(c), hw = (int64_t)c.res_out * c.res_out;
+    int64_t per = hw * c.cout;
+    if (c.conv_weight && hw_in * sg_np(c) > per) per = hw_in * sg_np(c);
+    const int64_t spc = SG_CHUNK_ELEMS / per;
+    return spc < 1 ? 1 : spc;
+}
+
+// ---- packed layout ----------------------------------------------------------------------------------------
+struct SgLayerView {
+    __half *w_hi, *w_lo;      // [np, cin]  row = tap*cout + co (rows >= 9 cout are zero)
+    float *scal;              // [4]: inv_wscale, wscale, absmax
+    float *bias, *noise_w;    // [cout]
+    float *noise;             // [res_out^2]
+    int style_off;            // column of s0 in the style matrix (s1 follows at + cout)
+};
+struct SgView {
+    unsigned *overflow;
+    float *cst;               // [16, c0] NHWC
+    float *style_wt;          // [dlatent, s_total]  A^T / sqrt(dlatent), all layers side by side
+    float *style_b;           // [s_total]
+    int *style_layer;         // [s_total]  layer of each column
+    int s_total;
+    float *rgb_w;             // [3, c_last] / sqrt(c_last)
+    float *rgb_b;             // [3]
+    SgLayerView L[SG_MAX_LAYERS];
+    size_t bytes;
+};
+static SgView sg_view(void *base, const gsb_stylegan_layer *layers, int n_layers, int dlatent) {
+    SgView v;
+    char *p = reinterpret_cast<char *>(base);
+    size_t off = 0;
+    auto take = [&](size_t bytes) { char *q = p + off; off += align_up(bytes, 256); return q; };
+    v.s_total = 0;
+    for (int l = 0; l < n_layers; ++l) v.s_total += 2 * layers[l].cout;
+    v.overflow = (unsigned *)take(256);
+    v.cst = (float *)take((size_t)16 * layers[0].cout * 4);
+    v.style_wt = (float *)take((size_t)dlatent * v.s_total * 4);
+    v.style_b = (float *)take((size_t)v.s_total * 4);
+    v.style_layer = (int *)take((size_t)v.s_total * 4);
+    v.rgb_w = (float *)take((size_t)3 * layers[n_layers - 1].cout * 4);
+    v.rgb_b = (float *)take(16);
+    int soff = 0;
+    for (int l = 0; l < n_layers; ++l) {
+        const gsb_stylegan_layer &c = layers[l];
+        const size_t wcount = c.conv_weight ? (size_t)sg_np(c) * c.cin : 0;
+        v.L[l].w_hi = (__half *)take(wcount * 2);
+        v.L[l].w_lo = (__half *)take(wcount * 2);
+        v.L[l].scal = (float *)take(16);
+        v.L[l].bias = (float *)take((size_t)c.cout * 4);
+        v.L[l].noise_w = (float *)take((size_t)c.cout * 4);
+        v.L[l].noise = (float *)take((size_t)c.res_out * c.res_out * 4);
+        v.L[l].style_off = soff;
+        soff += 2 * c.cout;
+    }
+    v.bytes = off;
+    return v;
+}
+
+static bool sg_pow2(int x, int lo, int hi) { return x >= lo && x <= hi && (x & (x - 1)) == 0; }
+
+static int sg_check(const gsb_stylegan_layer *layers, int n_layers, int dlatent) {
+    GSB_CHECK_ARG(layers && n_layers >= 1 && n_layers <= SG_MAX_LAYERS, "stylegan: need 1..%d layers", SG_MAX_LAYERS);
+    GSB_CHECK_ARG(dlatent >= 1 && dlatent <= 4096, "stylegan: bad dlatent %d", dlatent);
+    for (int l = 0; l < n_layers; ++l) {
+        const gsb_stylegan_layer &c = layers[l];
+        GSB_CHECK_ARG(sg_pow2(c.cout, 16, 512) && (l == 0 || sg_pow2(c.cin, 16, 512)),
+                      "stylegan: layer %d needs cin, cout powers of two in [16, 512] (cin=%d cout=%d)", l, c.cin, c.cout);
+        if (l == 0) GSB_CHECK_ARG(!c.conv_weight && !c.upsample && c.res_out == 4, "stylegan: layer 0 is the 4x4 constant input");
+        else GSB_CHECK_ARG(c.conv_weight && c.cin == layers[l - 1].cout && sg_res_in(c) == layers[l - 1].res_out && c.res_out <= 1024,
+                           "stylegan: layer %d does not chain", l);
+    }
+    return GSB_OK;
+}
+
+// ---- pack kernels ---------------------------------------------------------------------------------------
+__global__ void sg_absmax_kernel(const float *__restrict__ x, int64_t count, float scale, float *__restrict__ out) {
+    float m = 0.f;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
+        m = fmaxf(m, fabsf(x[i] * scale));
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<int *>(out), __float_as_int(m));      // (max of non-negative floats: exact)
+}
+// scal[2] = absmax -> scal[1] = 2^s, scal[0] = 2^-s with the largest |w 2^s| in [8192, 16384)
+__global__ void sg_pick_scale_kernel(float *__restrict__ scal) {
+    float m = scal[2];
+    if (!(m > 0.f)) m = 1.f;
+    int e = 0;
+    frexpf(m, &e);
+    scal[1] = ldexpf(1.f, 14 - e);
+    scal[0] = ldexpf(1.f, e - 14);
+}
+// W[co,ci,3,3] -> rows (tap, co), K-major over ci, times scale*2^s, split into fp16 hi/lo; `flip`: tap t -> 8-t (both axes)
+__global__ void sg_weight_pack_kernel(const float *__restrict__ W, int cout, int cin, int flip, float scale,
+                                      const float *__restrict__ scal, __half *__restrict__ hi, __half *__restrict__ lo) {
+    const float ws = scal[1];
+    const int64_t total = (int64_t)cout * cin * 9;
+    for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+        const int t = (int)(idx % 9);
+        const int64_t cc = idx / 9;
+        const int co = (int)(cc / cin), ci = (int)(cc % cin);
+        const int64_t o = ((int64_t)(flip ? 8 - t : t) * cout + co) * cin + ci;
+        tc::split1(W[idx] * scale * ws, hi[o], lo[o]);
+    }
+}
+// A [rows, K] (StyleMod lin.weight) -> dst[k * ld + r] = A[r, k] * scale; column `layer` tag per row
+__global__ void sg_transpose_scale_kernel(const float *__restrict__ A, int rows, int K, float scale, float *__restrict__ dst, int64_t ld,
+                                          int *__restrict__ tag, int layer) {
+    for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < (int64_t)rows * K; idx += (int64_t)gridDim.x * blockDim.x) {
+        const int r = (int)(idx / K), k = (int)(idx % K);
+        dst[(int64_t)k * ld + r] = A[idx] * scale;
+        if (k == 0) tag[r] = layer;
+    }
+}
+__global__ void sg_scale_copy_kernel(const float *__restrict__ src, int64_t count, float scale, float *__restrict__ dst) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
+        dst[i] = src[i] * scale;
+}
+// const [C, 16] (NCHW of one sample) -> [16, C]
+__global__ void sg_const_pack_kernel(const float *__restrict__ src, int C, float *__restrict__ dst) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 16 * C; i += gridDim.x * blockDim.x) dst[(i % 16) * C + i / 16] = src[i];
+}
+
+// ---- forward kernels ------------------------------------------------------------------------------------
+// S[b, j] = w_{layer(j)}[b] . style_wt[:, j] + style_b[j] for columns j < s_run; one thread per (b, j), k in order.
+// w_layers == 1: one latent for every layer; otherwise w [w_layers, n, dlatent] and layer l reads latent l.
+__global__ void __launch_bounds__(256)
+sg_style_kernel(const float *__restrict__ w, int w_layers, int64_t n, int dlatent, const float *__restrict__ wt,
+                const float *__restrict__ bias, const int *__restrict__ tag, int s_total, int s_run, float *__restrict__ S) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t b = blockIdx.y;
+    if (j >= s_run) return;
+    const int li = w_layers == 1 ? 0 : tag[j];
+    const float *wr = w + ((int64_t)li * n + b) * dlatent;
+    float acc = 0.f;
+    for (int k = 0; k < dlatent; ++k) acc = fmaf(wr[k], wt[(int64_t)k * s_total + j], acc);
+    S[b * s_run + j] = acc + bias[j];
+}
+
+// the 3x3 conv outputs of an up-conv layer (before the blur): out[b,y,x,co] = sum_tap Y[b,((y+ky-1)>>1, (x+kx-1)>>1),tap,co] over
+// 0 <= y+ky-1, x+kx-1 < R; Y at the input resolution R/2 with row length np.  One thread per 4 channels of an output pixel.
+__global__ void __launch_bounds__(256)
+sg_up_gather_kernel(const float *__restrict__ Y, int64_t nb, int R, int c, int np, float *__restrict__ U) {
+    const int cq = c >> 2;
+    const int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (idx >= nb * R * R * cq) return;
+    const int q = (int)(idx % cq);
+    const int64_t pixg = idx / cq;
+    const int x = (int)(pixg % R), y = (int)((pixg / R) % R);
+    const int64_t b = pixg / ((int64_t)R * R);
+    const int H = R >> 1;
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int ky = 0; ky < 3; ++ky) {
+        const int yy = y + ky - 1;
+        if (yy < 0 || yy >= R) continue;
+#pragma unroll
+        for (int kx = 0; kx < 3; ++kx) {
+            const int xx = x + kx - 1;
+            if (xx < 0 || xx >= R) continue;
+            const float4 v = *reinterpret_cast<const float4 *>(Y + ((b * H + (yy >> 1)) * H + (xx >> 1)) * (int64_t)np + (ky * 3 + kx) * c + 4 * q);
+            acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+        }
+    }
+    *reinterpret_cast<float4 *>(U + pixg * c + 4 * q) = acc;
+}
+
+// MODE 0: the constant input (src = const [16, c]); 1: stride-1 3x3 gather (src = Y [nb*R*R, np]); 2: the blur of the up-conv
+// output (src = U [nb, R, R, c], zero padding).  Then + bias + noise_w noise[p], leaky-ReLU -> A, and the tile's fp64 sums.
+// Grid (tiles, nb), 256 threads: thread = (pixel lane pl, channel quad q); a block covers `tile` consecutive pixels of one sample.
+template <int MODE>
+__global__ void __launch_bounds__(256)
+sg_epilogue_kernel(const float *__restrict__ src, int R, int c, int np, int tile, const float *__restrict__ bias,
+                   const float *__restrict__ noise_w, const float *__restrict__ noise, float *__restrict__ A, double *__restrict__ part) {
+    __shared__ double red[2][256][4];
+    const int cq = c >> 2, ppp = 256 / cq;
+    const int q = threadIdx.x % cq, pl = threadIdx.x / cq;
+    const int64_t b = blockIdx.y;
+    const int hw = R * R;
+    const float4 bs = *reinterpret_cast<const float4 *>(bias + 4 * q);
+    const float4 nw = *reinterpret_cast<const float4 *>(noise_w + 4 * q);
+    double s[4] = {0.0, 0.0, 0.0, 0.0}, ss[4] = {0.0, 0.0, 0.0, 0.0};
+    for (int p = blockIdx.x * tile + pl; p < (blockIdx.x + 1) * tile; p += ppp) {
+        const int y = p / R, x = p % R;
+        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (MODE == 0) {
+            acc = *reinterpret_cast<const float4 *>(src + (int64_t)p * c + 4 * q);
+        } else {
+#pragma unroll
+            for (int ky = 0; ky < 3; ++ky) {
+                const int yy = y + ky - 1;
+                if (yy < 0 || yy >= R) continue;
+#pragma unroll
+                for (int kx = 0; kx < 3; ++kx) {
+                    const int xx = x + kx - 1;
+                    if (xx < 0 || xx >= R) continue;
+                    if (MODE == 1) {
+                        const float4 v = *reinterpret_cast<const float4 *>(src + ((b * R + yy) * R + xx) * (int64_t)np + (ky * 3 + kx) * c + 4 * q);
+                        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+                    } else {
+                        const float wgt = (float)((ky == 1 ? 2 : 1) * (kx == 1 ? 2 : 1)) * 0.0625f;
+                        const float4 v = *reinterpret_cast<const float4 *>(src + ((b * R + yy) * R + xx) * (int64_t)c + 4 * q);
+                        acc.x = fmaf(wgt, v.x, acc.x); acc.y = fmaf(wgt, v.y, acc.y); acc.z = fmaf(wgt, v.z, acc.z); acc.w = fmaf(wgt, v.w, acc.w);
+                    }
+                }
+            }
+        }
+        const float nz = noise[p];
+        float f[4] = {acc.x + bs.x, acc.y + bs.y, acc.z + bs.z, acc.w + bs.w};
+        const float g[4] = {nw.x, nw.y, nw.z, nw.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            f[k] = fmaf(g[k], nz, f[k]);
+            f[k] = (f[k] >= 0.f) ? f[k] : 0.2f * f[k];
+            s[k] += (double)f[k];
+            ss[k] += (double)f[k] * (double)f[k];
+        }
+        *reinterpret_cast<float4 *>(A + (b * hw + p) * (int64_t)c + 4 * q) = make_float4(f[0], f[1], f[2], f[3]);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) { red[0][threadIdx.x][k] = s[k]; red[1][threadIdx.x][k] = ss[k]; }
+    __syncthreads();
+    if (pl == 0) {
+        for (int j = 1; j < ppp; ++j)
+#pragma unroll
+            for (int k = 0; k < 4; ++k) { s[k] += red[0][j * cq + q][k]; ss[k] += red[1][j * cq + q][k]; }
+        double *o = part + ((b * gridDim.x + blockIdx.x) * (int64_t)c + 4 * q) * 2;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) { o[2 * k] = s[k]; o[2 * k + 1] = ss[k]; }
+    }
+}
+
+// one warp per (sample, channel): tiles summed lane-strided in order, then a fixed shuffle tree.  aff[b, c] = {mean, rstd (s0+1), s1}
+__global__ void __launch_bounds__(256)
+sg_finish_kernel(const double *__restrict__ part, int64_t nb, int c, int tiles, int hw, const float *__restrict__ S, int64_t s_ld,
+                 int s_off, float4 *__restrict__ aff) {
+    const int64_t wid = blockIdx.x * (int64_t)(blockDim.x >> 5) + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (wid >= nb * c) return;
+    const int64_t b = wid / c;
+    const int ch = (int)(wid % c);
+    double s = 0.0, ss = 0.0;
+    for (int t = lane; t < tiles; t += 32) {
+        const double *o = part + ((b * tiles + t) * (int64_t)c + ch) * 2;
+        s += o[0];
+        ss += o[1];
+    }
+    s = warp_sum(s);
+    ss = warp_sum(ss);
+    if (lane == 0) {
+        const double mean = s / hw;
+        double var = ss / hw - mean * mean;
+        var = var > 0.0 ? var : 0.0;
+        const float rstd = (float)(1.0 / sqrt(var + 1e-5));
+        const float s0 = S[b * s_ld + s_off + ch], s1 = S[b * s_ld + s_off + c + ch];
+        aff[wid] = make_float4((float)mean, rstd * (s0 + 1.f), s1, 0.f);
+    }
+}
+
+// Sum of v over the c/4 threads that hold one pixel's channels (consecutive threads, c/4 a power of two that divides the block
+// size; every thread of the block calls this): shuffles inside a warp, then for c >= 256 the warps of the pixel in warp order.
+__device__ __forceinline__ float sg_pixel_sum(float v, int cq) {
+    const int span = cq < 32 ? cq : 32;
+    for (int off = span >> 1; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+    if (cq > 32) {
+        __shared__ float red[8];
+        const int wib = threadIdx.x >> 5, wpp = cq >> 5;
+        __syncthreads();
+        if ((threadIdx.x & 31) == 0) red[wib] = v;
+        __syncthreads();
+        const int w0 = wib / wpp * wpp;
+        v = 0.f;
+        for (int k = 0; k < wpp; ++k) v += red[w0 + k];
+    }
+    return v;
+}
+
+struct SgApply {
+    const float *A;              // [nb, hw, c] pre-norm activation (chunk-local)
+    const float4 *aff;           // [nb, c]
+    __half *out_hi, *out_lo;     // [nb, hw, c] (chunk-local) operand of the next layer, or nullptr
+    float *out_f32;              // hooked layer: row b at out_f32 + b*ld, or nullptr
+    int64_t ld;
+    const float *rgb_w, *rgb_b;  // torgb: [3, c] (scaled) and [3], or nullptr
+    float *rgb_out;              // [nb, hw, 3] (chunk-local)
+    unsigned *overflow;
+};
+// y = (x - mean) a + s1 for 4 channels of one pixel -> the enabled outputs.  Threads past the end take part in the RGB sums.
+__global__ void __launch_bounds__(256)
+sg_apply_kernel(SgApply e, int64_t nb, int hw, int c) {
+    const int cq = c >> 2;
+    const int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    const bool valid = idx < nb * hw * cq;
+    const int q = (int)(idx % cq);
+    const int64_t pixg = idx / cq;
+    const int64_t b = pixg / hw;
+    const int pix = (int)(pixg % hw);
+    float y[4] = {0.f, 0.f, 0.f, 0.f};
+    if (valid) {
+        const float4 x = *reinterpret_cast<const float4 *>(e.A + pixg * c + 4 * q);
+        const float xv[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const float4 a = e.aff[b * c + 4 * q + k];
+            y[k] = fmaf(xv[k] - a.x, a.y, a.z);
+        }
+        if (e.out_f32) *reinterpret_cast<float4 *>(e.out_f32 + b * e.ld + (int64_t)pix * c + 4 * q) = make_float4(y[0], y[1], y[2], y[3]);
+        if (e.out_hi) {
+            uint2 ph, pl;
+            const bool ovf = tc::split4(y, ph, pl);
+            *reinterpret_cast<uint2 *>(e.out_hi + pixg * c + 4 * q) = ph;
+            *reinterpret_cast<uint2 *>(e.out_lo + pixg * c + 4 * q) = pl;
+            if (ovf) atomicOr(e.overflow, 1u);
+        }
+    }
+    if (e.rgb_w) {
+#pragma unroll
+        for (int o = 0; o < 3; ++o) {
+            const float4 wv = *reinterpret_cast<const float4 *>(e.rgb_w + (int64_t)o * c + 4 * q);
+            const float r = sg_pixel_sum((y[0] * wv.x + y[1] * wv.y) + (y[2] * wv.z + y[3] * wv.w), cq);
+            if (valid && q == 0) e.rgb_out[pixg * 3 + o] = r + e.rgb_b[o];
+        }
+    }
+}
+
+// ---- workspace --------------------------------------------------------------------------------------------
+struct SgWs {
+    float *S;               // [n, s_run]
+    __half *act[2][2];      // [ping-pong][hi/lo]
+    float *Y, *U, *A;
+    double *part;
+    float4 *aff;
+    unsigned *queue;        // tile queue of the tap GEMM launches
+    size_t bytes;
+};
+static SgWs sg_ws(void *base, const gsb_stylegan_layer *layers, int n_run, int64_t n) {
+    SgWs w;
+    char *p = reinterpret_cast<char *>(base);
+    size_t off = 0;
+    auto take = [&](size_t bytes) { char *q = p + off; off += align_up(bytes, 256); return q; };
+    size_t s_run = 0, act_elems = 64, y_elems = 64, a_elems = 64, part_elems = 64, aff_elems = 64;
+    for (int l = 0; l < n_run; ++l) {
+        const gsb_stylegan_layer &c = layers[l];
+        s_run += 2 * c.cout;
+        const size_t hw = (size_t)c.res_out * c.res_out, hw_in = (size_t)sg_res_in(c) * sg_res_in(c);
+        if (l + 1 < n_run) act_elems = act_elems > n * hw * c.cout ? act_elems : n * hw * c.cout;
+        const size_t spc = (size_t)(sg_chunk_samples(c) < n ? sg_chunk_samples(c) : n);
+        if (c.conv_weight) y_elems = y_elems > spc * hw_in * sg_np(c) ? y_elems : spc * hw_in * sg_np(c);
+        a_elems = a_elems > spc * hw * c.cout ? a_elems : spc * hw * c.cout;
+        const size_t pe = spc * (hw / sg_tile_px(c)) * c.cout * 2;
+        part_elems = part_elems > pe ? part_elems : pe;
+        aff_elems = aff_elems > spc * c.cout ? aff_elems : spc * c.cout;
+    }
+    w.S = (float *)take((size_t)n * s_run * 4);
+    for (int a = 0; a < 2; ++a)
+        for (int h = 0; h < 2; ++h) w.act[a][h] = (__half *)take(act_elems * 2);
+    w.Y = (float *)take(y_elems * 4);
+    w.U = (float *)take(a_elems * 4);
+    w.A = (float *)take(a_elems * 4);
+    w.part = (double *)take(part_elems * 8);
+    w.aff = (float4 *)take(aff_elems * 16);
+    w.queue = (unsigned *)take(sizeof(unsigned));
+    w.bytes = off;
+    return w;
+}
+
+}  // namespace gsb
+
+extern "C" size_t gsb_stylegan_packed_bytes(const gsb_stylegan_layer *layers, int n_layers, int dlatent) {
+    if (gsb::sg_check(layers, n_layers, dlatent)) return 0;
+    return gsb::sg_view(nullptr, layers, n_layers, dlatent).bytes;
+}
+
+extern "C" int gsb_stylegan_pack(const gsb_stylegan_layer *layers, int n_layers, int dlatent, const float *d_const,
+                                 const float *d_rgb_weight, const float *d_rgb_bias, void *d_packed, size_t packed_bytes,
+                                 gsb_stream_t stream) {
+    using namespace gsb;
+    if (int r = sg_check(layers, n_layers, dlatent)) return r;
+    GSB_CHECK_ARG(d_const && d_rgb_weight && d_rgb_bias && d_packed, "stylegan_pack: null pointer");
+    SgView v = sg_view(d_packed, layers, n_layers, dlatent);
+    if (packed_bytes < v.bytes) { set_error("stylegan_pack: buffer too small (%zu < %zu)", packed_bytes, v.bytes); return GSB_ERR_WORKSPACE; }
+    cudaStream_t st = (cudaStream_t)stream;
+    GSB_CHECK_CUDA(cudaMemsetAsync(d_packed, 0, v.bytes, st));
+    sg_const_pack_kernel<<<8, 256, 0, st>>>(d_const, layers[0].cout, v.cst);
+    GSB_CHECK_LAUNCH();
+    for (int l = 0; l < n_layers; ++l) {
+        const gsb_stylegan_layer &c = layers[l];
+        GSB_CHECK_ARG(c.bias && c.noise && c.noise_weight && c.style_weight && c.style_bias,
+                      "stylegan_pack: layer %d has a null parameter pointer", l);
+        if (c.conv_weight) {
+            // MyConv2d with use_wscale, gain sqrt2, lrmul 1: w_mul = sqrt2 / sqrt(cin * 9) (model.py:51-62)
+            const float scale = (float)(sqrt(2.0) / sqrt(9.0 * c.cin));
+            const int64_t wcount = (int64_t)c.cout * c.cin * 9;
+            sg_absmax_kernel<<<128, 256, 0, st>>>(c.conv_weight, wcount, scale, v.L[l].scal + 2);
+            GSB_CHECK_LAUNCH();
+            sg_pick_scale_kernel<<<1, 1, 0, st>>>(v.L[l].scal);
+            GSB_CHECK_LAUNCH();
+            sg_weight_pack_kernel<<<256, 256, 0, st>>>(c.conv_weight, c.cout, c.cin, sg_flipped(c) ? 1 : 0, scale, v.L[l].scal,
+                                                       v.L[l].w_hi, v.L[l].w_lo);
+            GSB_CHECK_LAUNCH();
+        }
+        sg_scale_copy_kernel<<<4, 256, 0, st>>>(c.bias, c.cout, 1.0f, v.L[l].bias);
+        GSB_CHECK_LAUNCH();
+        sg_scale_copy_kernel<<<4, 256, 0, st>>>(c.noise_weight, c.cout, 1.0f, v.L[l].noise_w);
+        GSB_CHECK_LAUNCH();
+        sg_scale_copy_kernel<<<64, 256, 0, st>>>(c.noise, (int64_t)c.res_out * c.res_out, 1.0f, v.L[l].noise);
+        GSB_CHECK_LAUNCH();
+        // StyleMod lin: MyLinear(dlatent, 2 cout, gain 1, use_wscale): w_mul = 1 / sqrt(dlatent), b_mul = 1 (model.py:121-131)
+        sg_transpose_scale_kernel<<<256, 256, 0, st>>>(c.style_weight, 2 * c.cout, dlatent, (float)(1.0 / sqrt((double)dlatent)),
+                                                       v.style_wt + v.L[l].style_off, v.s_total, v.style_layer + v.L[l].style_off, l);
+        GSB_CHECK_LAUNCH();
+        sg_scale_copy_kernel<<<4, 256, 0, st>>>(c.style_bias, 2 * c.cout, 1.0f, v.style_b + v.L[l].style_off);
+        GSB_CHECK_LAUNCH();
+    }
+    const int cl = layers[n_layers - 1].cout;
+    // torgb: MyConv2d(c, 3, 1, gain 1, use_wscale): w_mul = 1 / sqrt(c)
+    sg_scale_copy_kernel<<<4, 256, 0, st>>>(d_rgb_weight, (int64_t)3 * cl, (float)(1.0 / sqrt((double)cl)), v.rgb_w);
+    GSB_CHECK_LAUNCH();
+    sg_scale_copy_kernel<<<1, 32, 0, st>>>(d_rgb_bias, 3, 1.0f, v.rgb_b);
+    GSB_CHECK_LAUNCH();
+    return GSB_OK;
+}
+
+extern "C" size_t gsb_stylegan_workspace_bytes(const gsb_stylegan_layer *layers, int n_run, int64_t n) {
+    if (!layers || n_run < 1 || n_run > gsb::SG_MAX_LAYERS || n < 1) return 0;
+    return gsb::sg_ws(nullptr, layers, n_run, n).bytes;
+}
+
+extern "C" int gsb_stylegan_forward(const void *d_packed, const gsb_stylegan_layer *layers, int n_layers, int n_run, int dlatent,
+                                    const float *d_w, int w_layers, int64_t n, float *d_act_out, int64_t ld_act, float *d_rgb_out,
+                                    void *d_workspace, size_t workspace_bytes, gsb_stream_t stream) {
+    using namespace gsb;
+    if (int r = sg_check(layers, n_layers, dlatent)) return r;
+    GSB_CHECK_ARG(d_packed && d_w && d_workspace && (d_act_out || d_rgb_out), "stylegan: null pointer");
+    GSB_CHECK_ARG(n_run >= 1 && n_run <= n_layers && n >= 0, "stylegan: n_run / n out of range");
+    GSB_CHECK_ARG(w_layers == 1 || w_layers >= n_run, "stylegan: w_layers must be 1 or cover every layer run (%d < %d)", w_layers, n_run);
+    GSB_CHECK_ARG(!d_rgb_out || n_run == n_layers, "stylegan: the image needs every layer (n_run == n_layers)");
+    if (n == 0) return GSB_OK;
+    GSB_CHECK_ARG(n <= 65535, "stylegan: at most 65535 samples per call (n = %lld)", (long long)n);
+    const gsb_stylegan_layer &last = layers[n_run - 1];
+    GSB_CHECK_ARG(!d_act_out || (ld_act >= (int64_t)last.res_out * last.res_out * last.cout && ld_act % 4 == 0), "stylegan: bad ld_act");
+    SgView v = sg_view(const_cast<void *>(d_packed), layers, n_layers, dlatent);
+    SgWs w = sg_ws(d_workspace, layers, n_run, n);
+    if (workspace_bytes < w.bytes) { set_error("stylegan: workspace too small (%zu < %zu)", workspace_bytes, w.bytes); return GSB_ERR_WORKSPACE; }
+    cudaStream_t st = (cudaStream_t)stream;
+
+    int s_run = 0;
+    for (int l = 0; l < n_run; ++l) s_run += 2 * layers[l].cout;
+    sg_style_kernel<<<dim3((unsigned)((s_run + 255) / 256), (unsigned)n), 256, 0, st>>>(d_w, w_layers, n, dlatent, v.style_wt, v.style_b,
+                                                                                       v.style_layer, v.s_total, s_run, w.S);
+    GSB_CHECK_LAUNCH();
+    for (int l = 0; l < n_run; ++l) {
+        const gsb_stylegan_layer &c = layers[l];
+        const int dst = l & 1;                                         // layer l reads act[dst ^ 1], writes act[dst]
+        const __half *a_hi = w.act[dst ^ 1][0], *a_lo = w.act[dst ^ 1][1];
+        const bool is_last = (l == n_run - 1);
+        const int R = c.res_out, H = sg_res_in(c), hw = R * R, hw_in = H * H, np = sg_np(c), tile = sg_tile_px(c), tiles = hw / tile;
+        const int64_t spc = sg_chunk_samples(c);
+        for (int64_t b0 = 0; b0 < n; b0 += spc) {
+            const int64_t nb = (b0 + spc <= n) ? spc : (n - b0);
+            const dim3 egrid((unsigned)tiles, (unsigned)nb);
+            if (!c.conv_weight) {
+                sg_epilogue_kernel<0><<<egrid, 256, 0, st>>>(v.cst, R, c.cout, 0, tile, v.L[l].bias, v.L[l].noise_w, v.L[l].noise, w.A, w.part);
+            } else {
+                if (int r = tc_gemm_plain(a_hi + b0 * hw_in * c.cin, a_lo + b0 * hw_in * c.cin, nb * hw_in, c.cin, v.L[l].w_hi, v.L[l].w_lo,
+                                          np, v.L[l].scal, w.Y, v.overflow, w.queue, 0, st)) return r;
+                if (c.upsample) {
+                    const int64_t total = nb * hw * (c.cout / 4);
+                    sg_up_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(w.Y, nb, R, c.cout, np, w.U);
+                    GSB_CHECK_LAUNCH();
+                    sg_epilogue_kernel<2><<<egrid, 256, 0, st>>>(w.U, R, c.cout, np, tile, v.L[l].bias, v.L[l].noise_w, v.L[l].noise, w.A, w.part);
+                } else {
+                    sg_epilogue_kernel<1><<<egrid, 256, 0, st>>>(w.Y, R, c.cout, np, tile, v.L[l].bias, v.L[l].noise_w, v.L[l].noise, w.A, w.part);
+                }
+            }
+            GSB_CHECK_LAUNCH();
+            sg_finish_kernel<<<(unsigned)((nb * c.cout + 7) / 8), 256, 0, st>>>(w.part, nb, c.cout, tiles, hw, w.S + b0 * s_run, s_run,
+                                                                               v.L[l].style_off, w.aff);
+            GSB_CHECK_LAUNCH();
+            SgApply e;
+            e.A = w.A;
+            e.aff = w.aff;
+            e.out_hi = is_last ? nullptr : w.act[dst][0] + b0 * hw * c.cout;
+            e.out_lo = is_last ? nullptr : w.act[dst][1] + b0 * hw * c.cout;
+            e.out_f32 = (is_last && d_act_out) ? d_act_out + b0 * ld_act : nullptr;
+            e.ld = ld_act;
+            e.rgb_w = (is_last && d_rgb_out) ? v.rgb_w : nullptr;
+            e.rgb_b = v.rgb_b;
+            e.rgb_out = (is_last && d_rgb_out) ? d_rgb_out + b0 * hw * 3 : nullptr;
+            e.overflow = v.overflow;
+            const int64_t total = nb * hw * (c.cout / 4);
+            sg_apply_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(e, nb, hw, c.cout);
+            GSB_CHECK_LAUNCH();
+        }
+    }
+    return GSB_OK;
+}
+
+extern "C" int gsb_stylegan_status(const void *d_packed, const gsb_stylegan_layer *layers, int n_layers, int dlatent, unsigned *h_flags) {
+    using namespace gsb;
+    if (int r = sg_check(layers, n_layers, dlatent)) return r;
+    GSB_CHECK_ARG(d_packed && h_flags, "stylegan_status: null pointer");
+    SgView v = sg_view(const_cast<void *>(d_packed), layers, n_layers, dlatent);
+    GSB_CHECK_CUDA(cudaMemcpy(h_flags, v.overflow, sizeof(unsigned), cudaMemcpyDeviceToHost));
+    return GSB_OK;
+}

@@ -526,6 +526,214 @@ class ProGAN(BaseModel):
         return self.model.packed().forward(self._single(x), n_run, out=out)[0]
 
 
+class StyleGAN(BaseModel):
+    """wrappers.py:270-436 (StyleGAN v1).  ``g_mapping`` runs the packed mapping kernels, the synthesis blocks the fused chain of
+    csrc/stylegan.cu.  Hookable layers: ``g_mapping`` and the blocks ``g_synthesis.blocks.RxR``.  Checkpoint:
+    ``$GANCONTROL_CHECKPOINT_DIR/stylegan/stylegan_<class>_<res>.pt`` (the reference's ``StyleGAN_G`` state dict; there is no network
+    to download it and no TensorFlow to convert a ``.pkl``); without one, ``random_init=<seed>`` (or env GANSPACE_B200_RANDOM_INIT)
+    builds ``stylegan.random_init(seed)``."""
+
+    CONFIGS = {"ffhq": 1024, "celebahq": 1024, "bedrooms": 256, "cars": 512, "cats": 256, "vases": 1024, "wikiart": 512,
+               "fireworks": 512, "abstract": 512, "anime": 512, "ukiyo-e": 512}
+    # deepest feature map get_or_compute decomposes (blocks.32x32, 512 x 32 x 32), the bound ProGAN uses: the large-d engine's
+    # stacked matrix takes (components + max(B, 2000, 3 components) + 1) x d x 4 bytes in HBM
+    MAX_DECOMPOSITION_DIMS = 524_288
+
+    def __init__(self, device, class_name, truncation=1.0, use_w=False, random_init=None):
+        super().__init__("StyleGAN", class_name or "ffhq")
+        assert self.outclass in self.CONFIGS, \
+            f'Invalid StyleGAN class {self.outclass}, should be one of [{", ".join(self.CONFIGS.keys())}]'
+        self.device = _native.require_cuda(device)
+        self.w_primary = use_w
+        self.resolution = self.CONFIGS[self.outclass]
+        self.name = f"StyleGAN-{self.outclass}"
+        self.has_latent_residual = True
+        self._random_init = random_init
+        self.load_model()
+        self.set_noise_seed(0)
+
+    def latent_space_name(self):
+        return "W" if self.w_primary else "Z"
+
+    def use_w(self):
+        self.w_primary = True
+
+    def use_z(self):
+        self.w_primary = False
+
+    def load_model(self):
+        from . import stylegan
+        root = os.environ.get("GANCONTROL_CHECKPOINT_DIR", Path(__file__).parent / "checkpoints")
+        checkpoint = Path(root) / f"stylegan/stylegan_{self.outclass}_{self.resolution}.pt"
+        seed = self._random_init
+        if seed is None and os.environ.get("GANSPACE_B200_RANDOM_INIT"):
+            seed = int(os.environ["GANSPACE_B200_RANDOM_INIT"])
+        if checkpoint.is_file() and seed is None:
+            self.model = stylegan.StyleGAN_G(self.resolution)
+            self.model.load_state_dict(torch.load(checkpoint, map_location="cpu"))
+            self.model = self.model.to(self.device)
+        elif seed is not None:
+            self.model = stylegan.random_init(seed, self.resolution).to(self.device)
+        elif checkpoint.with_suffix(".pkl").is_file():
+            raise RuntimeError(f"StyleGAN: {checkpoint.with_suffix('.pkl')} is a TensorFlow checkpoint; converting it needs TensorFlow "
+                               f"(the reference's StyleGAN_G.export_from_tf), which is not part of this package: convert it to {checkpoint}")
+        else:
+            raise RuntimeError(f"StyleGAN checkpoint {checkpoint} not found and no network access to download it; pass "
+                               "random_init=<seed> (or set GANSPACE_B200_RANDOM_INIT) for random-init weights")
+
+    def get_latent_shape(self):
+        """As StyleGAN2.get_latent_shape: the reference's sample_latent(1) consumes one draw of the global NumPy stream."""
+        _global_seed()
+        return (1, 512)
+
+    def get_max_latents(self):
+        return 18
+
+    def set_output_class(self, new_class):
+        if self.outclass != new_class:
+            raise RuntimeError("StyleGAN: cannot change output class without reloading")
+
+    def set_noise_seed(self, seed):
+        """wrappers.py:419-434: every NoiseLayer gets ``torch.randn(1, 1, H, W)`` right after ``manual_seed(seed)`` (so all maps of
+        one resolution are equal), drawn on the host and then moved to the device."""
+        for name, m in self.model.g_synthesis.named_modules(prefix="g_synthesis"):
+            if type(m).__name__ == "NoiseLayer":
+                H, W = [int(s) for s in name.split(".")[2].split("x")]
+                torch.random.manual_seed(seed)
+                m.noise = torch.randn(1, 1, H, W, dtype=torch.float32).to(self.device)
+
+    # ---- latents ----------------------------------------------------------------------------------------
+    def sample_latent(self, n_samples=1, seed=None, truncation=None):
+        if seed is None:
+            seed = _global_seed()
+        z = _native.legacy_normal([seed], 512 * n_samples, self.device).view(n_samples, 512)
+        if self.w_primary:
+            z = self.model.g_mapping(z)            # a module call: the g_mapping hook fires here in W mode, as in the reference
+        return z
+
+    def draw_z_async(self, n_samples, seed):
+        """The Z stream of ``sample_latent(n_samples, seed=seed)`` generated on a side stream (StyleGAN2.draw_z_async)."""
+        return StyleGAN2.draw_z_async(self, n_samples, seed)
+
+    def z_to_latent(self, z):
+        return self.model.g_mapping.packed().forward(z) if self.w_primary else z
+
+    def sample_latents_multi(self, n_samples, seeds, out=None, lazy=False):
+        """Several ``sample_latent(n_samples, seed=s)`` calls in one RNG launch (the decomposition driver's producer); no hooks fire.
+        ``lazy=True``: returns (latents, ensure) where ``ensure(row_end)`` maps rows [0, row_end) to W in place (W mode)."""
+        S = len(seeds)
+        z = _native.legacy_normal(list(seeds), 512 * n_samples, self.device,
+                                  out=None if out is None else out.view(S, 512 * n_samples),
+                                  parts=_native.split_parts(512 * n_samples)).view(S * n_samples, 512)
+        packed = self.model.g_mapping.packed() if self.w_primary else None
+        if not lazy:
+            return z if packed is None else packed.forward(z, out=z)
+        state = {"done": 0}
+
+        def ensure(row_end):
+            a, b = state["done"], min(row_end, z.shape[0])
+            if packed is not None and b > a:
+                packed.forward(z[a:b], out=z[a:b])
+            state["done"] = max(a, b)
+        return z, ensure
+
+    def check_numerics(self):
+        """Raise if a kernel flagged an out-of-range operand since the weights were packed (synchronises)."""
+        self.model.g_mapping.packed().check()
+        if self.model.g_synthesis._packed is not None:
+            self.model.g_synthesis._packed.check()
+
+    # ---- synthesis ----------------------------------------------------------------------------------------
+    def _hookable(self):
+        return ["g_mapping"] + self.model.block_names()
+
+    def _reject_sub_module_hooks(self):
+        hookable = set(self._hookable())
+        for name, m in self.model.named_modules():
+            if name and name not in hookable and (len(m._forward_hooks) or len(m._forward_pre_hooks)):
+                raise NotImplementedError(f"StyleGAN: a hook on '{name}' is not supported: g_mapping and the synthesis blocks run as "
+                                          f"fused kernels; the hookable layers are {', '.join(self._hookable())}")
+
+    def _w_layers(self, x):
+        """[18, n, 512] per-layer dlatents (wrappers.py:382-387 / model.py:382-393) from one latent or a list of 18 (Z or W)."""
+        if isinstance(x, list):
+            assert len(x) == 18, "Must provide 1 or 18 latents"
+            ws = [l if self.w_primary else self.model.g_mapping(l) for l in x]
+            return torch.stack([w.reshape(-1, 512).float() for w in ws])
+        w = x if self.w_primary else self.model.g_mapping(x)
+        return w.reshape(1, -1, 512).float()
+
+    def _run(self, w_layers, target, want_rgb):
+        """Blocks 0 .. ``target`` with the forward hooks of every hooked block on the way (a hooked earlier block gets its own run
+        of the chain); the image when ``want_rgb``."""
+        packed = self.model.g_synthesis.packed()
+        blocks = list(self.model.g_synthesis.blocks.values())
+        names = self.model.block_names()
+        w_layers = w_layers[:2 * (target + 1)] if w_layers.shape[0] > 1 else w_layers
+
+        def hand(i, act):
+            res, co = packed.shapes[2 * i + 1]
+            t = act.view(-1, res, res, co).permute(0, 3, 1, 2)                       # NCHW view of NHWC storage
+            if blocks[i](_result=t) is not t and (i < target or want_rgb):
+                raise NotImplementedError(f"an edit on layer '{names[i]}' cannot be propagated through the fused StyleGAN chain")
+
+        for i in [i for i in range(target) if len(blocks[i]._forward_hooks)]:
+            hand(i, packed.forward(w_layers[:2 * (i + 1)] if w_layers.shape[0] > 1 else w_layers, 2 * (i + 1))[0])
+        want_act = len(blocks[target]._forward_hooks) > 0
+        act, rgb = packed.forward(w_layers, 2 * (target + 1), want_act=want_act or not want_rgb, want_rgb=want_rgb)
+        if want_act:
+            hand(target, act)
+        return rgb
+
+    def forward(self, x):
+        """wrappers.py:375-377: images ``0.5 (torgb + 1)`` (unclamped) from one latent or a list of 18; hooked blocks fire."""
+        self._reject_sub_module_hooks()
+        w_layers = self._w_layers(x)
+        rgb = self._run(w_layers, len(self.model.g_synthesis.blocks) - 1, True)
+        return 0.5 * (rgb.permute(0, 3, 1, 2) + 1)
+
+    def _target_block(self, layer_name):
+        """The reference's stop rule (wrappers.py:394-417): the first block one of whose leaf modules' names contains ``layer_name``."""
+        for i, (n, blk) in enumerate(self.model.g_synthesis.blocks.items()):
+            leaves = [f"g_synthesis.blocks.{n}.{c}" for c, m in blk.named_modules(remove_duplicate=False) if c and not m._modules]
+            if any(layer_name in c for c in leaves):
+                return i
+        raise RuntimeError(f"Layer {layer_name} not encountered in partial_forward")
+
+    def partial_forward(self, x, layer_name):
+        self._reject_sub_module_hooks()
+        if not self.w_primary:
+            x = [self.model.g_mapping(l) for l in x] if isinstance(x, list) else self.model.g_mapping(x)
+        if "g_mapping" in layer_name or layer_name == "truncation":
+            return
+        w_primary, self.w_primary = self.w_primary, True                          # x holds W from here on
+        try:
+            w_layers = self._w_layers(x)
+        finally:
+            self.w_primary = w_primary
+        self._run(w_layers, self._target_block(layer_name), False)
+
+    def feature_layout(self, layer_name):
+        """Device feature order of ``activations_into``: ('nhwc', (H, W, C)) for a synthesis block."""
+        names = self.model.block_names()
+        if layer_name not in names:
+            return None
+        res, co = self.model.g_synthesis.packed().shapes[2 * names.index(layer_name) + 1]
+        if res * res * co > self.MAX_DECOMPOSITION_DIMS:
+            raise NotImplementedError(
+                f"StyleGAN {layer_name}: d = {res * res * co} exceeds {self.MAX_DECOMPOSITION_DIMS} (blocks.32x32), the largest feature map "
+                "the large-d IPCA engine is run at: its stacked matrix holds (components + batch + 1) rows of d floats in HBM")
+        return ("nhwc", (res, res, co))
+
+    def activations_into(self, x, layer_name, out):
+        """Output of block ``layer_name`` for latents x [n, 512] (in the current primary space) written as fp32 NHWC rows into
+        ``out`` [n, H*W*C] (may be row-strided): the decomposition driver's producer."""
+        n_run = 2 * (self.model.block_names().index(layer_name) + 1)
+        x = x.reshape(-1, 512)
+        w = x if self.w_primary else self.model.g_mapping.packed().forward(x)
+        return self.model.g_synthesis.packed().forward(w, n_run, out=out)[0]
+
+
 # ---- factories (wrappers.py:651-735) ---------------------------------------------------------------
 @singledispatch
 def get_model(name, output_class, device, **kwargs):
@@ -547,7 +755,9 @@ def get_model(name, output_class, device, **kwargs):
         model = BigGAN(device, name.split("-")[-1], class_name=output_class, random_init=kwargs.get("random_init"))
     elif name == "ProGAN":
         model = ProGAN(device, lsun_class=output_class, random_init=kwargs.get("random_init"))
-    elif name in ("StyleGAN", "DCGAN"):
+    elif name == "StyleGAN":
+        model = StyleGAN(device, class_name=output_class, random_init=kwargs.get("random_init"))
+    elif name == "DCGAN":
         raise RuntimeError(f"{name} is outside the GPU hot path (SURVEY.md section 2: not in any BASELINE config)")
     else:
         raise RuntimeError(f"Unknown model {name}")
