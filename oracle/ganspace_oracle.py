@@ -621,32 +621,33 @@ def styled_conv_forward(x, w, L, noise):
     return out.numpy()
 
 
-def styled_conv_shared(x, w, L, noise):
+def styled_conv_shared(x, w, L, noise, dtype=np.float32):
     """styled_conv_forward with the per-sample weights factored out (identical algebra, used for bulk oracle runs: the
     reference form builds a [B,co,ci,3,3] weight tensor per call): scale the input channels by the style, convolve with
     the SHARED scale*W through the same torch CPU conv kernels, multiply by demod afterwards (the blur is linear and
-    per-channel, so the demodulation commutes with it)."""
+    per-channel, so the demodulation commutes with it).  ``dtype``: the arithmetic's type (float64 for the per-layer parity
+    references of tests/test_render_gpu.py)."""
     import math
     import torch
     import torch.nn.functional as F
-    x = torch.from_numpy(np.ascontiguousarray(x, np.float32))
-    w = torch.from_numpy(np.ascontiguousarray(w, np.float32))
-    W = torch.from_numpy(L["weight"]) * (1 / math.sqrt(L["weight"].shape[1] * 9))            # [co,ci,3,3]
+    T = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype))
+    x, w = T(x), T(w)
+    W = T(L["weight"]) * (1 / math.sqrt(L["weight"].shape[1] * 9))                               # [co,ci,3,3]
     B, ci, H, _ = x.shape
-    style = F.linear(w, torch.from_numpy(L["mod_weight"]) * (1 / math.sqrt(512)), bias=torch.from_numpy(L["mod_bias"]))
+    style = F.linear(w, T(L["mod_weight"]) * (1 / math.sqrt(512)), bias=T(L["mod_bias"]))
     demod = torch.rsqrt((style * style) @ (W * W).sum([2, 3]).T + 1e-8)                       # [B,co]
     xs = x * style.view(B, ci, 1, 1)
     if L["upsample"]:
         out = F.conv_transpose2d(xs, W.transpose(0, 1), padding=0, stride=2)                   # [B,co,2H+1,2H+1]
         co = out.shape[1]
         out = F.pad(out, [1, 1, 1, 1]).reshape(B * co, 1, 2 * H + 3, 2 * H + 3)
-        kflip = torch.flip(torch.from_numpy(BLUR_K2D), [0, 1]).view(1, 1, 4, 4)
+        kflip = torch.flip(T(BLUR_K2D), [0, 1]).view(1, 1, 4, 4)
         out = F.conv2d(out, kflip).view(B, co, 2 * H, 2 * H)
     else:
         out = F.conv2d(xs, W, padding=1)
     out = out * demod.view(B, -1, 1, 1)
-    out = out + torch.tensor(float(L["noise_weight"])) * torch.from_numpy(np.asarray(noise, np.float32))[None, None]
-    out = (2 ** 0.5) * F.leaky_relu(out + torch.from_numpy(L["act_bias"]).view(1, -1, 1, 1), negative_slope=0.2)
+    out = out + torch.tensor(float(L["noise_weight"]), dtype=out.dtype) * T(noise)[None, None]
+    out = (2 ** 0.5) * F.leaky_relu(out + T(L["act_bias"]).view(1, -1, 1, 1), negative_slope=0.2)
     return out.numpy()
 
 
@@ -687,27 +688,28 @@ def styled_conv_taps(x_nhwc, w, L, noise):
     return out
 
 
-def to_rgb_forward(x, w, R, skip=None):
+def to_rgb_forward(x, w, R, skip=None, dtype=np.float32):
     """ToRGB (model.py:344-363): 1x1 modulated conv WITHOUT demodulation (ModulatedConv2d(ci, 3, 1, demodulate=False), scale
     1/sqrt(ci), :219-220,236), + bias, + Upsample(skip) (:33-51: upfirdn2d(skip, [1,3,3,1] outer / 16, up=2, pad=(2,1)),
-    native form op/upfirdn2d.py:157-198: zero insertion, pad, true convolution).  x [B,ci,H,W], w [B,512] -> [B,3,H,W]."""
+    native form op/upfirdn2d.py:157-198: zero insertion, pad, true convolution).  x [B,ci,H,W], w [B,512] -> [B,3,H,W], in
+    ``dtype`` arithmetic."""
     import math
     import torch
     import torch.nn.functional as F
-    x = torch.from_numpy(np.ascontiguousarray(x, np.float32))
-    w = torch.from_numpy(np.ascontiguousarray(w, np.float32))
+    T = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype))
+    x, w = T(x), T(w)
     B, ci, H, W = x.shape
-    style = F.linear(w, torch.from_numpy(R["mod_weight"]) * (1 / math.sqrt(512)), bias=torch.from_numpy(R["mod_bias"]))
-    weight = (1 / math.sqrt(ci)) * torch.from_numpy(R["weight"]).view(1, 3, ci, 1, 1) * style.view(B, 1, ci, 1, 1)
+    style = F.linear(w, T(R["mod_weight"]) * (1 / math.sqrt(512)), bias=T(R["mod_bias"]))
+    weight = (1 / math.sqrt(ci)) * T(R["weight"]).view(1, 3, ci, 1, 1) * style.view(B, 1, ci, 1, 1)
     out = F.conv2d(x.reshape(1, B * ci, H, W), weight.view(B * 3, ci, 1, 1), padding=0, groups=B).view(B, 3, H, W)
-    out = out + torch.from_numpy(R["bias"]).view(1, 3, 1, 1)
+    out = out + T(R["bias"]).view(1, 3, 1, 1)
     if skip is not None:
-        sk = torch.from_numpy(np.ascontiguousarray(skip, np.float32))
+        sk = T(skip)
         h = sk.shape[2]
-        up = torch.zeros(B, 3, 2 * h, 2 * h)
+        up = torch.zeros(B, 3, 2 * h, 2 * h, dtype=sk.dtype)
         up[:, :, ::2, ::2] = sk
         up = F.pad(up, [2, 1, 2, 1]).reshape(B * 3, 1, 2 * h + 3, 2 * h + 3)
-        kflip = torch.flip(torch.from_numpy(BLUR_K2D), [0, 1]).view(1, 1, 4, 4)
+        kflip = torch.flip(T(BLUR_K2D), [0, 1]).view(1, 1, 4, 4)
         out = out + F.conv2d(up, kflip).view(B, 3, 2 * h, 2 * h)
     return out.numpy()
 

@@ -42,16 +42,18 @@ def pixel_norm(x):
     return x / np.sqrt(np.mean(x * x, axis=1, keepdims=True) + 1e-8)
 
 
-def progan_block_forward(x, L, output=False):
-    """Reference form, float32 torch on the host.  x [B, ci, H, W] -> [B, co, H', W']."""
+def progan_block_forward(x, L, output=False, dtype=np.float32):
+    """Reference form, torch on the host in ``dtype`` (float32: the reference's own arithmetic; float64: the per-layer parity
+    reference of tests/test_progan_gpu.py).  x [B, ci, H, W] -> [B, co, H', W']."""
     import torch
     import torch.nn.functional as F
-    t = torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32))
+    T = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=dtype))
+    t = T(x)
     t = t / torch.sqrt(torch.mean(t ** 2, dim=1, keepdim=True) + 1e-8)
     if L["upsample"]:
         t = F.interpolate(t, scale_factor=2, mode="nearest")
-    t = F.conv2d(t, torch.from_numpy(L["weight"]), None, 1, L["padding"])
-    t = t * float(L["scale"]) + torch.from_numpy(L["b"]).view(1, -1, 1, 1)
+    t = F.conv2d(t, T(L["weight"]), None, 1, L["padding"])
+    t = t * float(L["scale"]) + T(L["b"]).view(1, -1, 1, 1)
     if not output:
         t = F.leaky_relu(t, 0.2)
     return t.numpy()

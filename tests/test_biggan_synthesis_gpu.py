@@ -1,15 +1,19 @@
 """BigGAN-deep synthesis on the GPU (csrc/biggan.cu through models.biggan.BigGAN): every generator.layers.k and the images against
-known answers the unmodified reference wrote (oracle/gen_golden_biggan_synth.py), one GenBlock and the SelfAttn against an fp64
-restatement, batch independence, hooks, edits and the get_or_compute guard."""
+known answers the unmodified reference wrote (oracle/gen_golden_biggan_synth.py), every layer and the RGB tail of the 512 and the
+128 generator on their own against an fp64 restatement on every element, one GenBlock and the SelfAttn at scaled random inputs, batch independence,
+hooks, edits and the get_or_compute guard."""
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
+from layer_parity import assert_spans_chunks, biggan_chunk_samples, biggan_tile, check, parity_batch
+
 pytestmark = pytest.mark.gpu
 
 ACT_TOL = 5e-4         # max |diff| / max |ref|: the bar of test_progan_gpu.py
 UNIT_TOL = 2e-5        # one module against its fp64 restatement
+LAYER_TOL = 4.5e-6     # one layer fed the chain's own input, against fp64, per sample: ~3x the worst measured (test_each_layer_vs_fp64)
 
 
 @pytest.fixture(scope="module")
@@ -126,6 +130,8 @@ def _attn64(sa, x):
 
 
 def test_genblock_up_and_drop_vs_fp64(model):
+    """The up-sampling, channel-dropping GenBlock on random inputs three times the unit scale and arbitrary condition vectors:
+    a regime the chain's own activations and the model's condition vectors (test_each_layer_vs_fp64) do not reach."""
     blk = model.model.generator.layers[3]                  # (up, 2048 -> 1024) at 8x8 -> 16x16
     assert blk.up_sample and blk.drop_channels
     gen = torch.Generator().manual_seed(5)
@@ -135,6 +141,78 @@ def test_genblock_up_and_drop_vs_fp64(model):
     out = chain.block(3, x.float().permute(0, 2, 3, 1).contiguous().cuda(), cond.float().cuda()).permute(0, 3, 1, 2)
     ref = _block64(blk, x.float().double(), cond.float().double(), model.truncation)
     assert _err(out.cpu().numpy(), ref.numpy()) < UNIT_TOL
+
+
+def _rgb64(g, x, t):
+    mean, var = (v.double().cpu() for v in g.bn.stats(t))
+    h = (x - mean[None, :, None, None]) / torch.sqrt(var + g.bn.eps)[None, :, None, None]
+    h = h * g.bn.weight.detach().double().cpu()[None, :, None, None] + g.bn.bias.detach().double().cpu()[None, :, None, None]
+    w = g.conv_to_rgb.effective_weight().double().cpu()[:3]            # the image keeps the first three output channels
+    return 0.5 * (torch.tanh(F.conv2d(F.relu(h), w, g.conv_to_rgb.bias.detach().double().cpu()[:3], padding=1)) + 1)
+
+
+@pytest.fixture(scope="module")
+def model128():
+    from ganspace_b200.models.biggan import BigGAN
+    return BigGAN(torch.device("cuda:0"), 128, "husky", random_init=4321)
+
+
+def _layer_cases():
+    from ganspace_b200.models.biggan import _LAYERS
+    cases = []
+    for res in (512, 128):
+        n_mod = len(_LAYERS[res]) + 1                      # the GenBlocks and the SelfAttn
+        cases += [pytest.param(res, k, id=f"{res}-layers.{k}") for k in range(n_mod)] + [pytest.param(res, "rgb", id=f"{res}-rgb")]
+    return cases
+
+
+@pytest.mark.parametrize("res,layer", _layer_cases())
+def test_each_layer_vs_fp64(model, model128, res, layer):
+    """generator.layers.k (GenBlock or SelfAttn) fed the chain's own output of layers.k-1 (of gen_z for k = 0), taken from the
+    retain hooks, with the condition vector the chain gives that block, against the fp64 restatement, on every element; the RGB
+    tail fed the last layer's output.  One latent per sample and per GenBlock, so a condition index that slips fails.  The batch
+    spans two 128-row tiles of the layer's input resolution and, at 4x4 and 8x8, ends in a ragged tile.  Measured on an H100
+    80GB HBM3 (700 W), both generators: worst 1.4e-6 (layers.3, the 8 -> 16 up-block with 2048 input channels), under 1e-6 for
+    every other GenBlock and the SelfAttn (3.7e-7 at 64x64), under 1e-6 for the RGB tail."""
+    from ganspace_b200.models.biggan import GenBlock
+    from ganspace_b200.netdissect.nethook import InstrumentedModel
+    m = model if res == 512 else model128
+    g = m.model.generator
+    mods = list(g.layers)
+    k = len(mods) - 1 if layer == "rgb" else layer
+    r_in = 4
+    for mod in mods[:k]:
+        r_in *= 2 if isinstance(mod, GenBlock) and mod.up_sample else 1
+    r_last = r_in * (2 if isinstance(mods[k], GenBlock) and mods[k].up_sample else 1)
+    spc = biggan_chunk_samples(r_last if layer == "rgb" else r_in)
+    n = parity_batch(spc)
+    assert_spans_chunks(n, spc)
+    zs = [m.sample_latent(n, seed=500 + 31 * k + i) for i in range(m.model.n_latents)]
+    conds = [c.double().cpu() for c in m._conds(zs)]
+    prev = "generator.gen_z" if k == 0 else f"generator.layers.{k - 1}"
+    names = [prev, f"generator.layers.{k}"]
+    inst = InstrumentedModel(m)
+    inst.retain_layers(names)
+    try:
+        if layer == "rgb":
+            got = m.forward(zs)
+            x = inst.retained_layer(names[1]).double().cpu()
+            ref = _rgb64(g, x, m.truncation)
+            tile = lambda s: biggan_tile(s, r_last)
+        else:
+            m.partial_forward(zs, names[1])
+            x = inst.retained_layer(prev)
+            x = (x.view(n, 4, 4, -1).permute(0, 3, 1, 2) if k == 0 else x).double().cpu()
+            got = inst.retained_layer(names[1])
+            if isinstance(mods[k], GenBlock):
+                ci = 1 + sum(isinstance(mod, GenBlock) for mod in mods[:k])
+                ref = _block64(mods[k], x, conds[ci], m.truncation)
+            else:
+                ref = _attn64(mods[k], x)
+            tile = lambda s: biggan_tile(s, r_in)
+        check(got.double().cpu().numpy(), ref.numpy(), LAYER_TOL, f"BigGAN-{res} {names[1] if layer != 'rgb' else 'rgb'}", chunk_of=tile)
+    finally:
+        inst.close()
 
 
 def test_selfattn_vs_fp64(model):

@@ -1,6 +1,7 @@
 """ProGAN on the GPU (csrc/progan.cu through models.wrappers.ProGAN): every block and the image against known answers written by
-the unmodified reference, the latent sampler against NumPy, partial == full at a hooked layer, independence of the batch size,
-and get_or_compute at layer4 against the reference's own .npz (oracle/gen_golden_progan.py)."""
+the unmodified reference, every block on its own against fp64 on every element, the latent sampler against NumPy, partial ==
+full at a hooked layer, independence of the batch size, and get_or_compute at layer4 against the reference's own .npz
+(oracle/gen_golden_progan.py)."""
 import tempfile
 from types import SimpleNamespace
 
@@ -8,9 +9,13 @@ import numpy as np
 import pytest
 import torch
 
+from layer_parity import assert_spans_chunks, check, nhwc_to_nchw, parity_batch, progan_chunk_samples
+from oracle import progan_oracle as po
+
 pytestmark = pytest.mark.gpu
 
 ACT_TOL = 5e-4         # max |diff| / max |ref| after up to 15 fused blocks (the bar of test_render_gpu.py)
+LAYER_TOL = 8e-6       # one block fed the chain's own input, against fp64, per sample: ~3x the worst measured (test_each_block_vs_fp64)
 
 
 @pytest.fixture(scope="module")
@@ -54,6 +59,36 @@ def test_every_block_and_image_vs_reference(ka, model):
     assert np.array_equal(model.forward([z]).cpu().numpy(), img)                 # a one-element list is the same latent
     with pytest.raises(AssertionError, match="single global latent"):
         model.forward([z, z])
+    model.check_numerics()
+
+
+@pytest.mark.parametrize("name", [spec[0] for spec in po.block_specs()])
+def test_each_block_vs_fp64(model, name):
+    """Block ``name`` fed the chain's own output of the block before (the latent for layer1) against the reference form in
+    fp64, on every element of a batch that spans two GEMM chunks of that block (the output block: of layer14, behind whose
+    epilogue it is fused), one latent per sample.  Measured on an H100 80GB HBM3 (700 W): worst 2.4e-6 (layer2, fp16 hi/lo
+    tensor-core products over 4608 terms), 1e-6 to 2e-6 at 4x4 .. 32x32, under 1e-6 from 64x64 on, 1.6e-7 for the output
+    block."""
+    params = po.progan_random_init(1234)                    # the model's weights (tests/test_progan.py pins the init order)
+    names = list(params)
+    i = names.index(name)
+    out_block = name.startswith("output")
+    packed = model.model.packed()
+    conv = i - 1 if out_block else i                         # the conv block whose chunks the batch must cross
+    res_in = 1 if conv == 0 else packed.shapes[conv - 1][0]
+    spc = progan_chunk_samples(res_in, params[names[conv]]["ksize"], packed.shapes[conv][1])
+    n = parity_batch(spc)
+    assert_spans_chunks(n, spc)
+    z = torch.from_numpy(np.random.RandomState(100 + i).standard_normal((n, 512)).astype(np.float32)).to(model.device)
+    if out_block:
+        act, rgb = packed.forward(z, i, want_rgb=True)
+        x = nhwc_to_nchw(act, n, *packed.shapes[i - 1])
+        got = rgb.permute(0, 3, 1, 2).double().cpu().numpy()
+    else:
+        x = z.double().cpu().numpy().reshape(n, 512, 1, 1) if i == 0 else nhwc_to_nchw(packed.forward(z, i)[0], n, *packed.shapes[i - 1])
+        got = nhwc_to_nchw(packed.forward(z, i + 1)[0], n, *packed.shapes[i])
+    ref = po.progan_block_forward(x, params[name], output=out_block, dtype=np.float64)
+    check(got, ref, LAYER_TOL, name, chunk_of=spc)
     model.check_numerics()
 
 

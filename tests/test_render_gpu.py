@@ -3,14 +3,20 @@ ToRGB / skip chain, StyleGAN2.forward with one latent, per-layer latents and sty
 the unmodified reference (oracle/gen_golden_r2.py G11), plus the reference's own test invariants (tests/partial_forward_test.py:
 partial == full at the hooked layer; tests/layerwise_z_test.py: forward(z) == forward(n_latents * [z])).
 convs.10 .. convs.15 are checked against the reference's full forward: its partial_forward never reaches them (substring match on
-the layer name, wrappers.py:241-246 -- INTEGRATION.md section 3)."""
+the layer name, wrappers.py:241-246 -- INTEGRATION.md section 3).  Every StyledConv and every ToRGB is also checked on its own
+against fp64, on every element, fed the chain's own input."""
 import numpy as np
 import pytest
 import torch
 
+from layer_parity import assert_spans_chunks, check, nhwc_to_nchw, parity_batch, stylegan2_chunk_samples
+from oracle import ganspace_oracle as oracle_go
+
 pytestmark = pytest.mark.gpu
 
 ACT_TOL = 5e-4         # max |diff| / max |ref| after up to 17 fused layers (fp16 hi/lo tensor-core products, ~1e-5 per layer)
+LAYER_TOL = 9e-6       # one StyledConv fed the chain's own input, against fp64, per sample: ~3x the worst measured
+RGB_TOL = 2e-6         # one ToRGB (fp32 1x1 conv + skip) fed the chain's own inputs, against fp64, per sample: ~3x the worst measured
 
 
 def _perturb(model, conv_names, rgb_names):
@@ -44,6 +50,86 @@ def model(deep):
 def _sub(act):
     step = max(1, act.shape[-1] // 32)
     return act[:, ::max(1, act.shape[1] // 16), ::step, ::step]
+
+
+CONV_NAMES = ["conv1"] + [f"convs.{i}" for i in range(16)]
+RGB_NAMES = ["to_rgb1"] + [f"to_rgbs.{j}" for j in range(8)]
+
+
+@pytest.fixture(scope="module")
+def perturbed():
+    """The 1024^2 generator with non-zero noise weights and activation biases in every StyledConv and non-zero ToRGB biases."""
+    from ganspace_b200.models import StyleGAN2
+    m = StyleGAN2(torch.device("cuda:0"), "ffhq", random_init=1234)
+    _perturb(m.model, CONV_NAMES, RGB_NAMES)
+    return m
+
+
+def _np(t):
+    return t.detach().float().cpu().numpy()
+
+
+def _per_layer_latents(seed, n):
+    return np.random.RandomState(seed).standard_normal((18, n, 512)).astype(np.float32)
+
+
+@pytest.mark.parametrize("name", CONV_NAMES)
+def test_each_styled_conv_vs_fp64(perturbed, name):
+    """StyledConv ``name`` (layer l of the chain, latent l) fed the chain's own output of layer l-1 (the constant input for
+    conv1) against the oracle's shared-weight form in fp64, on every element of a batch that spans two sample chunks of the
+    layer, one latent per sample and layer (gsb_synthesis_render with want_act).  Measured on an H100 80GB HBM3 (700 W): worst
+    2.8e-6 (conv1), 1.7e-6 to 2.6e-6 for the 512-channel layers, under 1.4e-6 from convs.9 on."""
+    m = perturbed
+    l = CONV_NAMES.index(name)
+    mod = ([m.model.conv1] + list(m.model.convs))[l]
+    syn = m._synthesis(len(CONV_NAMES))
+    res_in = 4 if l == 0 else syn.shapes[l - 1][0]
+    spc = stylegan2_chunk_samples(res_in)
+    n = parity_batch(spc)
+    assert_spans_chunks(n, spc)
+    w = _per_layer_latents(300 + l, n)
+    wd = torch.from_numpy(w).to(m.device)
+    if l == 0:
+        x = np.repeat(_np(m.model.input.input).astype(np.float64), n, axis=0)
+    else:
+        x = nhwc_to_nchw(syn.render(wd, l, [], want_act=True)[0], n, *syn.shapes[l - 1])
+    got = nhwc_to_nchw(syn.render(wd, l + 1, [], want_act=True)[0], n, *syn.shapes[l])
+    r = syn.shapes[l][0]
+    L = dict(weight=_np(mod.conv.weight[0]), mod_weight=_np(mod.conv.modulation.weight), mod_bias=_np(mod.conv.modulation.bias),
+             noise_weight=float(mod.noise.weight), act_bias=_np(mod.activate.bias), upsample=mod.conv.upsample)
+    ref = oracle_go.styled_conv_shared(x, w[l], L, _np(m.noise[l]).reshape(r, r), dtype=np.float64)
+    check(got, ref, LAYER_TOL, name, chunk_of=spc)
+    m.check_numerics()
+
+
+@pytest.mark.parametrize("name", RGB_NAMES)
+def test_each_to_rgb_vs_fp64(perturbed, name):
+    """ToRGB ``name`` (j; it follows layer 0 for j = 0, else layer 2j, and reads latent 2j + 1) fed the chain's own StyledConv
+    output and the chain's own previous skip image, against to_rgb_forward in fp64 (modulated 1x1 conv without demodulation,
+    bias, [1,3,3,1] up-sampled skip), on every element of a batch that spans two chunks of the layer it is fused into.
+    Measured on an H100 80GB HBM3 (700 W): worst 6.3e-7 (to_rgb1), 2.2e-7 to 4.7e-7 for the others."""
+    m = perturbed
+    j = RGB_NAMES.index(name)
+    lj = 2 * j
+    mods = [m.model.to_rgb1] + list(m.model.to_rgbs)
+    rgbs = [t.describe() for t in mods]
+    syn = m._synthesis(len(CONV_NAMES))
+    spc = stylegan2_chunk_samples(4 if lj == 0 else syn.shapes[lj - 1][0])
+    n = parity_batch(spc)
+    assert_spans_chunks(n, spc)
+    w = _per_layer_latents(400 + j, n)
+    wd = torch.from_numpy(w).to(m.device)
+    act, img = syn.render(wd, lj + 1, rgbs[:j + 1], want_act=True)
+    x = nhwc_to_nchw(act, n, *syn.shapes[lj])
+    got = img.permute(0, 3, 1, 2).double().cpu().numpy()
+    skip = None
+    if j > 0:
+        skip = syn.render(wd, lj - 1, rgbs[:j])[1].permute(0, 3, 1, 2).double().cpu().numpy()
+    R = {k: _np(v) for k, v in rgbs[j].items()}
+    R["weight"] = R.pop("conv_weight")
+    ref = oracle_go.to_rgb_forward(x, w[lj + 1], R, skip, dtype=np.float64)
+    check(got, ref, RGB_TOL, name, chunk_of=spc)
+    m.check_numerics()
 
 
 def test_deep_layers_and_to_rgb_known_answers(deep, model):

@@ -1,6 +1,7 @@
 """StyleGAN (v1) on the GPU (csrc/stylegan.cu and the mapping kernels through models.wrappers.StyleGAN): every block and the image
-for ffhq and bedrooms against known answers written by the unmodified reference, in Z mode and for 18 distinct W; one layer of each
-kind against the fp64 oracle fed its own input; the sampler against NumPy; partial == full at a hooked block; independence of the
+for ffhq and bedrooms against known answers written by the unmodified reference, in Z mode and for 18 distinct W; one block of
+each kind against the fp64 oracle fed its own input; every layer and torgb on its own against fp64 on every element, fed the
+chain's own input; the sampler against NumPy; partial == full at a hooked block; independence of the
 batch size; the three get_or_compute runs against the reference's own .npz (oracle/gen_golden_stylegan.py); and the guards."""
 import tempfile
 from types import SimpleNamespace
@@ -9,12 +10,14 @@ import numpy as np
 import pytest
 import torch
 
+from layer_parity import assert_spans_chunks, check, nhwc_to_nchw, parity_batch, stylegan_chunk_samples
 from oracle import stylegan_oracle as so
 
 pytestmark = pytest.mark.gpu
 
 ACT_TOL = 5e-4         # max |diff| / max |ref| after up to 18 fused layers (the bar of test_render_gpu.py / test_progan_gpu.py)
 LAYER_TOL = 1e-4       # one layer fed the oracle's own input, against fp64
+PARITY_TOL = 1.3e-5    # one layer fed the chain's own input, against fp64, per sample: ~3x the worst measured (test_each_layer_vs_fp64)
 DEV = torch.device("cuda:0")
 
 
@@ -100,6 +103,48 @@ def test_one_layer_of_each_kind_vs_fp64_oracle(models):
         got = got.view(1, r, r, c).permute(0, 3, 1, 2).double().cpu().numpy()
         err = np.abs(got - x).max() / np.abs(x).max()
         assert err < LAYER_TOL, (blk, err)
+    m.check_numerics()
+
+
+def _layer_cases():
+    cases = []
+    for cls, res in (("ffhq", 1024), ("bedrooms", 256)):
+        for l, (b, conv, _, _, _) in enumerate(so.layers({}, res)):
+            cases.append(pytest.param(cls, l, id=f"{cls}-{l:02d}-{b}.{'const' if conv is None else conv.rsplit('.', 1)[1]}"))
+        cases.append(pytest.param(cls, "torgb", id=f"{cls}-torgb"))
+    return cases
+
+
+@pytest.mark.parametrize("cls,layer", _layer_cases())
+def test_each_layer_vs_fp64(models, cls, layer):
+    """Layer ``layer`` of the synthesis chain (the input block's constant layer, a 3x3 conv, an up-conv below 128 px and one
+    from 128 px, which packs the flipped kernel) fed the chain's own output of the layer before, against the reference form in
+    fp64 (oracle layer_reference), on every element of a batch that spans two chunks of that layer; torgb fed the last layer's
+    output.  Every sample and every layer has its own latent ([L, n, 512]), so a latent or style index that slips by a layer
+    or by a sample fails.  Measured on an H100 80GB HBM3 (700 W), both classes: worst 4.3e-6 (the 4x4 conv and the 8x8 up-conv),
+    1e-6 to 3.5e-6 up to 64x64, under 1e-6 from 128x128 on (flipped kernel included), 1.4e-7 for torgb."""
+    m = models[cls]
+    sd = m.model.state_dict()
+    packed = m.model.g_synthesis.packed()
+    lays = so.layers(sd, m.resolution)
+    rgb = layer == "torgb"
+    l = len(lays) - 1 if rgb else layer
+    _, conv, epi, up, r = lays[l]
+    spc = stylegan_chunk_samples(r, packed.shapes[l][1], up, conv is not None)
+    n = parity_batch(spc)
+    assert_spans_chunks(n, spc)
+    w = np.random.RandomState(200 + l).standard_normal((len(lays), n, 512)).astype(np.float32)
+    wd = torch.from_numpy(w).to(DEV)
+    if rgb:
+        act, img = packed.forward(wd, len(lays), want_rgb=True)
+        got = img.permute(0, 3, 1, 2).double().cpu().numpy()
+        ref = so.torgb(nhwc_to_nchw(act, n, *packed.shapes[l]), sd)
+    else:
+        x = None if l == 0 else nhwc_to_nchw(packed.forward(wd, l)[0], n, *packed.shapes[l - 1])
+        got = nhwc_to_nchw(packed.forward(wd, l + 1)[0], n, *packed.shapes[l])
+        noise = m.model.g_synthesis.layer_modules()[l][1].top_epi.noise.noise.reshape(r, r)
+        ref = so.layer_reference(x, w[l], sd, conv, epi, up, noise)
+    check(got, ref, PARITY_TOL, f"{cls} {layer}", chunk_of=spc)
     m.check_numerics()
 
 

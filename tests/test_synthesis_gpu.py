@@ -64,7 +64,7 @@ def test_partial_forward_known_answers(golden, perturbed_model):
 
 
 def test_synthesis_chunking_and_native_layout(oracle, perturbed_model):
-    """A batch that spans several sample chunks with a ragged tail (33 samples at 16x16: chunks of 16), written through
+    """A batch that spans several sample chunks with a ragged tail (33 samples at 16x16: chunks of 8), written through
     activations_into into a row-strided buffer, against the oracle's reference-form StyledConv chain."""
     m = perturbed_model
     m.use_w()
