@@ -722,11 +722,53 @@ class LinregAccumulator:
         return M, zmean
 
 
-class PackedSynthesis:
+class _PackedTapGenerator:
+    """What the tap-GEMM generators (PackedSynthesis, PackedProGAN, PackedStyleGAN) share: the packed device buffer, ``shapes``
+    ((res_out, cout) per layer), the activation and image outputs, and the fp16-overflow status.  ``NAME`` is the family's
+    prefix in the C entry points; each subclass makes its own C calls."""
+
+    NAME = ""
+
+    def _pack(self, nbytes: int, pack):
+        """Allocates ``nbytes`` (the family's gsb_*_packed_bytes) and runs ``pack(d_packed, packed_bytes, stream)`` into it."""
+        if nbytes == 0:
+            raise NativeError(f"gsb_{self.NAME}_packed_bytes: {load().gsb_last_error().decode()}")
+        self.packed = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            _check(pack(_ptr(self.packed), self.packed.numel(), _stream()), f"gsb_{self.NAME}_pack")
+            torch.cuda.current_stream().synchronize()      # the fp32 parameter copies may be freed after this returns
+
+    def out_dims(self, n_run: int) -> int:
+        r, co = self.shapes[n_run - 1]
+        return r * r * co
+
+    def _outputs(self, n: int, n_run: int, out, want_act: bool, want_rgb: bool, device):
+        """(activation rows [n, out_dims] -- ``out`` if given -- or None, image [n, res, res, 3] or None)."""
+        act = rgb = None
+        if want_act:
+            d = self.out_dims(n_run)
+            act = torch.empty((n, d), dtype=torch.float32, device=device) if out is None else out
+            assert act.is_cuda and act.dtype == torch.float32 and act.shape == (n, d) and act.stride(1) == 1
+        if want_rgb:
+            res = self.shapes[-1][0]
+            rgb = torch.empty((n, res, res, 3), dtype=torch.float32, device=device)
+        return act, rgb
+
+    def check(self):
+        flags = C.c_uint(0)
+        with torch.cuda.device(self.device):
+            _check(self._status(C.byref(flags)), f"gsb_{self.NAME}_status")
+        if flags.value & 1:
+            raise NativeError(f"{self.NAME}: an operand exceeded fp16 range in the tensor-core path; results are invalid")
+
+
+class PackedSynthesis(_PackedTapGenerator):
     """StyleGAN2 synthesis layers conv1, convs.0 .. convs.k packed for the tap-GEMM kernels (gsb_synthesis_pack).
 
     ``layers``: dicts with conv_weight [co,ci,3,3], mod_weight [ci,S], mod_bias [ci], act_bias [co], noise [r,r],
     noise_weight [1] (fp32 CUDA tensors) and upsample (bool), res_in (int), in execution order."""
+
+    NAME = "synthesis"
 
     def __init__(self, const_input: torch.Tensor, layers, style_dim: int):
         lib = load()
@@ -751,18 +793,9 @@ class PackedSynthesis:
             d.cin, d.cout, d.upsample, d.res_in = ci, co, int(up), res_in
             self.shapes.append((res_out, co))
         cst = f32(const_input).reshape(-1, 4, 4)
-        nbytes = lib.gsb_synthesis_packed_bytes(self.desc, self.n_layers, self.style_dim)
-        if nbytes == 0:
-            raise NativeError(f"gsb_synthesis_packed_bytes: {lib.gsb_last_error().decode()}")
-        self.packed = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        with torch.cuda.device(self.device):
-            _check(lib.gsb_synthesis_pack(self.desc, self.n_layers, self.style_dim, _ptr(cst), _ptr(self.packed),
-                                          self.packed.numel(), _stream()), "gsb_synthesis_pack")
-            torch.cuda.current_stream().synchronize()      # the temporaries above may be freed after this returns
-
-    def out_dims(self, n_run: int) -> int:
-        r, co = self.shapes[n_run - 1]
-        return r * r * co
+        self._pack(lib.gsb_synthesis_packed_bytes(self.desc, self.n_layers, self.style_dim),
+                   lambda packed, nbytes, st: lib.gsb_synthesis_pack(self.desc, self.n_layers, self.style_dim, _ptr(cst), packed,
+                                                                     nbytes, st))
 
     def forward(self, w: torch.Tensor, n_run: int, out: torch.Tensor = None) -> torch.Tensor:
         """Activation of layer ``n_run - 1`` for w[n, style_dim]: fp32 NHWC rows [n, res*res*cout] (``out`` may be a
@@ -770,10 +803,8 @@ class PackedSynthesis:
         lib = load()
         assert w.is_cuda and w.dtype == torch.float32 and w.dim() == 2 and w.shape[1] == self.style_dim
         w = w.contiguous()
-        n, d = w.shape[0], self.out_dims(n_run)
-        if out is None:
-            out = torch.empty((n, d), dtype=torch.float32, device=w.device)
-        assert out.is_cuda and out.dtype == torch.float32 and out.shape == (n, d) and out.stride(1) == 1
+        n = w.shape[0]
+        out = self._outputs(n, n_run, out, True, False, w.device)[0]
         ws_bytes = lib.gsb_synthesis_workspace_bytes(self.desc, n_run, n)
         ws = scratch.get("synthesis", ws_bytes, w.device)
         with torch.cuda.device(w.device), instrument.section("synthesis"):
@@ -827,20 +858,17 @@ class PackedSynthesis:
         instrument.add_rows("synthesis", n)
         return act, rgb
 
-    def check(self):
-        flags = C.c_uint(0)
-        with torch.cuda.device(self.device):
-            _check(load().gsb_synthesis_status(_ptr(self.packed), self.desc, self.n_layers, self.style_dim, C.byref(flags)),
-                   "gsb_synthesis_status")
-        if flags.value & 1:
-            raise NativeError("synthesis: an operand exceeded fp16 range in the tensor-core path; results are invalid")
+    def _status(self, flags):
+        return load().gsb_synthesis_status(_ptr(self.packed), self.desc, self.n_layers, self.style_dim, flags)
 
 
-class PackedProGAN:
+class PackedProGAN(_PackedTapGenerator):
     """ProGAN blocks layer1 .. layerK and the RGB output block packed for the tap-GEMM kernels (gsb_progan_pack).
 
     ``blocks``: dicts with conv_weight [co,ci,k,k], bias [co] (fp32 tensors) and upsample (bool), in execution order;
     ``out_weight`` [3,c,1,1] / ``out_bias`` [3]: the output block."""
+
+    NAME = "progan"
 
     def __init__(self, blocks, out_weight: torch.Tensor, out_bias: torch.Tensor):
         lib = load()
@@ -863,18 +891,8 @@ class PackedProGAN:
         self.z_dim = int(self.desc[0].cin)
         ow, ob = f32(out_weight).reshape(3, -1), f32(out_bias).reshape(3)
         assert ow.shape[1] == self.shapes[-1][1]
-        nbytes = lib.gsb_progan_packed_bytes(self.desc, self.n_blocks)
-        if nbytes == 0:
-            raise NativeError(f"gsb_progan_packed_bytes: {lib.gsb_last_error().decode()}")
-        self.packed = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        with torch.cuda.device(self.device):
-            _check(lib.gsb_progan_pack(self.desc, self.n_blocks, _ptr(ow), _ptr(ob), _ptr(self.packed), self.packed.numel(),
-                                       _stream()), "gsb_progan_pack")
-            torch.cuda.current_stream().synchronize()      # the fp32 copies in `keep` may be freed after this returns
-
-    def out_dims(self, n_run: int) -> int:
-        r, co = self.shapes[n_run - 1]
-        return r * r * co
+        self._pack(lib.gsb_progan_packed_bytes(self.desc, self.n_blocks),
+                   lambda packed, nbytes, st: lib.gsb_progan_pack(self.desc, self.n_blocks, _ptr(ow), _ptr(ob), packed, nbytes, st))
 
     def forward(self, z: torch.Tensor, n_run: int, out: torch.Tensor = None, want_act: bool = True, want_rgb: bool = False):
         """Blocks 0 .. n_run-1 on z [n, z_dim].  Returns (activation of block n_run-1 as fp32 NHWC rows [n, res*res*cout] or None,
@@ -883,14 +901,8 @@ class PackedProGAN:
         lib = load()
         assert z.is_cuda and z.dtype == torch.float32 and z.dim() == 2 and z.shape[1] == self.z_dim
         z = z.contiguous()
-        n, d = z.shape[0], self.out_dims(n_run)
-        act = rgb = None
-        if want_act:
-            act = torch.empty((n, d), dtype=torch.float32, device=z.device) if out is None else out
-            assert act.is_cuda and act.dtype == torch.float32 and act.shape == (n, d) and act.stride(1) == 1
-        if want_rgb:
-            res = self.shapes[-1][0]
-            rgb = torch.empty((n, res, res, 3), dtype=torch.float32, device=z.device)
+        n = z.shape[0]
+        act, rgb = self._outputs(n, n_run, out, want_act, want_rgb, z.device)
         if n == 0:
             return act, rgb
         ws_bytes = lib.gsb_progan_workspace_bytes(self.desc, n_run, n)
@@ -903,20 +915,18 @@ class PackedProGAN:
         instrument.add_rows("progan", n)
         return act, rgb
 
-    def check(self):
-        flags = C.c_uint(0)
-        with torch.cuda.device(self.device):
-            _check(load().gsb_progan_status(_ptr(self.packed), self.desc, self.n_blocks, C.byref(flags)), "gsb_progan_status")
-        if flags.value & 1:
-            raise NativeError("progan: an operand exceeded fp16 range in the tensor-core path; results are invalid")
+    def _status(self, flags):
+        return load().gsb_progan_status(_ptr(self.packed), self.desc, self.n_blocks, flags)
 
 
-class PackedStyleGAN:
+class PackedStyleGAN(_PackedTapGenerator):
     """StyleGAN (v1) synthesis layers (two per block) and torgb packed for the tap-GEMM kernels (gsb_stylegan_pack).
 
     ``layers``: dicts with conv_weight [co,ci,3,3] (None for the first layer), bias [co], noise [r,r], noise_weight [co],
     style_weight [2co, dlatent], style_bias [2co] (fp32 tensors), upsample (bool) and res_out (int), in execution order;
     ``const`` [c0,4,4]: the InputBlock's constant; ``rgb_weight`` [3,c,1,1] / ``rgb_bias`` [3]: torgb."""
+
+    NAME = "stylegan"
 
     def __init__(self, layers, const: torch.Tensor, rgb_weight: torch.Tensor, rgb_bias: torch.Tensor, dlatent: int = 512):
         lib = load()
@@ -943,18 +953,9 @@ class PackedStyleGAN:
         cst = f32(const).reshape(self.shapes[0][1], 4, 4)
         rw, rb = f32(rgb_weight).reshape(3, -1), f32(rgb_bias).reshape(3)
         assert rw.shape[1] == self.shapes[-1][1]
-        nbytes = lib.gsb_stylegan_packed_bytes(self.desc, self.n_layers, self.dlatent)
-        if nbytes == 0:
-            raise NativeError(f"gsb_stylegan_packed_bytes: {lib.gsb_last_error().decode()}")
-        self.packed = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        with torch.cuda.device(self.device):
-            _check(lib.gsb_stylegan_pack(self.desc, self.n_layers, self.dlatent, _ptr(cst), _ptr(rw), _ptr(rb), _ptr(self.packed),
-                                         self.packed.numel(), _stream()), "gsb_stylegan_pack")
-            torch.cuda.current_stream().synchronize()      # the fp32 copies in `keep` may be freed after this returns
-
-    def out_dims(self, n_run: int) -> int:
-        r, co = self.shapes[n_run - 1]
-        return r * r * co
+        self._pack(lib.gsb_stylegan_packed_bytes(self.desc, self.n_layers, self.dlatent),
+                   lambda packed, nbytes, st: lib.gsb_stylegan_pack(self.desc, self.n_layers, self.dlatent, _ptr(cst), _ptr(rw), _ptr(rb),
+                                                                    packed, nbytes, st))
 
     def forward(self, w: torch.Tensor, n_run: int, out: torch.Tensor = None, want_act: bool = True, want_rgb: bool = False):
         """Layers 0 .. n_run-1 for dlatents ``w`` [n, dlatent] (one latent for every layer) or [Lw, n, dlatent] (layer l reads
@@ -965,14 +966,7 @@ class PackedStyleGAN:
         assert w.is_cuda and w.dtype == torch.float32 and w.shape[-1] == self.dlatent and w.dim() in (2, 3)
         w3 = (w[None] if w.dim() == 2 else w).contiguous()
         Lw, n = int(w3.shape[0]), int(w3.shape[1])
-        d = self.out_dims(n_run)
-        act = rgb = None
-        if want_act:
-            act = torch.empty((n, d), dtype=torch.float32, device=w.device) if out is None else out
-            assert act.is_cuda and act.dtype == torch.float32 and act.shape == (n, d) and act.stride(1) == 1
-        if want_rgb:
-            res = self.shapes[-1][0]
-            rgb = torch.empty((n, res, res, 3), dtype=torch.float32, device=w.device)
+        act, rgb = self._outputs(n, n_run, out, want_act, want_rgb, w.device)
         if n == 0:
             return act, rgb
         ws = scratch.get("stylegan", lib.gsb_stylegan_workspace_bytes(self.desc, n_run, n), w.device)
@@ -984,13 +978,8 @@ class PackedStyleGAN:
         instrument.add_rows("stylegan", n)
         return act, rgb
 
-    def check(self):
-        flags = C.c_uint(0)
-        with torch.cuda.device(self.device):
-            _check(load().gsb_stylegan_status(_ptr(self.packed), self.desc, self.n_layers, self.dlatent, C.byref(flags)),
-                   "gsb_stylegan_status")
-        if flags.value & 1:
-            raise NativeError("stylegan: an operand exceeded fp16 range in the tensor-core path; results are invalid")
+    def _status(self, flags):
+        return load().gsb_stylegan_status(_ptr(self.packed), self.desc, self.n_layers, self.dlatent, flags)
 
 
 def _f32_dev(t, what):

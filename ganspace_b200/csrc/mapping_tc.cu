@@ -281,42 +281,46 @@ __global__ void pixelnorm_split_kernel(const float *__restrict__ x, __half *__re
     for (int i = lane; i < dim / 4; i += 32) {
         float4 v = xr[i];
         const float f[4] = {v.x * r, v.y * r, v.z * r, v.w * r};
-        uint2 ph, pl;
-        ovf |= tc::split4(f, ph, pl);
-        reinterpret_cast<uint2 *>(hi + row * dim)[i] = ph;
-        reinterpret_cast<uint2 *>(lo + row * dim)[i] = pl;
+        tc::store_split4(f, hi, lo, row * dim + 4 * i, ovf);
     }
     if (ovf) atomicOr(overflow, 1u);
 }
 
-// per-layer power-of-two weight scale: the largest |w'| = |w| 2^s lands in [8192, 16384), so that hi keeps
-// its 11 bits and lo (<= 2^-12 |w'|) stays a normal fp16 number.  scales[0] = 2^s, scales[1] = 2^-s.
-__global__ void pick_wscale_kernel(const float *__restrict__ absmax, float *__restrict__ wscale,
-                                   float *__restrict__ inv_wscale) {
-    float m = *absmax;
+// ---- weight operand (tc_split_weight) ------------------------------------------------------------------------------
+__global__ void weight_absmax_kernel(const float *__restrict__ x, int64_t count, float scale, float *__restrict__ out) {
+    float m = 0.f;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
+        m = fmaxf(m, fabsf(x[i] * scale));
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<int *>(out), __float_as_int(m));   // m >= 0: int order == float order
+}
+
+// scal[2] = absmax -> scal[1] = 2^s, scal[0] = 2^-s with the largest |w 2^s| in [8192, 16384)
+__global__ void pick_wscale_kernel(float *__restrict__ scal) {
+    float m = scal[2];
     if (!(m > 0.f)) m = 1.f;
     int e = 0;
     frexpf(m, &e);                         // m = f * 2^e, f in [0.5, 1)
-    const int s = 14 - e;
-    *wscale = ldexpf(1.f, s);
-    *inv_wscale = ldexpf(1.f, -s);
+    scal[1] = ldexpf(1.f, 14 - e);
+    scal[0] = ldexpf(1.f, e - 14);
 }
 
-// weights: w' = (w*scale) * 2^s  ->  fp16 hi / lo
-__global__ void weight_split_kernel(const float *__restrict__ pw, int64_t count, const float *__restrict__ wscale_p,
-                                    __half *__restrict__ hi, __half *__restrict__ lo) {
-    const float wscale = *wscale_p;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x) {
-        tc::split1(pw[i] * wscale, hi[i], lo[i]);          // power-of-two scale: exact
+// one thread per (row, col) of W [rows, cols, taps]: w' = (scale W) 2^s (a power of two: exact) -> fp16 hi / lo at row
+// tap' rows + row, i.e. element tap' rows cols + idx; wsq[idx] = the fmaf chain of (scale W)^2 over the taps in order
+__global__ void weight_split_kernel(const float *__restrict__ W, int64_t total, int taps, float scale, int reverse,
+                                    const float *__restrict__ scal, __half *__restrict__ hi, __half *__restrict__ lo,
+                                    float *__restrict__ wsq) {
+    const float ws = scal[1];
+    for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+        float sq = 0.f;
+        for (int t = 0; t < taps; ++t) {
+            const float w = W[idx * taps + t] * scale;
+            sq = fmaf(w, w, sq);
+            const int64_t o = (int64_t)(reverse ? taps - 1 - t : t) * total + idx;
+            tc::split1(w * ws, hi[o], lo[o]);
+        }
+        if (wsq) wsq[idx] = sq;
     }
-}
-
-__global__ void absmax_kernel(const float *__restrict__ x, int64_t count, float *__restrict__ out) {
-    float m = 0.f;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
-        m = fmaxf(m, fabsf(x[i]));
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<int *>(out), __float_as_int(m));   // m >= 0: int order == float order
 }
 
 // ---- host side ------------------------------------------------------------------------------------------
@@ -332,14 +336,14 @@ static int make_tmap(CUtensorMap *map, const void *base, uint64_t rows, uint64_t
 }
 
 // Tensor-core packed layout (appended after the fp32 SIMT pack inside the same allocation):
-//   [n_layers][dim*dim] fp16 W_hi | [n_layers][dim*dim] fp16 W_lo | [3][n_layers] float {inv_wscale, wscale, absmax} | flag
+//   [n_layers][dim*dim] fp16 W_hi | [n_layers][dim*dim] fp16 W_lo | [n_layers][3] float {inv_wscale, wscale, absmax} | flag
 size_t mapping_tc_packed_bytes(int n_layers, int dim) {
     return align_up((size_t)n_layers * dim * dim * 2, 256) * 2 + align_up((size_t)3 * n_layers * sizeof(float), 256) + 256;
 }
 
 struct TcPackView {
     __half *w_hi, *w_lo;
-    float *inv_wscale, *wscale, *absmax;
+    float *scal;              // [n_layers][3], tc_split_weight's {inv_wscale, wscale, absmax}
     unsigned *overflow;
 };
 static TcPackView tc_pack_view(void *base, int n_layers, int dim) {
@@ -348,9 +352,7 @@ static TcPackView tc_pack_view(void *base, int n_layers, int dim) {
     size_t wb = align_up((size_t)n_layers * dim * dim * 2, 256);
     v.w_hi = reinterpret_cast<__half *>(p);
     v.w_lo = reinterpret_cast<__half *>(p + wb);
-    v.inv_wscale = reinterpret_cast<float *>(p + 2 * wb);
-    v.wscale = v.inv_wscale + n_layers;
-    v.absmax = v.wscale + n_layers;
+    v.scal = reinterpret_cast<float *>(p + 2 * wb);
     v.overflow = reinterpret_cast<unsigned *>(p + 2 * wb + align_up((size_t)3 * n_layers * sizeof(float), 256));
     return v;
 }
@@ -358,17 +360,31 @@ static TcPackView tc_pack_view(void *base, int n_layers, int dim) {
 // Splits the already scale-multiplied fp32 weights `pw` ([n_layers][dim*dim]); stream-ordered, no host sync.
 int mapping_tc_pack(const float *pw, int n_layers, int dim, void *tc_base, cudaStream_t st) {
     TcPackView v = tc_pack_view(tc_base, n_layers, dim);
-    GSB_CHECK_CUDA(cudaMemsetAsync(v.inv_wscale, 0, (size_t)3 * n_layers * sizeof(float), st));
+    GSB_CHECK_CUDA(cudaMemsetAsync(v.scal, 0, (size_t)3 * n_layers * sizeof(float), st));
     GSB_CHECK_CUDA(cudaMemsetAsync(v.overflow, 0, sizeof(unsigned), st));
     const int64_t per = (int64_t)dim * dim;
-    for (int l = 0; l < n_layers; ++l) {
-        absmax_kernel<<<64, 256, 0, st>>>(pw + l * per, per, v.absmax + l);
-        GSB_CHECK_LAUNCH();
-        pick_wscale_kernel<<<1, 1, 0, st>>>(v.absmax + l, v.wscale + l, v.inv_wscale + l);
-        GSB_CHECK_LAUNCH();
-        weight_split_kernel<<<256, 256, 0, st>>>(pw + l * per, per, v.wscale + l, v.w_hi + l * per, v.w_lo + l * per);
-        GSB_CHECK_LAUNCH();
+    for (int l = 0; l < n_layers; ++l)
+        if (int r = tc_split_weight(pw + l * per, dim, dim, 1, 1.0f, false, dim, v.w_hi + l * per, v.w_lo + l * per, v.scal + 3 * l,
+                                    nullptr, st)) return r;
+    return GSB_OK;
+}
+
+int tc_split_weight(const float *w, int rows, int cols, int taps, float scale, bool reverse_taps, int n_pad, __half *hi, __half *lo,
+                    float *scal, float *wsq, cudaStream_t st) {
+    const int64_t tap_rows = (int64_t)taps * rows, total = (int64_t)rows * cols;
+    GSB_CHECK_ARG(w && hi && lo && scal && rows > 0 && cols > 0 && taps > 0 && n_pad >= tap_rows && n_pad % 32 == 0,
+                  "tc_split_weight: bad shape (rows=%d cols=%d taps=%d n_pad=%d)", rows, cols, taps, n_pad);
+    if (n_pad > tap_rows) {
+        const size_t pad_bytes = (size_t)(n_pad - tap_rows) * cols * sizeof(__half);
+        GSB_CHECK_CUDA(cudaMemsetAsync(hi + tap_rows * cols, 0, pad_bytes, st));
+        GSB_CHECK_CUDA(cudaMemsetAsync(lo + tap_rows * cols, 0, pad_bytes, st));
     }
+    weight_absmax_kernel<<<256, 256, 0, st>>>(w, total * taps, scale, scal + 2);
+    GSB_CHECK_LAUNCH();
+    pick_wscale_kernel<<<1, 1, 0, st>>>(scal);
+    GSB_CHECK_LAUNCH();
+    weight_split_kernel<<<1024, 256, 0, st>>>(w, total, taps, scale, reverse_taps ? 1 : 0, scal, hi, lo, wsq);
+    GSB_CHECK_LAUNCH();
     return GSB_OK;
 }
 
@@ -446,12 +462,7 @@ int tc_linear(const float *x, const float *w, const float *bias, float *y, int64
     float *scal = (float *)(p0 + 2 * xb + 2 * wb);              // inv_wscale, wscale, absmax
     unsigned *overflow = (unsigned *)(p0 + 2 * xb + 2 * wb + 256);
     GSB_CHECK_CUDA(cudaMemsetAsync(scal, 0, 512, st));
-    absmax_kernel<<<256, 256, 0, st>>>(w, (int64_t)N * K, scal + 2);
-    GSB_CHECK_LAUNCH();
-    pick_wscale_kernel<<<1, 1, 0, st>>>(scal + 2, scal + 1, scal);
-    GSB_CHECK_LAUNCH();
-    weight_split_kernel<<<1024, 256, 0, st>>>(w, (int64_t)N * K, scal + 1, w_hi, w_lo);
-    GSB_CHECK_LAUNCH();
+    if (int r = tc_split_weight(w, N, K, 1, 1.0f, false, N, w_hi, w_lo, scal, nullptr, st)) return r;
     pixelnorm_split_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(x, x_hi, x_lo, n, K, 0, overflow);
     GSB_CHECK_LAUNCH();
     CUtensorMap tm_ah, tm_al, tm_wh, tm_wl;
@@ -498,7 +509,7 @@ int mapping_forward_tc(const float *pb, void *tc_base, int n_layers, int dim,
         p.out_lo = last ? nullptr : a_lo[dst];
         p.out_f32 = last ? d_w : nullptr;
         p.overflow = v.overflow;
-        p.inv_wscale = v.inv_wscale + l;
+        p.inv_wscale = v.scal + 3 * l;
         p.M = (int)n; p.N_total = dim; p.K = dim; p.mode = 0;
         if (int r = tc_launch_layer(tm_ah, tm_al, tm_wh, tm_wl, p, queue, leave_free_sms, st)) return r;
     }

@@ -20,20 +20,19 @@
 // activation is written as fp32 NHWC rows with a caller-given row stride.  Samples are processed in chunks whose tap planes
 // fit the L2.  The per-pixel reductions over channels use warp shuffles and a fixed-order shared-memory step: a sample's
 // result does not depend on the batch it is part of.
-#include "tc_common.cuh"
+#include "tap_conv.cuh"
 #include <math.h>
 
 namespace gsb {
 
 constexpr int PG_MAX_BLOCKS = 24;
-constexpr int64_t PG_CHUNK_ELEMS = (int64_t)2048 * 9 * 512;       // fp32 tap-plane elements per GEMM launch: 38 MB of the 50 MB L2
 
 static int pg_taps(const gsb_progan_block &c) { return c.ksize * c.ksize; }
 static int pg_res_out(const gsb_progan_block &c) { return c.ksize == 4 ? 4 : (c.upsample ? 2 * c.res_in : c.res_in); }
-// samples per chunk
+// samples per chunk: the tap planes of one GEMM launch fit TAP_CHUNK_ELEMS
 static int64_t pg_chunk_samples(const gsb_progan_block &c) {
     const int64_t per_sample = (int64_t)c.res_in * c.res_in * pg_taps(c) * c.cout;
-    const int64_t spc = PG_CHUNK_ELEMS / per_sample;
+    const int64_t spc = TAP_CHUNK_ELEMS / per_sample;
     return spc < 1 ? 1 : spc;
 }
 
@@ -83,41 +82,6 @@ static int pg_check(const gsb_progan_block *blocks, int n_blocks) {
     return GSB_OK;
 }
 
-// ---- pack kernels ---------------------------------------------------------------------------------------
-__global__ void pg_absmax_kernel(const float *__restrict__ x, int64_t count, float scale, float *__restrict__ out) {
-    float m = 0.f;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
-        m = fmaxf(m, fabsf(x[i] * scale));
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<int *>(out), __float_as_int(m));      // (max of non-negative floats: exact)
-}
-// scal[2] = absmax -> scal[1] = 2^s, scal[0] = 2^-s with the largest |w 2^s| in [8192, 16384)
-__global__ void pg_pick_scale_kernel(float *__restrict__ scal) {
-    float m = scal[2];
-    if (!(m > 0.f)) m = 1.f;
-    int e = 0;
-    frexpf(m, &e);
-    scal[1] = ldexpf(1.f, 14 - e);
-    scal[0] = ldexpf(1.f, e - 14);
-}
-// W[co,ci,ky,kx] -> rows (tap, co), K-major over ci, times scale*2^s, split into fp16 hi/lo; `reverse`: tap t -> taps-1-t
-__global__ void pg_weight_pack_kernel(const float *__restrict__ W, int cout, int cin, int taps, int reverse, float scale,
-                                      const float *__restrict__ scal, __half *__restrict__ hi, __half *__restrict__ lo) {
-    const float ws = scal[1];
-    const int64_t total = (int64_t)cout * cin * taps;
-    for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-        const int t = (int)(idx % taps);
-        const int64_t cc = idx / taps;
-        const int co = (int)(cc / cin), ci = (int)(cc % cin);
-        const int64_t o = ((int64_t)(reverse ? taps - 1 - t : t) * cout + co) * cin + ci;
-        tc::split1(W[idx] * scale * ws, hi[o], lo[o]);
-    }
-}
-__global__ void pg_scale_copy_kernel(const float *__restrict__ src, int64_t count, float scale, float *__restrict__ dst) {
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
-        dst[i] = src[i] * scale;
-}
-
 // ---- forward kernels ------------------------------------------------------------------------------------
 // PixelNorm of the latent (one warp per row) -> fp16 hi/lo operand of layer1
 __global__ void __launch_bounds__(256)
@@ -137,31 +101,9 @@ pg_latent_norm_kernel(const float *__restrict__ z, int64_t n, int c, __half *__r
     for (int k = 4 * lane; k < c; k += 128) {
         const float4 v = *reinterpret_cast<const float4 *>(zr + k);
         const float f[4] = {v.x / den, v.y / den, v.z / den, v.w / den};
-        uint2 ph, pl;
-        ovf |= tc::split4(f, ph, pl);
-        *reinterpret_cast<uint2 *>(hi + row * c + k) = ph;
-        *reinterpret_cast<uint2 *>(lo + row * c + k) = pl;
+        tc::store_split4(f, hi, lo, row * c + k, ovf);
     }
     if (ovf) atomicOr(overflow, 1u);
-}
-
-// Sum of v over the c/4 threads that hold one pixel's channels (consecutive threads, c/4 a power of two that divides the
-// block size; every thread of the block calls this).  Shuffles inside a warp, then for c >= 256 the 2 .. 8 warps of the pixel
-// are added in warp order from shared memory: the same order for every pixel, batch size and launch.
-__device__ __forceinline__ float pg_pixel_sum(float v, int cq) {
-    const int span = cq < 32 ? cq : 32;
-    for (int off = span >> 1; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-    if (cq > 32) {
-        __shared__ float red[8];
-        const int wib = threadIdx.x >> 5, wpp = cq >> 5;            // warp in block, warps per pixel
-        __syncthreads();                                            // the previous call's readers are done
-        if ((threadIdx.x & 31) == 0) red[wib] = v;
-        __syncthreads();
-        const int w0 = wib / wpp * wpp;
-        v = 0.f;
-        for (int k = 0; k < wpp; ++k) v += red[w0 + k];
-    }
-    return v;
 }
 
 struct PgEpi {
@@ -186,22 +128,19 @@ __device__ __forceinline__ void pg_epilogue(const PgEpi &e, float4 acc, bool val
     }
     if (!e.out_hi && !e.rgb_w) return;
     const int cq = c >> 2;
-    const float ss = pg_pixel_sum((f[0] * f[0] + f[1] * f[1]) + (f[2] * f[2] + f[3] * f[3]), cq);
+    const float ss = pixel_sum((f[0] * f[0] + f[1] * f[1]) + (f[2] * f[2] + f[3] * f[3]), cq);
     const float den = sqrtf(ss / (float)c + 1e-8f);
     const float g[4] = {f[0] / den, f[1] / den, f[2] / den, f[3] / den};
     if (e.out_hi && valid) {
-        uint2 ph, pl;
-        const bool ovf = tc::split4(g, ph, pl);
-        const int64_t off = (b * hw + pix) * (int64_t)c + 4 * q;
-        *reinterpret_cast<uint2 *>(e.out_hi + off) = ph;
-        *reinterpret_cast<uint2 *>(e.out_lo + off) = pl;
+        bool ovf = false;
+        tc::store_split4(g, e.out_hi, e.out_lo, (b * hw + pix) * (int64_t)c + 4 * q, ovf);
         if (ovf) atomicOr(e.overflow, 1u);
     }
     if (e.rgb_w) {
 #pragma unroll
         for (int o = 0; o < 3; ++o) {
             const float4 wv = *reinterpret_cast<const float4 *>(e.rgb_w + (int64_t)o * c + 4 * q);
-            const float r = pg_pixel_sum((g[0] * wv.x + g[1] * wv.y) + (g[2] * wv.z + g[3] * wv.w), cq);
+            const float r = pixel_sum((g[0] * wv.x + g[1] * wv.y) + (g[2] * wv.z + g[3] * wv.w), cq);
             if (valid && q == 0) e.rgb_out[(b * hw + pix) * 3 + o] = r + e.rgb_b[o];
         }
     }
@@ -221,25 +160,8 @@ pg_gather_kernel(const float *__restrict__ Y, int64_t nb, int R, int c, PgEpi e)
     const int64_t b = pixg / ((int64_t)R * R);
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
     if (valid) {
-        if (MODE == 0) {
-            acc = *reinterpret_cast<const float4 *>(Y + pixg * c + 4 * q);
-        } else {
-            const int H = (MODE == 2) ? (R >> 1) : R;
-#pragma unroll
-            for (int ky = 0; ky < 3; ++ky) {
-                const int yy = y + ky - 1;
-                if (yy < 0 || yy >= R) continue;
-                const int ys = (MODE == 2) ? (yy >> 1) : yy;
-#pragma unroll
-                for (int kx = 0; kx < 3; ++kx) {
-                    const int xx = x + kx - 1;
-                    if (xx < 0 || xx >= R) continue;
-                    const int xs = (MODE == 2) ? (xx >> 1) : xx;
-                    const float4 v = *reinterpret_cast<const float4 *>(Y + ((b * H + ys) * H + xs) * (int64_t)(9 * c) + (ky * 3 + kx) * c + 4 * q);
-                    acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-                }
-            }
-        }
+        if (MODE == 0) acc = *reinterpret_cast<const float4 *>(Y + pixg * c + 4 * q);
+        else acc = tap_sum3x3<MODE == 2>(Y, 9 * c, b, y, x, R, c, q);
     }
     pg_epilogue(e, acc, valid, b, y * R + x, R * R, c, q);
 }
@@ -297,21 +219,16 @@ extern "C" int gsb_progan_pack(const gsb_progan_block *blocks, int n_blocks, con
         // WScaleLayer.scale = gain / sqrt(fan_in), gain = sqrt2 / kernel_size, fan_in = in_channels (proggan.py:113,129-130)
         const float scale = (float)(sqrt(2.0) / c.ksize / sqrt((double)c.cin));
         const int taps = pg_taps(c);
-        const int64_t wcount = (int64_t)c.cout * c.cin * taps;
-        pg_absmax_kernel<<<128, 256, 0, st>>>(c.conv_weight, wcount, scale, v.L[l].scal + 2);
-        GSB_CHECK_LAUNCH();
-        pg_pick_scale_kernel<<<1, 1, 0, st>>>(v.L[l].scal);
-        GSB_CHECK_LAUNCH();
-        pg_weight_pack_kernel<<<256, 256, 0, st>>>(c.conv_weight, c.cout, c.cin, taps, c.ksize == 4, scale, v.L[l].scal, v.L[l].w_hi,
-                                                   v.L[l].w_lo);
-        GSB_CHECK_LAUNCH();
-        pg_scale_copy_kernel<<<4, 256, 0, st>>>(c.bias, c.cout, 1.0f, v.L[l].bias);
+        // layer1's taps are stored reversed (see the top of this file)
+        if (int r = tc_split_weight(c.conv_weight, c.cout, c.cin, taps, scale, c.ksize == 4, taps * c.cout, v.L[l].w_hi, v.L[l].w_lo,
+                                    v.L[l].scal, nullptr, st)) return r;
+        scale_copy_kernel<<<4, 256, 0, st>>>(c.bias, c.cout, 1.0f, nullptr, v.L[l].bias);
         GSB_CHECK_LAUNCH();
     }
     const int cl = blocks[n_blocks - 1].cout;
-    pg_scale_copy_kernel<<<4, 256, 0, st>>>(d_out_weight, (int64_t)3 * cl, (float)(1.0 / sqrt((double)cl)), v.out_w);   // gain 1 (proggan.py:163)
+    scale_copy_kernel<<<4, 256, 0, st>>>(d_out_weight, (int64_t)3 * cl, (float)(1.0 / sqrt((double)cl)), nullptr, v.out_w);   // gain 1 (proggan.py:163)
     GSB_CHECK_LAUNCH();
-    pg_scale_copy_kernel<<<1, 32, 0, st>>>(d_out_bias, 3, 1.0f, v.out_b);
+    scale_copy_kernel<<<1, 32, 0, st>>>(d_out_bias, 3, 1.0f, nullptr, v.out_b);
     GSB_CHECK_LAUNCH();
     return GSB_OK;
 }

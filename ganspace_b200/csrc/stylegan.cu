@@ -28,13 +28,12 @@
 //
 // Channel counts: cin and cout are powers of two in [16, 512].  The 16-channel layers of the 1024-px generators run on the same
 // path: the GEMM needs only K % 8 == 0, and its N = 9 cout is padded with zero weight rows to a multiple of 32.
-#include "tc_common.cuh"
+#include "tap_conv.cuh"
 #include <math.h>
 
 namespace gsb {
 
 constexpr int SG_MAX_LAYERS = 18;
-constexpr int64_t SG_CHUNK_ELEMS = (int64_t)2048 * 9 * 512;      // fp32 elements of the largest per-chunk buffer (38 MB)
 constexpr int SG_TILE_PASSES = 8;                                 // pixel passes of one epilogue block (the statistics tile)
 
 static int sg_np(const gsb_stylegan_layer &c) { return (9 * c.cout + 31) / 32 * 32; }           // GEMM N (padded)
@@ -49,7 +48,7 @@ static int64_t sg_chunk_samples(const gsb_stylegan_layer &c) {
     const int64_t hw_in = (int64_t)sg_res_in(c) * sg_res_in(c), hw = (int64_t)c.res_out * c.res_out;
     int64_t per = hw * c.cout;
     if (c.conv_weight && hw_in * sg_np(c) > per) per = hw_in * sg_np(c);
-    const int64_t spc = SG_CHUNK_ELEMS / per;
+    const int64_t spc = TAP_CHUNK_ELEMS / per;
     return spc < 1 ? 1 : spc;
 }
 
@@ -121,35 +120,6 @@ static int sg_check(const gsb_stylegan_layer *layers, int n_layers, int dlatent)
 }
 
 // ---- pack kernels ---------------------------------------------------------------------------------------
-__global__ void sg_absmax_kernel(const float *__restrict__ x, int64_t count, float scale, float *__restrict__ out) {
-    float m = 0.f;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
-        m = fmaxf(m, fabsf(x[i] * scale));
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<int *>(out), __float_as_int(m));      // (max of non-negative floats: exact)
-}
-// scal[2] = absmax -> scal[1] = 2^s, scal[0] = 2^-s with the largest |w 2^s| in [8192, 16384)
-__global__ void sg_pick_scale_kernel(float *__restrict__ scal) {
-    float m = scal[2];
-    if (!(m > 0.f)) m = 1.f;
-    int e = 0;
-    frexpf(m, &e);
-    scal[1] = ldexpf(1.f, 14 - e);
-    scal[0] = ldexpf(1.f, e - 14);
-}
-// W[co,ci,3,3] -> rows (tap, co), K-major over ci, times scale*2^s, split into fp16 hi/lo; `flip`: tap t -> 8-t (both axes)
-__global__ void sg_weight_pack_kernel(const float *__restrict__ W, int cout, int cin, int flip, float scale,
-                                      const float *__restrict__ scal, __half *__restrict__ hi, __half *__restrict__ lo) {
-    const float ws = scal[1];
-    const int64_t total = (int64_t)cout * cin * 9;
-    for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-        const int t = (int)(idx % 9);
-        const int64_t cc = idx / 9;
-        const int co = (int)(cc / cin), ci = (int)(cc % cin);
-        const int64_t o = ((int64_t)(flip ? 8 - t : t) * cout + co) * cin + ci;
-        tc::split1(W[idx] * scale * ws, hi[o], lo[o]);
-    }
-}
 // A [rows, K] (StyleMod lin.weight) -> dst[k * ld + r] = A[r, k] * scale; column `layer` tag per row
 __global__ void sg_transpose_scale_kernel(const float *__restrict__ A, int rows, int K, float scale, float *__restrict__ dst, int64_t ld,
                                           int *__restrict__ tag, int layer) {
@@ -158,14 +128,6 @@ __global__ void sg_transpose_scale_kernel(const float *__restrict__ A, int rows,
         dst[(int64_t)k * ld + r] = A[idx] * scale;
         if (k == 0) tag[r] = layer;
     }
-}
-__global__ void sg_scale_copy_kernel(const float *__restrict__ src, int64_t count, float scale, float *__restrict__ dst) {
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
-        dst[i] = src[i] * scale;
-}
-// const [C, 16] (NCHW of one sample) -> [16, C]
-__global__ void sg_const_pack_kernel(const float *__restrict__ src, int C, float *__restrict__ dst) {
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 16 * C; i += gridDim.x * blockDim.x) dst[(i % 16) * C + i / 16] = src[i];
 }
 
 // ---- forward kernels ------------------------------------------------------------------------------------
@@ -184,8 +146,8 @@ sg_style_kernel(const float *__restrict__ w, int w_layers, int64_t n, int dlaten
     S[b * s_run + j] = acc + bias[j];
 }
 
-// the 3x3 conv outputs of an up-conv layer (before the blur): out[b,y,x,co] = sum_tap Y[b,((y+ky-1)>>1, (x+kx-1)>>1),tap,co] over
-// 0 <= y+ky-1, x+kx-1 < R; Y at the input resolution R/2 with row length np.  One thread per 4 channels of an output pixel.
+// the 3x3 conv outputs of an up-conv layer (before the blur), from Y at the input resolution R/2 with row length np.  One thread
+// per 4 channels of an output pixel.
 __global__ void __launch_bounds__(256)
 sg_up_gather_kernel(const float *__restrict__ Y, int64_t nb, int R, int c, int np, float *__restrict__ U) {
     const int cq = c >> 2;
@@ -195,21 +157,7 @@ sg_up_gather_kernel(const float *__restrict__ Y, int64_t nb, int R, int c, int n
     const int64_t pixg = idx / cq;
     const int x = (int)(pixg % R), y = (int)((pixg / R) % R);
     const int64_t b = pixg / ((int64_t)R * R);
-    const int H = R >> 1;
-    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-    for (int ky = 0; ky < 3; ++ky) {
-        const int yy = y + ky - 1;
-        if (yy < 0 || yy >= R) continue;
-#pragma unroll
-        for (int kx = 0; kx < 3; ++kx) {
-            const int xx = x + kx - 1;
-            if (xx < 0 || xx >= R) continue;
-            const float4 v = *reinterpret_cast<const float4 *>(Y + ((b * H + (yy >> 1)) * H + (xx >> 1)) * (int64_t)np + (ky * 3 + kx) * c + 4 * q);
-            acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-        }
-    }
-    *reinterpret_cast<float4 *>(U + pixg * c + 4 * q) = acc;
+    *reinterpret_cast<float4 *>(U + pixg * c + 4 * q) = tap_sum3x3<true>(Y, np, b, y, x, R, c, q);
 }
 
 // MODE 0: the constant input (src = const [16, c]); 1: stride-1 3x3 gather (src = Y [nb*R*R, np]); 2: the blur of the up-conv
@@ -232,6 +180,8 @@ sg_epilogue_kernel(const float *__restrict__ src, int R, int c, int np, int tile
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
         if (MODE == 0) {
             acc = *reinterpret_cast<const float4 *>(src + (int64_t)p * c + 4 * q);
+        } else if (MODE == 1) {
+            acc = tap_sum3x3<false>(src, np, b, y, x, R, c, q);
         } else {
 #pragma unroll
             for (int ky = 0; ky < 3; ++ky) {
@@ -241,14 +191,9 @@ sg_epilogue_kernel(const float *__restrict__ src, int R, int c, int np, int tile
                 for (int kx = 0; kx < 3; ++kx) {
                     const int xx = x + kx - 1;
                     if (xx < 0 || xx >= R) continue;
-                    if (MODE == 1) {
-                        const float4 v = *reinterpret_cast<const float4 *>(src + ((b * R + yy) * R + xx) * (int64_t)np + (ky * 3 + kx) * c + 4 * q);
-                        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-                    } else {
-                        const float wgt = (float)((ky == 1 ? 2 : 1) * (kx == 1 ? 2 : 1)) * 0.0625f;
-                        const float4 v = *reinterpret_cast<const float4 *>(src + ((b * R + yy) * R + xx) * (int64_t)c + 4 * q);
-                        acc.x = fmaf(wgt, v.x, acc.x); acc.y = fmaf(wgt, v.y, acc.y); acc.z = fmaf(wgt, v.z, acc.z); acc.w = fmaf(wgt, v.w, acc.w);
-                    }
+                    const float wgt = (float)((ky == 1 ? 2 : 1) * (kx == 1 ? 2 : 1)) * 0.0625f;
+                    const float4 v = *reinterpret_cast<const float4 *>(src + ((b * R + yy) * R + xx) * (int64_t)c + 4 * q);
+                    acc.x = fmaf(wgt, v.x, acc.x); acc.y = fmaf(wgt, v.y, acc.y); acc.z = fmaf(wgt, v.z, acc.z); acc.w = fmaf(wgt, v.w, acc.w);
                 }
             }
         }
@@ -304,24 +249,6 @@ sg_finish_kernel(const double *__restrict__ part, int64_t nb, int c, int tiles, 
     }
 }
 
-// Sum of v over the c/4 threads that hold one pixel's channels (consecutive threads, c/4 a power of two that divides the block
-// size; every thread of the block calls this): shuffles inside a warp, then for c >= 256 the warps of the pixel in warp order.
-__device__ __forceinline__ float sg_pixel_sum(float v, int cq) {
-    const int span = cq < 32 ? cq : 32;
-    for (int off = span >> 1; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-    if (cq > 32) {
-        __shared__ float red[8];
-        const int wib = threadIdx.x >> 5, wpp = cq >> 5;
-        __syncthreads();
-        if ((threadIdx.x & 31) == 0) red[wib] = v;
-        __syncthreads();
-        const int w0 = wib / wpp * wpp;
-        v = 0.f;
-        for (int k = 0; k < wpp; ++k) v += red[w0 + k];
-    }
-    return v;
-}
-
 struct SgApply {
     const float *A;              // [nb, hw, c] pre-norm activation (chunk-local)
     const float4 *aff;           // [nb, c]
@@ -353,10 +280,8 @@ sg_apply_kernel(SgApply e, int64_t nb, int hw, int c) {
         }
         if (e.out_f32) *reinterpret_cast<float4 *>(e.out_f32 + b * e.ld + (int64_t)pix * c + 4 * q) = make_float4(y[0], y[1], y[2], y[3]);
         if (e.out_hi) {
-            uint2 ph, pl;
-            const bool ovf = tc::split4(y, ph, pl);
-            *reinterpret_cast<uint2 *>(e.out_hi + pixg * c + 4 * q) = ph;
-            *reinterpret_cast<uint2 *>(e.out_lo + pixg * c + 4 * q) = pl;
+            bool ovf = false;
+            tc::store_split4(y, e.out_hi, e.out_lo, pixg * c + 4 * q, ovf);
             if (ovf) atomicOr(e.overflow, 1u);
         }
     }
@@ -364,7 +289,7 @@ sg_apply_kernel(SgApply e, int64_t nb, int hw, int c) {
 #pragma unroll
         for (int o = 0; o < 3; ++o) {
             const float4 wv = *reinterpret_cast<const float4 *>(e.rgb_w + (int64_t)o * c + 4 * q);
-            const float r = sg_pixel_sum((y[0] * wv.x + y[1] * wv.y) + (y[2] * wv.z + y[3] * wv.w), cq);
+            const float r = pixel_sum((y[0] * wv.x + y[1] * wv.y) + (y[2] * wv.z + y[3] * wv.w), cq);
             if (valid && q == 0) e.rgb_out[pixg * 3 + o] = r + e.rgb_b[o];
         }
     }
@@ -428,7 +353,7 @@ extern "C" int gsb_stylegan_pack(const gsb_stylegan_layer *layers, int n_layers,
     if (packed_bytes < v.bytes) { set_error("stylegan_pack: buffer too small (%zu < %zu)", packed_bytes, v.bytes); return GSB_ERR_WORKSPACE; }
     cudaStream_t st = (cudaStream_t)stream;
     GSB_CHECK_CUDA(cudaMemsetAsync(d_packed, 0, v.bytes, st));
-    sg_const_pack_kernel<<<8, 256, 0, st>>>(d_const, layers[0].cout, v.cst);
+    const_nhwc_kernel<<<8, 256, 0, st>>>(d_const, layers[0].cout, v.cst);
     GSB_CHECK_LAUNCH();
     for (int l = 0; l < n_layers; ++l) {
         const gsb_stylegan_layer &c = layers[l];
@@ -437,33 +362,28 @@ extern "C" int gsb_stylegan_pack(const gsb_stylegan_layer *layers, int n_layers,
         if (c.conv_weight) {
             // MyConv2d with use_wscale, gain sqrt2, lrmul 1: w_mul = sqrt2 / sqrt(cin * 9) (model.py:51-62)
             const float scale = (float)(sqrt(2.0) / sqrt(9.0 * c.cin));
-            const int64_t wcount = (int64_t)c.cout * c.cin * 9;
-            sg_absmax_kernel<<<128, 256, 0, st>>>(c.conv_weight, wcount, scale, v.L[l].scal + 2);
-            GSB_CHECK_LAUNCH();
-            sg_pick_scale_kernel<<<1, 1, 0, st>>>(v.L[l].scal);
-            GSB_CHECK_LAUNCH();
-            sg_weight_pack_kernel<<<256, 256, 0, st>>>(c.conv_weight, c.cout, c.cin, sg_flipped(c) ? 1 : 0, scale, v.L[l].scal,
-                                                       v.L[l].w_hi, v.L[l].w_lo);
-            GSB_CHECK_LAUNCH();
+            // the flipped kernel (both spatial axes) of a 3x3 conv is its taps in reverse order
+            if (int r = tc_split_weight(c.conv_weight, c.cout, c.cin, 9, scale, sg_flipped(c), sg_np(c), v.L[l].w_hi, v.L[l].w_lo,
+                                        v.L[l].scal, nullptr, st)) return r;
         }
-        sg_scale_copy_kernel<<<4, 256, 0, st>>>(c.bias, c.cout, 1.0f, v.L[l].bias);
+        scale_copy_kernel<<<4, 256, 0, st>>>(c.bias, c.cout, 1.0f, nullptr, v.L[l].bias);
         GSB_CHECK_LAUNCH();
-        sg_scale_copy_kernel<<<4, 256, 0, st>>>(c.noise_weight, c.cout, 1.0f, v.L[l].noise_w);
+        scale_copy_kernel<<<4, 256, 0, st>>>(c.noise_weight, c.cout, 1.0f, nullptr, v.L[l].noise_w);
         GSB_CHECK_LAUNCH();
-        sg_scale_copy_kernel<<<64, 256, 0, st>>>(c.noise, (int64_t)c.res_out * c.res_out, 1.0f, v.L[l].noise);
+        scale_copy_kernel<<<64, 256, 0, st>>>(c.noise, (int64_t)c.res_out * c.res_out, 1.0f, nullptr, v.L[l].noise);
         GSB_CHECK_LAUNCH();
         // StyleMod lin: MyLinear(dlatent, 2 cout, gain 1, use_wscale): w_mul = 1 / sqrt(dlatent), b_mul = 1 (model.py:121-131)
         sg_transpose_scale_kernel<<<256, 256, 0, st>>>(c.style_weight, 2 * c.cout, dlatent, (float)(1.0 / sqrt((double)dlatent)),
                                                        v.style_wt + v.L[l].style_off, v.s_total, v.style_layer + v.L[l].style_off, l);
         GSB_CHECK_LAUNCH();
-        sg_scale_copy_kernel<<<4, 256, 0, st>>>(c.style_bias, 2 * c.cout, 1.0f, v.style_b + v.L[l].style_off);
+        scale_copy_kernel<<<4, 256, 0, st>>>(c.style_bias, 2 * c.cout, 1.0f, nullptr, v.style_b + v.L[l].style_off);
         GSB_CHECK_LAUNCH();
     }
     const int cl = layers[n_layers - 1].cout;
     // torgb: MyConv2d(c, 3, 1, gain 1, use_wscale): w_mul = 1 / sqrt(c)
-    sg_scale_copy_kernel<<<4, 256, 0, st>>>(d_rgb_weight, (int64_t)3 * cl, (float)(1.0 / sqrt((double)cl)), v.rgb_w);
+    scale_copy_kernel<<<4, 256, 0, st>>>(d_rgb_weight, (int64_t)3 * cl, (float)(1.0 / sqrt((double)cl)), nullptr, v.rgb_w);
     GSB_CHECK_LAUNCH();
-    sg_scale_copy_kernel<<<1, 32, 0, st>>>(d_rgb_bias, 3, 1.0f, v.rgb_b);
+    scale_copy_kernel<<<1, 32, 0, st>>>(d_rgb_bias, 3, 1.0f, nullptr, v.rgb_b);
     GSB_CHECK_LAUNCH();
     return GSB_OK;
 }

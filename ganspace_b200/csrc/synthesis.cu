@@ -20,7 +20,7 @@
 // over channels; between layers they travel as fp16 hi/lo pairs already multiplied by the NEXT layer's style.
 // The hooked layer's activation is written as fp32 NHWC rows of length res*res*co with a caller-given row stride
 // (directly into the large-d IPCA batch buffer).  Samples are processed in chunks whose tap planes (Y) fit the L2.
-#include "tc_common.cuh"
+#include "tap_conv.cuh"
 #include <math.h>
 
 namespace gsb {
@@ -87,53 +87,6 @@ static int check_layers(const gsb_styled_conv *layers, int n_layers, int style_d
     return GSB_OK;
 }
 
-// ---- pack kernels ---------------------------------------------------------------------------------------
-__global__ void sy_absmax_kernel(const float *__restrict__ x, int64_t count, float scale, float *__restrict__ out) {
-    float m = 0.f;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
-        m = fmaxf(m, fabsf(x[i] * scale));
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<int *>(out), __float_as_int(m));
-}
-// scal[2] = absmax -> scal[1] = 2^s, scal[0] = 2^-s with the largest |w 2^s| in [8192, 16384)
-__global__ void sy_pick_scale_kernel(float *__restrict__ scal) {
-    float m = scal[2];
-    if (!(m > 0.f)) m = 1.f;
-    int e = 0;
-    frexpf(m, &e);
-    scal[1] = ldexpf(1.f, 14 - e);
-    scal[0] = ldexpf(1.f, e - 14);
-}
-// W[co,ci,ky,kx] -> rows (tap, co), K-major over ci, times scale*2^s, split into fp16 hi/lo; and wsq[co,ci]
-__global__ void sy_weight_pack_kernel(const float *__restrict__ W, int cout, int cin, float scale, const float *__restrict__ scal,
-                                      __half *__restrict__ hi, __half *__restrict__ lo, float *__restrict__ wsq) {
-    const float ws = scal[1];
-    const int64_t total = (int64_t)cout * cin;
-    for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-        const int co = (int)(idx / cin), ci = (int)(idx % cin);
-        float sq = 0.f;
-#pragma unroll
-        for (int tap = 0; tap < 9; ++tap) {
-            const float w = W[idx * 9 + tap] * scale;
-            sq = fmaf(w, w, sq);
-            const int64_t o = ((int64_t)tap * cout + co) * cin + ci;
-            tc::split1(w * ws, hi[o], lo[o]);
-        }
-        wsq[idx] = sq;
-    }
-}
-__global__ void sy_scale_copy_kernel(const float *__restrict__ src, int64_t count, float scale, const float *__restrict__ dev_scale,
-                                     float *__restrict__ dst) {
-    const float s = dev_scale ? scale * dev_scale[0] : scale;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
-        dst[i] = src[i] * s;
-}
-// const[c, 4, 4] -> [16, c]
-__global__ void sy_const_nhwc_kernel(const float *__restrict__ src, int c, float *__restrict__ dst) {
-    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx < 16 * c) { const int p = idx / c, ch = idx % c; dst[idx] = src[ch * 16 + p]; }
-}
-
 // ---- forward kernels ------------------------------------------------------------------------------------
 __global__ void sy_square_kernel(const float *__restrict__ x, int64_t count, float *__restrict__ y) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -142,13 +95,6 @@ __global__ void sy_square_kernel(const float *__restrict__ x, int64_t count, flo
 __global__ void sy_rsqrt_eps_kernel(float *__restrict__ x, int64_t count) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i < count) x[i] = 1.0f / sqrtf(x[i] + 1e-8f);
-}
-
-__device__ __forceinline__ void store_split4(const float (&f)[4], __half *hi, __half *lo, int64_t off, bool &ovf) {
-    uint2 ph, pl;
-    ovf |= tc::split4(f, ph, pl);
-    *reinterpret_cast<uint2 *>(hi + off) = ph;
-    *reinterpret_cast<uint2 *>(lo + off) = pl;
 }
 
 // ConstantInput (model.py:300-304) times the first layer's style: out[b,p,c] = const[p,c] * s[b,c]  -> hi/lo
@@ -165,7 +111,7 @@ __global__ void sy_const_modulate_kernel(const float *__restrict__ cst, const fl
     const float4 sv = *reinterpret_cast<const float4 *>(s + b * c + 4 * q);
     const float f[4] = {cv.x * sv.x, cv.y * sv.y, cv.z * sv.z, cv.w * sv.w};
     bool ovf = false;
-    store_split4(f, hi, lo, pix * c + 4 * q, ovf);
+    tc::store_split4(f, hi, lo, pix * c + 4 * q, ovf);
     if (ovf) atomicOr(overflow, 1u);
 }
 
@@ -258,7 +204,7 @@ __device__ __forceinline__ void sy_epilogue(const EpiParams &e, float4 acc, int6
         const float4 sn = *reinterpret_cast<const float4 *>(e.s_next + b * c + 4 * q);
         f[0] *= sn.x; f[1] *= sn.y; f[2] *= sn.z; f[3] *= sn.w;
         bool ovf = false;
-        store_split4(f, e.out_hi, e.out_lo, (b * hw + pix) * (int64_t)c + 4 * q, ovf);
+        tc::store_split4(f, e.out_hi, e.out_lo, (b * hw + pix) * (int64_t)c + 4 * q, ovf);
         if (ovf) atomicOr(e.overflow, 1u);
     } else if (e.out_f32) {
         *reinterpret_cast<float4 *>(e.out_f32 + b * e.ld + (int64_t)pix * c + 4 * q) = make_float4(f[0], f[1], f[2], f[3]);
@@ -294,30 +240,17 @@ __global__ void sy_rgb_init_kernel(const float *__restrict__ bias, const float *
     o[0] = acc[0]; o[1] = acc[1]; o[2] = acc[2];
 }
 
-// stride-1 3x3: gather the nine tap planes.  Y [nb*H*W, 9*c]
+// stride-1 3x3: gather the nine tap planes.  Y [nb*R*R, 9*c]
 __global__ void __launch_bounds__(256)
-sy_conv_gather_kernel(const float *__restrict__ Y, int64_t nb, int H, int W, int c, EpiParams e) {
+sy_conv_gather_kernel(const float *__restrict__ Y, int64_t nb, int R, int c, EpiParams e) {
     const int cq = c >> 2;
     const int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (idx >= nb * H * W * cq) return;
+    if (idx >= nb * R * R * cq) return;
     const int q = (int)(idx % cq);
     const int64_t pixg = idx / cq;
-    const int x = (int)(pixg % W), y = (int)((pixg / W) % H);
-    const int64_t b = pixg / ((int64_t)W * H);
-    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-    for (int ky = 0; ky < 3; ++ky) {
-        const int yy = y + ky - 1;
-        if (yy < 0 || yy >= H) continue;
-#pragma unroll
-        for (int kx = 0; kx < 3; ++kx) {
-            const int xx = x + kx - 1;
-            if (xx < 0 || xx >= W) continue;
-            const float4 v = *reinterpret_cast<const float4 *>(Y + ((b * H + yy) * W + xx) * (int64_t)(9 * c) + (ky * 3 + kx) * c + 4 * q);
-            acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-        }
-    }
-    sy_epilogue(e, acc, b, y * W + x, H * W, c, q);
+    const int x = (int)(pixg % R), y = (int)((pixg / R) % R);
+    const int64_t b = pixg / ((int64_t)R * R);
+    sy_epilogue(e, tap_sum3x3<false>(Y, 9 * c, b, y, x, R, c, q), b, y * R + x, R * R, c, q);
 }
 
 // stride-2 transposed conv: T[b,u,v,:] on the (2H+1) x (2W+1) grid = sum of the tap planes that land on (u,v)
@@ -447,7 +380,7 @@ extern "C" int gsb_synthesis_pack(const gsb_styled_conv *layers, int n_layers, i
     cudaStream_t st = (cudaStream_t)stream;
     GSB_CHECK_CUDA(cudaMemsetAsync(d_packed, 0, v.bytes, st));
     const int c0 = layers[0].cin;
-    sy_const_nhwc_kernel<<<(16 * c0 + 255) / 256, 256, 0, st>>>(d_const_input, c0, v.const_nhwc);
+    const_nhwc_kernel<<<8, 256, 0, st>>>(d_const_input, c0, v.const_nhwc);
     GSB_CHECK_LAUNCH();
     for (int l = 0; l < n_layers; ++l) {
         const gsb_styled_conv &c = layers[l];
@@ -455,21 +388,16 @@ extern "C" int gsb_synthesis_pack(const gsb_styled_conv *layers, int n_layers, i
                       "synthesis_pack: layer %d has a null parameter pointer", l);
         const float scale = (float)(1.0 / sqrt((double)c.cin * 9.0));           // ModulatedConv2d.scale (model.py:219-220)
         const float mscale = (float)(1.0 / sqrt((double)style_dim));              // EqualLinear.scale, lr_mul = 1 (model.py:143)
-        const int64_t wcount = (int64_t)c.cout * c.cin * 9;
-        sy_absmax_kernel<<<128, 256, 0, st>>>(c.conv_weight, wcount, scale, v.L[l].scal + 2);
+        if (int r = tc_split_weight(c.conv_weight, c.cout, c.cin, 9, scale, false, 9 * c.cout, v.L[l].w_hi, v.L[l].w_lo, v.L[l].scal,
+                                    v.L[l].wsq, st)) return r;
+        scale_copy_kernel<<<128, 256, 0, st>>>(c.mod_weight, (int64_t)c.cin * style_dim, mscale, nullptr, v.L[l].modw);
         GSB_CHECK_LAUNCH();
-        sy_pick_scale_kernel<<<1, 1, 0, st>>>(v.L[l].scal);
+        scale_copy_kernel<<<4, 256, 0, st>>>(c.mod_bias, c.cin, 1.0f, nullptr, v.L[l].modb);
         GSB_CHECK_LAUNCH();
-        sy_weight_pack_kernel<<<256, 256, 0, st>>>(c.conv_weight, c.cout, c.cin, scale, v.L[l].scal, v.L[l].w_hi, v.L[l].w_lo, v.L[l].wsq);
-        GSB_CHECK_LAUNCH();
-        sy_scale_copy_kernel<<<128, 256, 0, st>>>(c.mod_weight, (int64_t)c.cin * style_dim, mscale, nullptr, v.L[l].modw);
-        GSB_CHECK_LAUNCH();
-        sy_scale_copy_kernel<<<4, 256, 0, st>>>(c.mod_bias, c.cin, 1.0f, nullptr, v.L[l].modb);
-        GSB_CHECK_LAUNCH();
-        sy_scale_copy_kernel<<<4, 256, 0, st>>>(c.act_bias, c.cout, 1.0f, nullptr, v.L[l].actb);
+        scale_copy_kernel<<<4, 256, 0, st>>>(c.act_bias, c.cout, 1.0f, nullptr, v.L[l].actb);
         GSB_CHECK_LAUNCH();
         const int ro = res_out_of(c);
-        sy_scale_copy_kernel<<<64, 256, 0, st>>>(c.noise, (int64_t)ro * ro, 1.0f, c.noise_weight, v.L[l].noise);
+        scale_copy_kernel<<<64, 256, 0, st>>>(c.noise, (int64_t)ro * ro, 1.0f, c.noise_weight, v.L[l].noise);
         GSB_CHECK_LAUNCH();
     }
     return GSB_OK;
@@ -536,7 +464,7 @@ static int synthesis_run(const void *d_packed, const gsb_styled_conv *layers, in
                           "synthesis: ToRGB %d does not match layer %d (cin=%d, cout=%d)", j, l, t.cin, c.cout);
             rgb_cur = (j == n_rgb - 1) ? d_rgb_out : w.rgb[j & 1];
             const float mscale = (float)(1.0 / sqrt((double)style_dim));
-            sy_scale_copy_kernel<<<64, 256, 0, st>>>(t.mod_weight, (int64_t)c.cout * style_dim, mscale, nullptr, w.rgb_modw);
+            scale_copy_kernel<<<64, 256, 0, st>>>(t.mod_weight, (int64_t)c.cout * style_dim, mscale, nullptr, w.rgb_modw);
             GSB_CHECK_LAUNCH();
             if (int r = sy_linear(latent(2 * j + 1), w.rgb_modw, t.mod_bias, w.rgb_s, n, c.cout, style_dim, stream)) return r;
             const int64_t tot = n * hw_out;
@@ -572,7 +500,7 @@ static int synthesis_run(const void *d_packed, const gsb_styled_conv *layers, in
                 GSB_CHECK_LAUNCH();
             } else {
                 const int64_t o_total = nb * hw_out * cq;
-                sy_conv_gather_kernel<<<(unsigned)((o_total + 255) / 256), 256, 0, st>>>(w.Y, nb, H, H, c.cout, e);
+                sy_conv_gather_kernel<<<(unsigned)((o_total + 255) / 256), 256, 0, st>>>(w.Y, nb, H, c.cout, e);
                 GSB_CHECK_LAUNCH();
             }
         }

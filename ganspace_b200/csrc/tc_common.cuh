@@ -142,6 +142,13 @@ __device__ __forceinline__ bool split4(const float (&f)[4], uint2 &hi, uint2 &lo
     split2(f[2], f[3], hi.y, lo.y);
     return (fabsf(f[0]) > 60000.f) | (fabsf(f[1]) > 60000.f) | (fabsf(f[2]) > 60000.f) | (fabsf(f[3]) > 60000.f);
 }
+// split4 stored at hi + off and lo + off (off a multiple of 4); ovf |= the overflow test
+__device__ __forceinline__ void store_split4(const float (&f)[4], __half *hi, __half *lo, int64_t off, bool &ovf) {
+    uint2 ph, pl;
+    ovf |= split4(f, ph, pl);
+    *reinterpret_cast<uint2 *>(hi + off) = ph;
+    *reinterpret_cast<uint2 *>(lo + off) = pl;
+}
 
 }  // namespace tc
 
@@ -183,5 +190,16 @@ int tc_linear(const float *x, const float *w, const float *bias, float *y, int64
               cudaStream_t st);
 int tc_gemm_plain(const __half *a_hi, const __half *a_lo, int64_t M, int K, const __half *w_hi, const __half *w_lo, int N,
                   const float *inv_wscale, float *out, unsigned *overflow, unsigned *queue, int leave_free_sms, cudaStream_t st);
+// The weight operand of tc_gemm_plain and of the mapping layers from fp32 W [rows, cols, taps] (taps fastest).  The operand is
+// w' = scale W 2^s, with the power of two that puts max |w'| in [8192, 16384): hi keeps its 11 bits and lo = fp16(w' - hi) stays
+// a normal fp16 number.  Writes
+//   scal [3]          {inv_wscale = 2^-s (the pointer the GEMM takes), wscale = 2^s, absmax = max |scale W|}; scal[2] must be
+//                     zero on entry (it is an atomic max)
+//   hi, lo [n_pad, cols]  row tap' rows + r = w'[r, :, tap], tap' = tap or, with reverse_taps, taps - 1 - tap; rows from
+//                     taps rows to n_pad (a multiple of 32, the GEMM's N) are zero
+//   wsq [rows, cols]  (unless nullptr) the sum over taps, in tap order, of (scale W)^2 as an fmaf chain
+// Stream-ordered, no host sync.
+int tc_split_weight(const float *w, int rows, int cols, int taps, float scale, bool reverse_taps, int n_pad, __half *hi, __half *lo,
+                    float *scal, float *wsq, cudaStream_t st);
 
 }  // namespace gsb

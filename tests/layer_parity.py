@@ -12,9 +12,9 @@ test whose batch fits one chunk, so every per-layer test runs a batch that spans
 one sample, ends in a partly filled one (``parity_batch``)."""
 import numpy as np
 
-# csrc/progan.cu PG_CHUNK_ELEMS / pg_chunk_samples: fp32 tap-plane elements per GEMM launch
+# csrc/tap_conv.cuh TAP_CHUNK_ELEMS / progan.cu pg_chunk_samples: fp32 tap-plane elements per GEMM launch
 PG_CHUNK_ELEMS = 2048 * 9 * 512
-# csrc/stylegan.cu SG_CHUNK_ELEMS / sg_chunk_samples: elements of the largest per-chunk buffer
+# csrc/tap_conv.cuh TAP_CHUNK_ELEMS / stylegan.cu sg_chunk_samples: elements of the largest per-chunk buffer
 SG_CHUNK_ELEMS = 2048 * 9 * 512
 # csrc/synthesis.cu SY_CHUNK_ROWS / chunk_samples: GEMM rows (input pixels) per launch
 SY_CHUNK_ROWS = 2048
