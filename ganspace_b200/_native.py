@@ -399,6 +399,30 @@ def mt19937_raw(seeds, n_per_stream: int, device) -> torch.Tensor:
 MAPPING_DEFAULT = "tc"
 
 
+def source_key(tensors, *extra) -> tuple:
+    """What a packed copy of ``tensors`` depends on: ``(t._version, t.data_ptr())`` of each tensor (``None`` entries skipped),
+    so that an in-place edit and a replaced storage both show, followed by the ``extra`` values."""
+    return tuple((t._version, t.data_ptr()) for t in tensors if t is not None) + extra
+
+
+class Repacked:
+    """The last object built from a set of source tensors (a packed generator, a folded weight); ``get`` rebuilds it when
+    ``source_key`` of the sources changes."""
+
+    def __init__(self):
+        self._key = self._obj = None
+
+    def get(self, tensors, build, *extra):
+        key = source_key(tensors, *extra)
+        if self._obj is None or self._key != key:
+            self._obj, self._key = build(), key
+        return self._obj
+
+    def current(self):
+        """The last object built, or None; never builds."""
+        return self._obj
+
+
 class PackedMapping:
     """Pre-scaled mapping-network weights in the layout the kernels read (gsb_mapping_pack)."""
 

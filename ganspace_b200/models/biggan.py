@@ -26,14 +26,13 @@ from __future__ import annotations
 import math
 import os
 import re
-from pathlib import Path
 
 import numpy as np
 import torch
 from torch import nn
 
 from .. import _native
-from .wrappers import BaseModel, _global_seed
+from .wrappers import _checkpoint, _DeviceGenerator, _global_seed
 
 # ImageNet class ids for the names GANSpace's configs use (the reference resolves names through
 # nltk/WordNet, biggan utils.py:174-216, which is not available offline)
@@ -80,17 +79,14 @@ class _SNParams(nn.Module):
         self.weight_orig = nn.Parameter(sn.weight_orig.detach().clone())
         self.register_buffer("weight_u", sn.weight_u.detach().clone())
         self.register_buffer("weight_v", sn.weight_v.detach().clone())
-        self._eff = None
-        self._key = None
+        self.weight_cache = _native.Repacked()
 
     def effective_weight(self) -> torch.Tensor:
-        key = (self.weight_orig._version, self.weight_orig.data_ptr(), self.weight_u._version, self.weight_v._version)
-        if self._eff is None or self._key != key:
+        def build():
             w = self.weight_orig.detach()
             sigma = torch.dot(self.weight_u, torch.mv(w.reshape(w.shape[0], -1), self.weight_v))      # torch spectral_norm, eval mode
-            self._eff = (w / sigma).contiguous()
-            self._key = key
-        return self._eff
+            return (w / sigma).contiguous()
+        return self.weight_cache.get([self.weight_orig, self.weight_u, self.weight_v], build)
 
 
 class SNLinear(_SNParams):
@@ -394,7 +390,9 @@ class _Chain:
         return img
 
 
-class BigGAN(BaseModel):
+class BigGAN(_DeviceGenerator):
+    _latent_shape = (1, 128)
+
     def __init__(self, device, resolution, class_name, truncation=1.0, random_init=None):
         super().__init__(f"BigGAN-{resolution}", class_name)
         self.device = _native.require_cuda(device)
@@ -410,27 +408,20 @@ class BigGAN(BaseModel):
     def load_model(self, name):
         if self.resolution not in _LAYERS:
             raise RuntimeError("Unknown BigGAN model name", name)
-        root = os.environ.get("GANCONTROL_CHECKPOINT_DIR", Path(__file__).parent / "checkpoints")
-        weights = Path(root) / name / "pytorch_model.bin"
-        seed = self._random_init
-        if seed is None and os.environ.get("GANSPACE_B200_RANDOM_INIT"):
-            seed = int(os.environ["GANSPACE_B200_RANDOM_INIT_BIGGAN"]) if os.environ.get("GANSPACE_B200_RANDOM_INIT_BIGGAN") \
-                else int(os.environ["GANSPACE_B200_RANDOM_INIT"])
-        if weights.is_file() and seed is None:
+        source = self._weight_source(_checkpoint(f"{name}/pytorch_model.bin"), overrides=("GANSPACE_B200_RANDOM_INIT_BIGGAN",))
+        if isinstance(source, int):
+            torch.manual_seed(source)
             net = _BigGANNet(self.resolution)
-            net.load_state_dict(torch.load(weights, map_location="cpu"), strict=False)      # as BigGAN.from_pretrained
-        elif seed is not None:
-            torch.manual_seed(int(seed))
-            net = _BigGANNet(self.resolution)
-            synthesis_fill(net, int(seed))
+            synthesis_fill(net, source)
         else:
-            raise RuntimeError(f"BigGAN weights {weights} not found and no network access; pass random_init=<seed>")
+            net = _BigGANNet(self.resolution)
+            net.load_state_dict(torch.load(source, map_location="cpu"), strict=False)      # as BigGAN.from_pretrained
         # only the embedding and gen_z go to the device here: the synthesis weights are folded and uploaded on the first
         # synthesis call (_chain), so that gen_z-only runs (decomposition of generator.gen_z) never touch them
         net.embeddings.to(self.device)
         net.generator.gen_z.to(self.device)
         self.model = net
-        self._chain_cache = None
+        self._chain_cache = _native.Repacked()
 
     # ---- latents ----------------------------------------------------------------------------------
     def sample_latent(self, n_samples=1, truncation=None, seed=None):
@@ -497,10 +488,7 @@ class BigGAN(BaseModel):
         """The synthesis weights folded and uploaded at the current truncation (again when a parameter or buffer changes)."""
         g = self.model.generator
         tensors = [t for m in (g.layers, g.bn, g.conv_to_rgb) for t in list(m.parameters()) + list(m.buffers())]
-        key = (float(self.truncation), tuple((t._version, t.data_ptr()) for t in tensors))
-        if self._chain_cache is None or self._chain_cache[0] != key:
-            self._chain_cache = (key, _Chain(self.model, float(self.truncation), self.device))
-        return self._chain_cache[1]
+        return self._chain_cache.get(tensors, lambda: _Chain(self.model, float(self.truncation), self.device), float(self.truncation))
 
     def _synthesize(self, x, n_modules, want_image):
         """gen_z, then generator.layers[:n_modules] (and the tail when ``want_image``), firing the hooks of every layer on the
@@ -527,10 +515,7 @@ class BigGAN(BaseModel):
             else:
                 act = chain.attn(i, act)
             if len(mod._forward_hooks):
-                view = act.permute(0, 3, 1, 2)                             # NCHW view of NHWC storage
-                if mod(_result=view) is not view and (want_image or i < len(layers) - 1):
-                    raise NotImplementedError(f"an edit on layer 'generator.layers.{i}' cannot be propagated through the "
-                                              "BigGAN chain")
+                self._hand_off(mod, act, act.shape[1], act.shape[3], want_image or i < len(layers) - 1, f"generator.layers.{i}")
         return chain.rgb(act).permute(0, 3, 1, 2) if want_image else None
 
     def forward(self, x):

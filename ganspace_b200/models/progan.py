@@ -67,8 +67,7 @@ class ProgressiveGenerator(nn.Sequential):
         named.append((f"output_{dim}x{dim}", Block(sizes[-1], 3, 1, 0, gain=1)))
         super().__init__(OrderedDict(named))
         self.resolution = dim
-        self._packed = None
-        self._packed_key = None
+        self.pack_cache = _native.Repacked()
 
     def block_names(self):
         return list(self._modules)
@@ -76,12 +75,8 @@ class ProgressiveGenerator(nn.Sequential):
     def packed(self) -> "_native.PackedProGAN":
         """The chain packed for the kernels; re-packed when a parameter changes."""
         mods = list(self._modules.values())
-        key = tuple((p._version, p.data_ptr()) for m in mods for p in (m.conv.weight, m.wscale.b))
-        if self._packed is None or self._packed_key != key:
-            out = mods[-1]
-            self._packed = _native.PackedProGAN([m.describe() for m in mods[:-1]], out.conv.weight, out.wscale.b)
-            self._packed_key = key
-        return self._packed
+        return self.pack_cache.get([p for m in mods for p in (m.conv.weight, m.wscale.b)], lambda: _native.PackedProGAN(
+            [m.describe() for m in mods[:-1]], mods[-1].conv.weight, mods[-1].wscale.b))
 
     def forward(self, x):
         raise NotImplementedError("call ProGAN.forward / partial_forward (models/wrappers.py): they drive the fused chain")

@@ -144,18 +144,12 @@ class G_mapping(nn.Sequential):
         for i in range(8):
             layers += [(f"dense{i}", MyLinear(DLATENT, DLATENT, gain=math.sqrt(2), lrmul=0.01)), (f"dense{i}_act", act)]
         super().__init__(OrderedDict(layers))
-        self._packed = None
-        self._packed_key = None
+        self.pack_cache = _native.Repacked()
 
     def packed(self) -> "_native.PackedMapping":
         lins = [getattr(self, f"dense{i}") for i in range(8)]
-        key = tuple((l.weight._version, l.bias._version, l.weight.data_ptr(), l.bias.data_ptr()) for l in lins)
-        if self._packed is None or self._packed_key != key:
-            w = torch.stack([l.weight.detach() for l in lins])
-            b = torch.stack([l.bias.detach() for l in lins]) / math.sqrt(2)
-            self._packed = _native.PackedMapping(w, b, 0.01)
-            self._packed_key = key
-        return self._packed
+        return self.pack_cache.get([t for l in lins for t in (l.weight, l.bias)], lambda: _native.PackedMapping(
+            torch.stack([l.weight.detach() for l in lins]), torch.stack([l.bias.detach() for l in lins]) / math.sqrt(2), 0.01))
 
     def forward(self, z):
         return self.packed().forward(z, pixelnorm=True)
@@ -178,8 +172,7 @@ class G_synthesis(nn.Module):
         self.torgb = MyConv2d(last, 3, 1, gain=1)
         self.blocks = nn.ModuleDict(OrderedDict(blocks))
         self.resolution = resolution
-        self._packed = None
-        self._packed_key = None
+        self.pack_cache = _native.Repacked()
 
     def forward(self, *a, **k):
         raise NotImplementedError("g_synthesis runs as the fused chain: call StyleGAN.forward / partial_forward")
@@ -201,18 +194,16 @@ class G_synthesis(nn.Module):
         noise = [epi.top_epi.noise.noise for _, epi, _, _ in layers]
         if any(n is None for n in noise):
             raise RuntimeError("StyleGAN: a NoiseLayer has no noise map (StyleGAN.set_noise_seed sets them)")
-        key = tuple((p._version, p.data_ptr()) for p in self.parameters())
-        key += tuple((n._version, n.data_ptr()) for n in noise)
-        if self._packed is None or self._packed_key != key:
+
+        def build():
             inp = self.blocks["4x4"]
             descs = []
             for (conv, epi, up, r), nz in zip(layers, noise):
                 descs.append(dict(conv_weight=None if conv is None else conv.weight, bias=inp.bias if conv is None else conv.bias,
                                   noise=nz, noise_weight=epi.top_epi.noise.weight, style_weight=epi.style_mod.lin.weight,
                                   style_bias=epi.style_mod.lin.bias, upsample=up, res_out=r))
-            self._packed = _native.PackedStyleGAN(descs, inp.const, self.torgb.weight, self.torgb.bias, DLATENT)
-            self._packed_key = key
-        return self._packed
+            return _native.PackedStyleGAN(descs, inp.const, self.torgb.weight, self.torgb.bias, DLATENT)
+        return self.pack_cache.get(list(self.parameters()) + noise, build)
 
 
 class StyleGAN_G(nn.Sequential):

@@ -42,17 +42,14 @@ class EqualLinear(nn.Module):
         self.activation = activation
         self.scale = (1 / math.sqrt(in_dim)) * lr_mul
         self.lr_mul = lr_mul
-        self._packed = None
-        self._packed_key = None
+        self.pack_cache = _native.Repacked()
 
     def forward(self, x):
         if self.activation != "fused_lrelu" or self.weight.shape[0] != self.weight.shape[1]:
             raise NotImplementedError("EqualLinear outside the mapping network is not built yet (SURVEY 8 a5)")
-        key = (self.weight._version, self.bias._version, self.weight.data_ptr())
-        if self._packed is None or self._packed_key != key:
-            self._packed = _native.PackedMapping(self.weight.detach()[None], self.bias.detach()[None], self.lr_mul)
-            self._packed_key = key
-        return self._packed.forward(x, pixelnorm=False)
+        packed = self.pack_cache.get([self.weight, self.bias], lambda: _native.PackedMapping(
+            self.weight.detach()[None], self.bias.detach()[None], self.lr_mul))
+        return packed.forward(x, pixelnorm=False)
 
     def __repr__(self):
         return f"{self.__class__.__name__}({self.weight.shape[1]}, {self.weight.shape[0]})"
@@ -70,18 +67,12 @@ class MappingNetwork(nn.Sequential):
             layers.append(EqualLinear(style_dim, style_dim, lr_mul=lr_mlp, activation="fused_lrelu"))
         super().__init__(*layers)
         self.style_dim, self.n_mlp, self.lr_mlp = style_dim, n_mlp, lr_mlp
-        self._packed = None
-        self._packed_key = None
+        self.pack_cache = _native.Repacked()
 
     def packed(self) -> "_native.PackedMapping":
         lins = list(self)[1:]
-        key = tuple((l.weight._version, l.bias._version, l.weight.data_ptr()) for l in lins)
-        if self._packed is None or self._packed_key != key:
-            w = torch.stack([l.weight.detach() for l in lins])
-            b = torch.stack([l.bias.detach() for l in lins])
-            self._packed = _native.PackedMapping(w, b, self.lr_mlp)
-            self._packed_key = key
-        return self._packed
+        return self.pack_cache.get([t for l in lins for t in (l.weight, l.bias)], lambda: _native.PackedMapping(
+            torch.stack([l.weight.detach() for l in lins]), torch.stack([l.bias.detach() for l in lins]), self.lr_mlp))
 
     def forward(self, z):
         if any(len(m._forward_hooks) or len(m._forward_pre_hooks) for m in self):

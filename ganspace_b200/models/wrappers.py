@@ -92,7 +92,102 @@ class BaseModel(AbstractBaseClass, torch.nn.Module):
         return self.model.named_modules(*args, **kwargs)
 
 
-class StyleGAN2(BaseModel):
+def _checkpoint(relpath) -> Path:
+    return Path(os.environ.get("GANCONTROL_CHECKPOINT_DIR", Path(__file__).parent / "checkpoints")) / relpath
+
+
+class _DeviceGenerator(BaseModel):
+    """What the wrappers of the generators that run on the device (StyleGAN2, StyleGAN, ProGAN, BigGAN) share: where the weights
+    come from, the latent shape, the fixed output class, handing a fused chain's activations to the hooks, and the largest
+    feature map that is decomposed."""
+
+    _latent_shape = (1, 512)
+    MAX_DECOMPOSITION_DIMS = None               # None: no bound
+
+    def _weight_source(self, checkpoint: Path, overrides=()):
+        """The seed of random-init weights, an int: ``random_init=``, else env GANSPACE_B200_RANDOM_INIT (whose value the first
+        set variable of ``overrides`` replaces).  Without a seed, ``checkpoint`` if it is a file; else raises."""
+        seed = self._random_init
+        if seed is None and os.environ.get("GANSPACE_B200_RANDOM_INIT"):
+            seed = next(os.environ[e] for e in (*overrides, "GANSPACE_B200_RANDOM_INIT") if os.environ.get(e))
+        if seed is not None:
+            return int(seed)
+        if checkpoint.is_file():
+            return checkpoint
+        raise RuntimeError(f"{self.model_name} checkpoint {checkpoint} not found and no network access to download it; pass "
+                           "random_init=<seed> (or set GANSPACE_B200_RANDOM_INIT) for random-init weights")
+
+    def get_latent_shape(self):
+        """The reference samples one latent for its shape (wrappers.py:60-61).  The draw from the global NumPy stream that this
+        sample_latent(1) consumes is kept (later seeds depend on it); the kernels behind it are not launched."""
+        _global_seed()
+        return self._latent_shape
+
+    def set_output_class(self, new_class):
+        if self.outclass != new_class:
+            raise RuntimeError(f"{self.model_name}: cannot change output class without reloading")
+
+    def _hand_off(self, module, act, res, channels, downstream, name):
+        """Hands the fused chain's NHWC activation ``act`` of layer ``name`` to the forward hooks of ``module`` as an NCHW view,
+        and returns the view.  A hook that returns another tensor edits the layer.  The chain cannot take an edit back, so when
+        the run goes on past this layer (``downstream``) the edit raises instead of being silently ignored."""
+        view = act.view(-1, res, res, channels).permute(0, 3, 1, 2)
+        if module(_result=view) is not view and downstream:
+            raise NotImplementedError(f"an edit on layer '{name}' cannot be propagated through the fused {self.model_name} chain")
+        return view
+
+    def _nhwc_layout(self, layer_name, res, channels):
+        """``feature_layout`` of a conv layer: ('nhwc', (H, W, C)), the device order of ``activations_into``; the reference's
+        flattening is NCHW -- a fixed permutation, applied once to the exported components."""
+        d = res * res * channels
+        if self.MAX_DECOMPOSITION_DIMS is not None and d > self.MAX_DECOMPOSITION_DIMS:
+            raise NotImplementedError(
+                f"{self.model_name} {layer_name}: d = {d} exceeds {self.MAX_DECOMPOSITION_DIMS}, the largest feature map the large-d "
+                "IPCA engine is run at: its stacked matrix holds (components + batch + 1) rows of d floats in HBM")
+        return ("nhwc", (res, res, channels))
+
+
+class _StyledGenerator(_DeviceGenerator):
+    """A device generator with a mapping network (StyleGAN2, StyleGAN): latents are in Z, or in W after ``use_w``."""
+
+    def latent_space_name(self):
+        return "W" if self.w_primary else "Z"
+
+    def use_w(self):
+        self.w_primary = True
+
+    def use_z(self):
+        self.w_primary = False
+
+    def _draw_z(self, n_samples, seed):
+        return _native.legacy_normal([seed], 512 * n_samples, self.device).view(n_samples, 512)
+
+    def sample_latent(self, n_samples=1, seed=None, truncation=None):
+        z = self._draw_z(n_samples, _global_seed() if seed is None else seed)
+        # a module call: the mapping network's hooks fire here in W mode, as in the reference
+        return self._mapping()(z) if self.w_primary else z
+
+    def draw_z_async(self, n_samples, seed):
+        """The Z stream of ``sample_latent(n_samples, seed=seed)`` generated on a side stream; returns a callable that makes
+        the current stream wait for it and hands back z [n_samples, 512]."""
+        side = getattr(self, "_side_stream", None)
+        if side is None:
+            with torch.cuda.device(self.device):
+                side = self._side_stream = torch.cuda.Stream(device=self.device)
+        with torch.cuda.device(self.device):
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                z = self._draw_z(n_samples, seed)
+
+        def result():
+            with torch.cuda.device(self.device):
+                torch.cuda.current_stream().wait_stream(side)
+            z.record_stream(torch.cuda.current_stream())
+            return z
+        return result
+
+
+class StyleGAN2(_StyledGenerator):
     CONFIGS = {"ffhq": 1024, "car": 512, "cat": 256, "church": 256, "horse": 256,
                "bedrooms": 256, "kitchen": 256, "places": 256}
 
@@ -108,73 +203,27 @@ class StyleGAN2(BaseModel):
         self.name = f"StyleGAN2-{self.outclass}"
         self.has_latent_residual = True
         self._random_init = random_init
+        self._synth, self._synth_keys = _native.Repacked(), ()
         self.load_model()
         self.set_noise_seed(0)
 
-    def latent_space_name(self):
-        return "W" if self.w_primary else "Z"
-
-    def use_w(self):
-        self.w_primary = True
-
-    def use_z(self):
-        self.w_primary = False
-
     def load_model(self):
-        root = os.environ.get("GANCONTROL_CHECKPOINT_DIR", Path(__file__).parent / "checkpoints")
-        checkpoint = Path(root) / f"stylegan2/stylegan2_{self.outclass}_{self.resolution}.pt"
-        seed = self._random_init
-        if seed is None and os.environ.get("GANSPACE_B200_RANDOM_INIT"):
-            seed = int(os.environ["GANSPACE_B200_RANDOM_INIT"])
-        if checkpoint.is_file() and seed is None:
-            self.model = stylegan2.Generator(self.resolution, 512, 8)
-            ckpt = torch.load(checkpoint, map_location="cpu")
-            self.model.load_state_dict(ckpt["g_ema"], strict=False)
-            self.model = self.model.to(self.device)
-            self.latent_avg = ckpt["latent_avg"].to(self.device)
-        elif seed is not None:
+        source = self._weight_source(_checkpoint(f"stylegan2/stylegan2_{self.outclass}_{self.resolution}.pt"))
+        if isinstance(source, int):
             # the reference's default init, bit-for-bit: parameters are created on the host in the
             # reference's order under one manual seed, then moved to the device
-            torch.manual_seed(int(seed))
+            torch.manual_seed(source)
             self.model = stylegan2.Generator(self.resolution, 512, 8).to(self.device)
             self.latent_avg = torch.zeros(512, device=self.device)
         else:
-            raise RuntimeError(
-                f"StyleGAN2 checkpoint {checkpoint} not found and no network access to download it; pass "
-                "random_init=<seed> (or set GANSPACE_B200_RANDOM_INIT) for random-init weights")
+            self.model = stylegan2.Generator(self.resolution, 512, 8)
+            ckpt = torch.load(source, map_location="cpu")
+            self.model.load_state_dict(ckpt["g_ema"], strict=False)
+            self.model = self.model.to(self.device)
+            self.latent_avg = ckpt["latent_avg"].to(self.device)
 
-    def get_latent_shape(self):
-        """The reference samples one latent for its shape (wrappers.py:60-61).  The draw from the global NumPy stream that this
-        sample_latent(1) consumes is kept (later seeds depend on it); the two kernels behind it are not launched."""
-        _global_seed()
-        return (1, 512)
-
-    def sample_latent(self, n_samples=1, seed=None, truncation=None):
-        if seed is None:
-            seed = _global_seed()
-        z = _native.legacy_normal([seed], 512 * n_samples, self.device).view(n_samples, 512)
-        if self.w_primary:
-            z = self.model.style(z)
-        return z
-
-    def draw_z_async(self, n_samples, seed):
-        """The Z stream of ``sample_latent(n_samples, seed=seed)`` generated on a side stream; returns a callable that makes
-        the current stream wait for it and hands back z [n_samples, 512]."""
-        side = getattr(self, "_side_stream", None)
-        if side is None:
-            with torch.cuda.device(self.device):
-                side = self._side_stream = torch.cuda.Stream(device=self.device)
-        with torch.cuda.device(self.device):
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                z = _native.legacy_normal([seed], 512 * n_samples, self.device).view(n_samples, 512)
-
-        def result():
-            with torch.cuda.device(self.device):
-                torch.cuda.current_stream().wait_stream(side)
-            z.record_stream(torch.cuda.current_stream())
-            return z
-        return result
+    def _mapping(self):
+        return self.model.style
 
     def z_to_latent(self, z):
         """What sample_latent does after drawing z (wrappers.py:176-179): the mapping network in W mode."""
@@ -209,11 +258,10 @@ class StyleGAN2(BaseModel):
             g1 = min(S, g0 + sizes[min(len(bounds), len(sizes) - 1)])
             bounds.append((g0, g1))
             g0 = g1
-        sides = getattr(self, "_rng_streams", None)
-        if sides is None:                       # (more than one stream: groups alternate; measured slower -- they crowd out the GEMMs)
+        side = getattr(self, "_rng_stream", None)
+        if side is None:
             with torch.cuda.device(self.device):
-                sides = self._rng_streams = [torch.cuda.Stream(device=self.device)
-                                             for _ in range(max(1, int(os.environ.get("GANSPACE_B200_RNG_STREAMS", "1"))))]
+                side = self._rng_stream = torch.cuda.Stream(device=self.device)
         events = []
         seeds_dev = _native.seeds_tensor(list(seeds), self.device)       # ONE host->device copy, before any long kernel is queued
         # the first group decides when the first partial_fit statistics exist (the merge chain, the critical path of a small-d
@@ -227,23 +275,19 @@ class StyleGAN2(BaseModel):
             gmax = max(b - a for a, b in bounds)
             wsb = _native.load().gsb_legacy_normal_split_workspace_bytes
             need = max(wsb(gmax, 512 * n_samples, parts), wsb(bounds[0][1] - bounds[0][0], 512 * n_samples, parts0))
-            for i, side in enumerate(sides):
-                _native.scratch.get(f"rng_split{i}", need, _native.require_cuda(self.device)).record_stream(side)
+            _native.scratch.get("rng_split_lazy", need, _native.require_cuda(self.device)).record_stream(side)
         with torch.cuda.device(self.device):
-            for side in sides:
-                side.wait_stream(torch.cuda.current_stream())
-            for gi, (a, b) in enumerate(bounds):
-                side = sides[gi % len(sides)]
-                with torch.cuda.stream(side):
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                for gi, (a, b) in enumerate(bounds):
                     _native.legacy_normal(seeds_dev[a:b], 512 * n_samples, self.device,
                                           out=z[a * n_samples:b * n_samples].view(b - a, 512 * n_samples),
-                                          parts=parts0 if gi == 0 else parts, scratch_key=f"rng_split{gi % len(sides)}")
+                                          parts=parts0 if gi == 0 else parts, scratch_key="rng_split_lazy")
                     ev = torch.cuda.Event()
                     ev.record(side)
                     events.append(ev)
-            for side in sides:
-                z.record_stream(side)
-                seeds_dev.record_stream(side)          # read by launches that run long after this function has returned
+            z.record_stream(side)
+            seeds_dev.record_stream(side)          # read by launches that run long after this function has returned
         packed = self.model.style.packed() if self.w_primary else None
         state = {"g": 0, "keep": seeds_dev}
         free_sms = int(os.environ.get("GANSPACE_B200_LAZY_FREE_SMS", 32 if parts > 1 else 48))
@@ -262,15 +306,11 @@ class StyleGAN2(BaseModel):
     def check_numerics(self):
         """Raise if a kernel flagged an out-of-range activation since the weights were packed (synchronises)."""
         self.model.style.packed().check()
-        if getattr(self, "_synth_cache", None) is not None:
-            self._synth_cache[1].check()
+        if self._synth.current() is not None:
+            self._synth.current().check()
 
     def get_max_latents(self):
         return self.model.n_latent
-
-    def set_output_class(self, new_class):
-        if self.outclass != new_class:
-            raise RuntimeError("StyleGAN2: cannot change output class without reloading")
 
     def forward(self, x):
         """wrappers.py:188-192: images in [0, 1] (before clamping) from one latent, a pair, or one latent per layer.  Hooked
@@ -289,55 +329,49 @@ class StyleGAN2(BaseModel):
         each gets its own run of the fused chain up to that layer."""
         mods = [self.model.conv1] + list(self.model.convs)
         rgbs = [self.model.to_rgb1] + list(self.model.to_rgbs)
+        names, rgb_names = self.synthesis_layer_names(), self._rgb_names()
         w_layers = latent.permute(1, 0, 2).contiguous()
         for i in range(target + 1):
             if len(mods[i]._forward_hooks):
                 syn = self._synthesis(i + 1)
-                res, co = syn.shapes[i]
                 act, _ = syn.render(w_layers, i + 1, [], want_act=True)
-                act = act.view(-1, res, res, co).permute(0, 3, 1, 2)                   # NCHW view of NHWC storage
-                if mods[i](_result=act) is not act:
-                    raise NotImplementedError(f"an edit on layer '{self.synthesis_layer_names()[i]}' cannot be propagated through "
-                                              "the fused synthesis chain")
+                self._hand_off(mods[i], act, *syn.shapes[i], True, names[i])
         for j in range(rgb_upto + 1):
             if len(rgbs[j]._forward_hooks):
-                syn = self._synthesis(2 * j + 1)
-                _, img = syn.render(w_layers, 2 * j + 1, [r.describe() for r in rgbs[:j + 1]])
-                img = img.permute(0, 3, 1, 2)
-                if rgbs[j](_result=img) is not img:
-                    raise NotImplementedError("an edit on a ToRGB layer cannot be propagated through the fused synthesis chain")
+                _, img = self._synthesis(2 * j + 1).render(w_layers, 2 * j + 1, [r.describe() for r in rgbs[:j + 1]])
+                self._hand_off(rgbs[j], img, img.shape[1], 3, True, rgb_names[j])
 
     # ---- synthesis chain conv1, convs.0 .. convs.k (wrappers.py:224-255) ------------------------------------
     def synthesis_layer_names(self):
         return ["conv1"] + [f"convs.{i}" for i in range(len(self.model.convs))]
 
+    def _rgb_names(self):
+        return ["to_rgb1"] + [f"to_rgbs.{i}" for i in range(len(self.model.to_rgbs))]
+
     def _synthesis(self, n_run):
-        """PackedSynthesis covering at least the first ``n_run`` StyledConv layers (re-packed when a parameter or a
-        noise map of those layers changes, or when a deeper layer is asked for)."""
+        """PackedSynthesis covering at least the first ``n_run`` StyledConv layers.  A pack of more layers serves as long as the
+        constant and the parameters and noise maps of these ``n_run`` layers are the ones it was packed from."""
         mods = [self.model.conv1] + list(self.model.convs)
-        cst = self.model.input.input
-        keys = [(cst._version, cst.data_ptr())]
-        keys += [(m.conv.weight._version, m.conv.weight.data_ptr(), m.conv.modulation.weight._version,
-                  m.conv.modulation.bias._version, m.noise.weight._version, m.activate.bias._version,
-                  self.noise[i].data_ptr(), self.noise[i]._version) for i, m in enumerate(mods[:n_run])]
-        cached = getattr(self, "_synth_cache", None)
-        if cached is None or len(cached[0]) < len(keys) or cached[0][:len(keys)] != keys:
+        keys = (_native.source_key([self.model.input.input]),) + tuple(
+            _native.source_key([m.conv.weight, m.conv.modulation.weight, m.conv.modulation.bias, m.noise.weight, m.activate.bias,
+                                self.noise[i]]) for i, m in enumerate(mods[:n_run]))
+        if self._synth_keys[:len(keys)] != keys:
+            self._synth_keys = keys               # a stale or too short pack: the get() below packs n_run layers
+
+        def build():
             layers, res = [], 4
             for i, m in enumerate(mods[:n_run]):
                 layers.append(m.describe(self.noise[i], res))
                 res = 2 * res if m.conv.upsample else res
-            packed = _native.PackedSynthesis(cst.detach()[0], layers, self.model.style_dim)
-            self._synth_cache = cached = (keys, packed)
-        return cached[1]
+            return _native.PackedSynthesis(self.model.input.input.detach()[0], layers, self.model.style_dim)
+        return self._synth.get([], build, self._synth_keys)
 
     def feature_layout(self, layer_name):
-        """Native (device) feature order of ``activations_into`` for this layer: ('nhwc', (H, W, C)); the reference's
-        flattening is NCHW -- a fixed permutation, applied once to the exported components."""
         names = self.synthesis_layer_names()
         if layer_name not in names:
             return None
-        res, co = self._synthesis(names.index(layer_name) + 1).shapes[names.index(layer_name)]
-        return ("nhwc", (res, res, co))
+        i = names.index(layer_name)
+        return self._nhwc_layout(layer_name, *self._synthesis(i + 1).shapes[i])
 
     def activations_into(self, x, layer_name, out):
         """Hooked-layer activations of latents x [n,512] (in the current primary space) written as fp32 NHWC rows into
@@ -362,7 +396,7 @@ class StyleGAN2(BaseModel):
             self.model.input(latent[:, 0])
             return
         names = self.synthesis_layer_names()
-        rgb_names = ["to_rgb1"] + [f"to_rgbs.{i}" for i in range(len(self.model.to_rgbs))]
+        rgb_names = self._rgb_names()
         rgb_hooked = any(len(m._forward_hooks) for m in [self.model.to_rgb1] + list(self.model.to_rgbs))
         if layer_name in names and len(styles) == 1 and not rgb_hooked:
             # one global latent, no ToRGB hook: the decomposition's own call pattern -- the single-latent entry point
@@ -371,12 +405,8 @@ class StyleGAN2(BaseModel):
             w = styles[0].reshape(-1, 512)
             for i in [i for i in range(target) if len(mods[i]._forward_hooks)] + [target]:
                 syn = self._synthesis(target + 1)
-                res, co = syn.shapes[i]
-                act = syn.forward(w, i + 1).view(-1, res, res, co).permute(0, 3, 1, 2)    # NCHW view of NHWC storage
-                if mods[i](_result=act) is not act and i < target:
-                    # (an edit on the target layer itself has nothing downstream inside partial_forward)
-                    raise NotImplementedError(f"an edit on layer '{names[i]}' cannot be propagated through the fused synthesis "
-                                              f"chain to '{layer_name}'")
+                # (an edit on the target layer itself has nothing downstream inside partial_forward)
+                self._hand_off(mods[i], syn.forward(w, i + 1), *syn.shapes[i], i < target, names[i])
         elif layer_name in names:
             target = names.index(layer_name)
             # the reference computes every to_rgb that precedes the target as well (wrappers.py:232-255)
@@ -397,7 +427,7 @@ class StyleGAN2(BaseModel):
                 self.noise.append(torch.randn(1, 1, 2 ** i, 2 ** i).to(self.device))
 
 
-class ProGAN(BaseModel):
+class ProGAN(_DeviceGenerator):
     """wrappers.py:469-522 on the fused chain of csrc/progan.cu.  Z space only; hookable layers are the blocks
     ``layer1 .. layer14`` and ``output_256x256``.  Checkpoint: ``$GANCONTROL_CHECKPOINT_DIR/progan/<class>_lsun.pth`` (there is no
     network to download it); without one, ``random_init=<seed>`` (or env GANSPACE_B200_RANDOM_INIT) builds
@@ -420,24 +450,13 @@ class ProGAN(BaseModel):
 
     def load_model(self):
         from . import progan
-        root = os.environ.get("GANCONTROL_CHECKPOINT_DIR", Path(__file__).parent / "checkpoints")
-        checkpoint = Path(root) / f"progan/{self.outclass}_lsun.pth"
-        seed = self._random_init
-        if seed is None and os.environ.get("GANSPACE_B200_RANDOM_INIT"):
-            seed = int(os.environ["GANSPACE_B200_RANDOM_INIT"])
-        if checkpoint.is_file() and seed is None:
-            self.model = progan.from_state_dict(torch.load(checkpoint, map_location="cpu")).to(self.device)
-        elif seed is not None:
-            self.model = progan.random_init(seed).to(self.device)
+        source = self._weight_source(_checkpoint(f"progan/{self.outclass}_lsun.pth"))
+        if isinstance(source, int):
+            self.model = progan.random_init(source).to(self.device)
         else:
-            raise RuntimeError(f"ProGAN checkpoint {checkpoint} not found and no network access to download it; pass "
-                               "random_init=<seed> (or set GANSPACE_B200_RANDOM_INIT) for random-init weights")
+            self.model = progan.from_state_dict(torch.load(source, map_location="cpu")).to(self.device)
         self.z_dim = self.model.layer1.conv.in_channels
-
-    def get_latent_shape(self):
-        """As StyleGAN2.get_latent_shape: the reference's sample_latent(1) consumes one draw of the global NumPy stream."""
-        _global_seed()
-        return (1, self.z_dim, 1, 1)
+        self._latent_shape = (1, self.z_dim, 1, 1)
 
     def sample_latent(self, n_samples=1, seed=None, truncation=None):
         """zdataset.py:26-40: ``RandomState(seed).standard_normal(n * z_dim)`` as float32 [n, z_dim, 1, 1], drawn on the device."""
@@ -451,10 +470,6 @@ class ProGAN(BaseModel):
                                   out=None if out is None else out.view(len(seeds), self.z_dim * n_samples),
                                   parts=_native.split_parts(self.z_dim * n_samples))
         return z.view(len(seeds) * n_samples, self.z_dim, 1, 1)
-
-    def set_output_class(self, new_class):
-        if self.outclass != new_class:
-            raise RuntimeError("ProGAN: cannot change output class without reloading")
 
     def check_numerics(self):
         """Raise if a kernel flagged an out-of-range operand since the weights were packed (synchronises)."""
@@ -476,25 +491,14 @@ class ProGAN(BaseModel):
         packed = self.model.packed()
         n_conv = len(mods) - 1
         last = min(target, n_conv - 1)
-
-        def nchw(act, i):
-            res, co = packed.shapes[i]
-            return act.view(-1, res, res, co).permute(0, 3, 1, 2)                # NCHW view of NHWC storage
-
-        def hand(i, t):
-            if mods[i](_result=t) is not t and i < target:
-                raise NotImplementedError(f"an edit on layer '{names[i]}' cannot be propagated through the fused ProGAN chain")
-
         for i in [i for i in range(last) if len(mods[i]._forward_hooks)]:
-            hand(i, nchw(packed.forward(z, i + 1)[0], i))
+            self._hand_off(mods[i], packed.forward(z, i + 1)[0], *packed.shapes[i], i < target, names[i])
         want_act = len(mods[last]._forward_hooks) > 0 or not want_rgb
         act, rgb = packed.forward(z, last + 1, want_act=want_act, want_rgb=want_rgb)
         if want_act:
-            hand(last, nchw(act, last))
+            self._hand_off(mods[last], act, *packed.shapes[last], last < target, names[last])
         if want_rgb:
-            img = rgb.permute(0, 3, 1, 2)
-            out = mods[n_conv](_result=img)
-            return out
+            return mods[n_conv](_result=rgb.permute(0, 3, 1, 2))
         return None
 
     def forward(self, x):
@@ -508,16 +512,10 @@ class ProGAN(BaseModel):
         self._run(x, target, want_rgb=(target == len(names) - 1))
 
     def feature_layout(self, layer_name):
-        """Device feature order of ``activations_into``: ('nhwc', (H, W, C)) for a conv block."""
         names = self.model.block_names()
         if layer_name not in names[:-1]:
             return None
-        res, co = self.model.packed().shapes[names.index(layer_name)]
-        if res * res * co > self.MAX_DECOMPOSITION_DIMS:
-            raise NotImplementedError(
-                f"ProGAN {layer_name}: d = {res * res * co} exceeds {self.MAX_DECOMPOSITION_DIMS} (layer10), the largest feature map "
-                "the large-d IPCA engine is run at: its stacked matrix holds (components + batch + 1) rows of d floats in HBM")
-        return ("nhwc", (res, res, co))
+        return self._nhwc_layout(layer_name, *self.model.packed().shapes[names.index(layer_name)])
 
     def activations_into(self, x, layer_name, out):
         """Activations of block ``layer_name`` for latents x [n, z_dim(,1,1)] written as fp32 NHWC rows into ``out`` [n, H*W*C]
@@ -526,7 +524,7 @@ class ProGAN(BaseModel):
         return self.model.packed().forward(self._single(x), n_run, out=out)[0]
 
 
-class StyleGAN(BaseModel):
+class StyleGAN(_StyledGenerator):
     """wrappers.py:270-436 (StyleGAN v1).  ``g_mapping`` runs the packed mapping kernels, the synthesis blocks the fused chain of
     csrc/stylegan.cu.  Hookable layers: ``g_mapping`` and the blocks ``g_synthesis.blocks.RxR``.  Checkpoint:
     ``$GANCONTROL_CHECKPOINT_DIR/stylegan/stylegan_<class>_<res>.pt`` (the reference's ``StyleGAN_G`` state dict; there is no network
@@ -552,46 +550,26 @@ class StyleGAN(BaseModel):
         self.load_model()
         self.set_noise_seed(0)
 
-    def latent_space_name(self):
-        return "W" if self.w_primary else "Z"
-
-    def use_w(self):
-        self.w_primary = True
-
-    def use_z(self):
-        self.w_primary = False
-
     def load_model(self):
         from . import stylegan
-        root = os.environ.get("GANCONTROL_CHECKPOINT_DIR", Path(__file__).parent / "checkpoints")
-        checkpoint = Path(root) / f"stylegan/stylegan_{self.outclass}_{self.resolution}.pt"
-        seed = self._random_init
-        if seed is None and os.environ.get("GANSPACE_B200_RANDOM_INIT"):
-            seed = int(os.environ["GANSPACE_B200_RANDOM_INIT"])
-        if checkpoint.is_file() and seed is None:
-            self.model = stylegan.StyleGAN_G(self.resolution)
-            self.model.load_state_dict(torch.load(checkpoint, map_location="cpu"))
-            self.model = self.model.to(self.device)
-        elif seed is not None:
-            self.model = stylegan.random_init(seed, self.resolution).to(self.device)
-        elif checkpoint.with_suffix(".pkl").is_file():
-            raise RuntimeError(f"StyleGAN: {checkpoint.with_suffix('.pkl')} is a TensorFlow checkpoint; converting it needs TensorFlow "
-                               f"(the reference's StyleGAN_G.export_from_tf), which is not part of this package: convert it to {checkpoint}")
+        checkpoint = _checkpoint(f"stylegan/stylegan_{self.outclass}_{self.resolution}.pt")
+        try:
+            source = self._weight_source(checkpoint)
+        except RuntimeError:
+            if checkpoint.with_suffix(".pkl").is_file():
+                raise RuntimeError(f"StyleGAN: {checkpoint.with_suffix('.pkl')} is a TensorFlow checkpoint; converting it needs "
+                                   "TensorFlow (the reference's StyleGAN_G.export_from_tf), which is not part of this package: "
+                                   f"convert it to {checkpoint}") from None
+            raise
+        if isinstance(source, int):
+            self.model = stylegan.random_init(source, self.resolution).to(self.device)
         else:
-            raise RuntimeError(f"StyleGAN checkpoint {checkpoint} not found and no network access to download it; pass "
-                               "random_init=<seed> (or set GANSPACE_B200_RANDOM_INIT) for random-init weights")
-
-    def get_latent_shape(self):
-        """As StyleGAN2.get_latent_shape: the reference's sample_latent(1) consumes one draw of the global NumPy stream."""
-        _global_seed()
-        return (1, 512)
+            self.model = stylegan.StyleGAN_G(self.resolution)
+            self.model.load_state_dict(torch.load(source, map_location="cpu"))
+            self.model = self.model.to(self.device)
 
     def get_max_latents(self):
         return 18
-
-    def set_output_class(self, new_class):
-        if self.outclass != new_class:
-            raise RuntimeError("StyleGAN: cannot change output class without reloading")
 
     def set_noise_seed(self, seed):
         """wrappers.py:419-434: every NoiseLayer gets ``torch.randn(1, 1, H, W)`` right after ``manual_seed(seed)`` (so all maps of
@@ -603,17 +581,8 @@ class StyleGAN(BaseModel):
                 m.noise = torch.randn(1, 1, H, W, dtype=torch.float32).to(self.device)
 
     # ---- latents ----------------------------------------------------------------------------------------
-    def sample_latent(self, n_samples=1, seed=None, truncation=None):
-        if seed is None:
-            seed = _global_seed()
-        z = _native.legacy_normal([seed], 512 * n_samples, self.device).view(n_samples, 512)
-        if self.w_primary:
-            z = self.model.g_mapping(z)            # a module call: the g_mapping hook fires here in W mode, as in the reference
-        return z
-
-    def draw_z_async(self, n_samples, seed):
-        """The Z stream of ``sample_latent(n_samples, seed=seed)`` generated on a side stream (StyleGAN2.draw_z_async)."""
-        return StyleGAN2.draw_z_async(self, n_samples, seed)
+    def _mapping(self):
+        return self.model.g_mapping
 
     def z_to_latent(self, z):
         return self.model.g_mapping.packed().forward(z) if self.w_primary else z
@@ -640,8 +609,8 @@ class StyleGAN(BaseModel):
     def check_numerics(self):
         """Raise if a kernel flagged an out-of-range operand since the weights were packed (synchronises)."""
         self.model.g_mapping.packed().check()
-        if self.model.g_synthesis._packed is not None:
-            self.model.g_synthesis._packed.check()
+        if self.model.g_synthesis.pack_cache.current() is not None:
+            self.model.g_synthesis.pack_cache.current().check()
 
     # ---- synthesis ----------------------------------------------------------------------------------------
     def _hookable(self):
@@ -670,13 +639,7 @@ class StyleGAN(BaseModel):
         blocks = list(self.model.g_synthesis.blocks.values())
         names = self.model.block_names()
         w_layers = w_layers[:2 * (target + 1)] if w_layers.shape[0] > 1 else w_layers
-
-        def hand(i, act):
-            res, co = packed.shapes[2 * i + 1]
-            t = act.view(-1, res, res, co).permute(0, 3, 1, 2)                       # NCHW view of NHWC storage
-            if blocks[i](_result=t) is not t and (i < target or want_rgb):
-                raise NotImplementedError(f"an edit on layer '{names[i]}' cannot be propagated through the fused StyleGAN chain")
-
+        hand = lambda i, act: self._hand_off(blocks[i], act, *packed.shapes[2 * i + 1], i < target or want_rgb, names[i])
         for i in [i for i in range(target) if len(blocks[i]._forward_hooks)]:
             hand(i, packed.forward(w_layers[:2 * (i + 1)] if w_layers.shape[0] > 1 else w_layers, 2 * (i + 1))[0])
         want_act = len(blocks[target]._forward_hooks) > 0
@@ -714,16 +677,10 @@ class StyleGAN(BaseModel):
         self._run(w_layers, self._target_block(layer_name), False)
 
     def feature_layout(self, layer_name):
-        """Device feature order of ``activations_into``: ('nhwc', (H, W, C)) for a synthesis block."""
         names = self.model.block_names()
         if layer_name not in names:
             return None
-        res, co = self.model.g_synthesis.packed().shapes[2 * names.index(layer_name) + 1]
-        if res * res * co > self.MAX_DECOMPOSITION_DIMS:
-            raise NotImplementedError(
-                f"StyleGAN {layer_name}: d = {res * res * co} exceeds {self.MAX_DECOMPOSITION_DIMS} (blocks.32x32), the largest feature map "
-                "the large-d IPCA engine is run at: its stacked matrix holds (components + batch + 1) rows of d floats in HBM")
-        return ("nhwc", (res, res, co))
+        return self._nhwc_layout(layer_name, *self.model.g_synthesis.packed().shapes[2 * names.index(layer_name) + 1])
 
     def activations_into(self, x, layer_name, out):
         """Output of block ``layer_name`` for latents x [n, 512] (in the current primary space) written as fp32 NHWC rows into
