@@ -97,6 +97,9 @@ SIGNATURES = {
     "gsb_fbpca_workspace_bytes": (_Z, [_I, _I, _I]),
     "gsb_fbpca_solve": (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _Z, _P]),
     "gsb_fbpca_status": (_I, [_P, _I, _P, _P]),
+    "gsb_synthesis_styles": (_I, [_P, _P, _I, _I, _P, _I, _P, _I, _L, _P, _P, _P, _Z, _P]),
+    "gsb_synthesis_render_styled_workspace_bytes": (_Z, [_P, _I, _L]),
+    "gsb_synthesis_render_styled": (_I, [_P, _P, _I, _I, _I, _P, _I, _P, _P, _L, _P, _L, _P, _P, _Z, _P]),
 }
 
 
@@ -851,25 +854,10 @@ class PackedSynthesis(_PackedTapGenerator):
         to_rgbs.0, ... up to the one that follows layer n_run-1 or earlier.  Returns (activation of layer n_run-1 as fp32 NHWC
         rows or None, skip image after the last ToRGB as fp32 NHWC [n, res, res, 3] or None)."""
         lib = load()
-        assert w_layers.is_cuda and w_layers.dtype == torch.float32 and w_layers.dim() == 3 and w_layers.shape[2] == self.style_dim
-        w_layers = w_layers.contiguous()
+        w_layers = self._latents(w_layers)
         Lw, n = int(w_layers.shape[0]), int(w_layers.shape[1])
-        keep = []
-        descs = (ToRGBDesc * max(1, len(rgbs)))()
-        for j, r in enumerate(rgbs):
-            ts = {k: r[k].detach().to(self.device, torch.float32).contiguous() for k in ("conv_weight", "mod_weight", "mod_bias", "bias")}
-            keep.append(ts)
-            cin = ts["conv_weight"].shape[-1]
-            assert ts["conv_weight"].numel() == 3 * cin and ts["bias"].numel() == 3
-            for k, t in ts.items():
-                setattr(descs[j], k, t.data_ptr())
-            descs[j].cin = int(cin)
-        act = rgb = None
-        if want_act:
-            act = torch.empty((n, self.out_dims(n_run)), dtype=torch.float32, device=self.device)
-        if rgbs:
-            res = self.shapes[2 * (len(rgbs) - 1)][0]
-            rgb = torch.empty((n, res, res, 3), dtype=torch.float32, device=self.device)
+        descs, keep = self._rgb_descs(rgbs)
+        act, rgb = self._render_outputs(n, n_run, len(rgbs), want_act)
         ws_bytes = lib.gsb_synthesis_render_workspace_bytes(self.desc, n_run, n, self.style_dim)
         ws = scratch.get("synthesis", ws_bytes, self.device)
         with torch.cuda.device(self.device), instrument.section("synthesis"):
@@ -880,6 +868,92 @@ class PackedSynthesis(_PackedTapGenerator):
                 torch.cuda.current_stream().synchronize()      # the temporary parameter copies may be freed after this
         instrument.count(1)
         instrument.add_rows("synthesis", n)
+        return act, rgb
+
+    def styles(self, w_layers: torch.Tensor, conv_idx, rgb_idx=(), rgbs=()):
+        """The style-space rows (gsb_synthesis_styles): for per-layer latents ``w_layers`` [Lw, n, style_dim] (entries as in
+        ``render``), the modulation output [n, cin] of every chain layer in ``conv_idx`` and of every ToRGB in ``rgb_idx`` (0 =
+        to_rgb1, j + 1 = to_rgbs.j; ``rgbs`` describes ToRGBs 0 .. max(rgb_idx) as in ``render``).  Returns ({layer: rows},
+        {ToRGB: rows}).  The launches are the chain's own style stage, so at the same n the rows are the ones it consumes."""
+        lib = load()
+        w_layers = self._latents(w_layers)
+        Lw, n = int(w_layers.shape[0]), int(w_layers.shape[1])
+        conv_idx, rgb_idx = sorted(set(conv_idx)), sorted(set(rgb_idx))
+        assert all(0 <= l < self.n_layers for l in conv_idx) and all(0 <= j < len(rgbs) for j in rgb_idx)
+        new = lambda c: torch.empty((n, c), dtype=torch.float32, device=self.device)
+        S = {l: new(self.desc[l].cin) for l in conv_idx}
+        R = {j: new(self.desc[2 * j].cout) for j in rgb_idx}
+        S_ptrs = (C.c_void_p * self.n_layers)(*[S[l].data_ptr() if l in S else None for l in range(self.n_layers)])
+        n_rgb = rgb_idx[-1] + 1 if rgb_idx else 0
+        R_ptrs = (C.c_void_p * max(1, n_rgb))(*[R[j].data_ptr() if j in R else None for j in range(n_rgb)])
+        descs, keep = self._rgb_descs(list(rgbs)[:n_rgb])
+        ws = scratch.get("synthesis_styles", max([self.desc[2 * j].cout for j in rgb_idx], default=0) * self.style_dim * 4,
+                         self.device)
+        with torch.cuda.device(self.device), instrument.section("styles"):
+            _check(lib.gsb_synthesis_styles(_ptr(self.packed), self.desc, self.n_layers, self.style_dim, descs, n_rgb, _ptr(w_layers),
+                                            Lw, n, S_ptrs, R_ptrs, _ptr(ws), ws.numel(), _stream()), "gsb_synthesis_styles")
+            if keep:
+                torch.cuda.current_stream().synchronize()
+        instrument.count(len(conv_idx) + 2 * len(rgb_idx))
+        instrument.add_rows("styles", n)
+        return S, R
+
+    def render_styled(self, S, rgb_S, n_run: int, rgbs, want_act: bool = False):
+        """``render`` on caller-given styles (gsb_synthesis_render_styled): ``S[l]`` [n, cin] for the chain layers 0 .. n_run-1 and
+        ``rgb_S[j]`` [n, cin] for every ToRGB in ``rgbs`` (only their conv_weight and bias are read).  Same outputs as ``render``."""
+        lib = load()
+        S = [self._style_rows(t, self.desc[l].cin) for l, t in enumerate(S[:n_run])]
+        assert len(S) == n_run and len(rgb_S) == len(rgbs)
+        n = S[0].shape[0]
+        rgb_S = [self._style_rows(t, self.desc[2 * j].cout) for j, t in enumerate(rgb_S)]
+        assert all(t.shape[0] == n for t in S + rgb_S), "every style needs the same number of rows"
+        descs, keep = self._rgb_descs(rgbs)
+        act, rgb = self._render_outputs(n, n_run, len(rgbs), want_act)
+        S_ptrs = (C.c_void_p * n_run)(*[t.data_ptr() for t in S])
+        R_ptrs = (C.c_void_p * max(1, len(rgb_S)))(*[t.data_ptr() for t in rgb_S])
+        ws_bytes = lib.gsb_synthesis_render_styled_workspace_bytes(self.desc, n_run, n)
+        ws = scratch.get("synthesis", ws_bytes, self.device)
+        with torch.cuda.device(self.device), instrument.section("synthesis"):
+            _check(lib.gsb_synthesis_render_styled(_ptr(self.packed), self.desc, self.n_layers, n_run, self.style_dim, descs, len(rgbs),
+                                                   S_ptrs, R_ptrs, n, _ptr(act), act.stride(0) if act is not None else 0, _ptr(rgb),
+                                                   _ptr(ws), ws.numel(), _stream()), "gsb_synthesis_render_styled")
+            if keep:
+                torch.cuda.current_stream().synchronize()
+        instrument.count(1)
+        instrument.add_rows("synthesis", n)
+        return act, rgb
+
+    def _latents(self, w_layers):
+        assert w_layers.is_cuda and w_layers.dtype == torch.float32 and w_layers.dim() == 3 and w_layers.shape[2] == self.style_dim
+        return w_layers.contiguous()
+
+    def _style_rows(self, t, width):
+        assert t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and t.shape[1] == width, \
+            f"style rows [n, {width}] fp32 on the device expected, got {tuple(t.shape)} {t.dtype}"
+        return t.contiguous()
+
+    def _rgb_descs(self, rgbs):
+        """(ToRGBDesc array, the fp32 device copies it points to) for the ToRGB dicts ``rgbs``; parameters that already are
+        contiguous fp32 device tensors are used in place."""
+        keep = []
+        descs = (ToRGBDesc * max(1, len(rgbs)))()
+        for j, r in enumerate(rgbs):
+            ts = {k: r[k].detach().to(self.device, torch.float32).contiguous() for k in ("conv_weight", "mod_weight", "mod_bias", "bias")}
+            keep += [t for k, t in ts.items() if t.data_ptr() != r[k].data_ptr()]
+            cin = ts["conv_weight"].shape[-1]
+            assert ts["conv_weight"].numel() == 3 * cin and ts["bias"].numel() == 3
+            for k, t in ts.items():
+                setattr(descs[j], k, t.data_ptr())
+            descs[j].cin = int(cin)
+        return descs, keep
+
+    def _render_outputs(self, n, n_run, n_rgb, want_act):
+        act = rgb = None
+        if want_act:
+            act = torch.empty((n, self.out_dims(n_run)), dtype=torch.float32, device=self.device)
+        if n_rgb:
+            res = self.shapes[2 * (n_rgb - 1)][0]
+            rgb = torch.empty((n, res, res, 3), dtype=torch.float32, device=self.device)
         return act, rgb
 
     def _status(self, flags):

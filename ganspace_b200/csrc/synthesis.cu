@@ -310,20 +310,25 @@ sy_blur_epilogue_kernel(const float *__restrict__ T, int64_t nb, int H2, int W2,
 }
 
 // ---- workspace --------------------------------------------------------------------------------------------
+constexpr int SY_MAX_RGB = SY_MAX_LAYERS / 2 + 1;
 struct SynthWs {
     float *S[SY_MAX_LAYERS], *D[SY_MAX_LAYERS];
     float *s2;
     __half *act[2][2];     // [ping-pong][hi/lo]
     float *Y, *T;
     unsigned *queue;        // tile queue of the tap GEMM launches
-    float *rgb[2], *rgb_s, *rgb_modw;      // render path: skip images (ping-pong), ToRGB style, scaled modulation weight
+    float *rgb[2];          // render path: skip images (ping-pong)
+    float *rgb_s[SY_MAX_RGB], *rgb_modw;   // with the style stage: ToRGB styles, scaled ToRGB modulation weight
     size_t bytes;
 };
 static int chunk_samples(const gsb_styled_conv &c) {
     int spc = SY_CHUNK_ROWS / (c.res_in * c.res_in);
     return spc < 1 ? 1 : spc;
 }
-static SynthWs synth_ws(void *base, const gsb_styled_conv *layers, int n_run, int64_t n, bool with_rgb = false, int style_dim = 0) {
+// own_styles: the workspace also holds the styles S[l] (and, with_rgb, those of the ToRGBs that can follow layers[0..n_run)) that
+// the style stage writes; without it the caller passes them (gsb_synthesis_render_styled)
+static SynthWs synth_ws(void *base, const gsb_styled_conv *layers, int n_run, int64_t n, bool with_rgb = false, int style_dim = 0,
+                        bool own_styles = true) {
     SynthWs w;
     char *p = reinterpret_cast<char *>(base);
     size_t off = 0;
@@ -331,7 +336,7 @@ static SynthWs synth_ws(void *base, const gsb_styled_conv *layers, int n_run, in
     size_t cmax = 0, act_elems = 0, y_elems = 0, t_elems = 0;
     for (int l = 0; l < n_run; ++l) {
         const gsb_styled_conv &c = layers[l];
-        w.S[l] = (float *)take((size_t)n * c.cin * 4);
+        w.S[l] = own_styles ? (float *)take((size_t)n * c.cin * 4) : nullptr;
         w.D[l] = (float *)take((size_t)n * c.cout * 4);
         cmax = cmax > (size_t)c.cin ? cmax : (size_t)c.cin;
         const size_t in_elems = (size_t)n * c.res_in * c.res_in * c.cin;
@@ -350,18 +355,50 @@ static SynthWs synth_ws(void *base, const gsb_styled_conv *layers, int n_run, in
     w.Y = (float *)take(y_elems * 4);
     w.T = (float *)take((t_elems ? t_elems : 64) * 4);
     w.queue = (unsigned *)take(sizeof(unsigned));
-    w.rgb[0] = w.rgb[1] = w.rgb_s = w.rgb_modw = nullptr;
+    w.rgb[0] = w.rgb[1] = w.rgb_modw = nullptr;
+    for (int j = 0; j < SY_MAX_RGB; ++j) w.rgb_s[j] = nullptr;
     if (with_rgb) {
         const int ro = res_out_of(layers[n_run - 1]);
-        size_t cm = 0;
-        for (int l = 0; l < n_run; ++l) cm = cm > (size_t)layers[l].cout ? cm : (size_t)layers[l].cout;
         for (int a = 0; a < 2; ++a) w.rgb[a] = (float *)take((size_t)n * ro * ro * 3 * 4);
-        w.rgb_s = (float *)take((size_t)n * cm * 4);
-        w.rgb_modw = (float *)take(cm * (size_t)style_dim * 4);
+        if (own_styles) {
+            size_t cm = 0;
+            for (int j = 0; 2 * j < n_run; ++j) {
+                w.rgb_s[j] = (float *)take((size_t)n * layers[2 * j].cout * 4);
+                cm = cm > (size_t)layers[2 * j].cout ? cm : (size_t)layers[2 * j].cout;
+            }
+            w.rgb_modw = (float *)take(cm * (size_t)style_dim * 4);
+        }
     }
     w.bytes = off;
     return w;
 }
+
+// ---- style stage (model.py:226,234) ----------------------------------------------------------------------
+// StyledConv layer l: s = w modw^T + modb with the modulation weight scaled at pack time
+static int conv_style(const SynthView &v, const gsb_styled_conv &c, int l, const float *w, int64_t n, int style_dim, float *s,
+                      gsb_stream_t stream) {
+    return sy_linear(w, v.L[l].modw, v.L[l].modb, s, n, c.cin, style_dim, stream);
+}
+// ToRGB: the modulation weight is scaled per call into modw (cin * style_dim floats)
+static int rgb_style(const gsb_to_rgb &t, const float *w, int64_t n, int style_dim, float *modw, float *s, gsb_stream_t stream) {
+    const float mscale = (float)(1.0 / sqrt((double)style_dim));
+    scale_copy_kernel<<<64, 256, 0, (cudaStream_t)stream>>>(t.mod_weight, (int64_t)t.cin * style_dim, mscale, nullptr, modw);
+    GSB_CHECK_LAUNCH();
+    return sy_linear(w, modw, t.mod_bias, s, n, t.cin, style_dim, stream);
+}
+// rgbs[j] follows layer 2j of layers[0..n_following); need_mod: its modulation parameters are read
+static int check_rgbs(const gsb_styled_conv *layers, int n_following, const gsb_to_rgb *rgbs, int n_rgb, bool need_mod) {
+    GSB_CHECK_ARG(n_rgb >= 0 && n_rgb <= SY_MAX_RGB && (n_rgb == 0 || rgbs), "synthesis: bad ToRGB list");
+    for (int j = 0; j < n_rgb; ++j) {
+        const gsb_to_rgb &t = rgbs[j];
+        GSB_CHECK_ARG(2 * j < n_following, "synthesis: ToRGB %d has no layer %d to follow", j, 2 * j);
+        const int c = layers[2 * j].cout;
+        GSB_CHECK_ARG(t.conv_weight && t.bias && (!need_mod || (t.mod_weight && t.mod_bias)) && t.cin == c && (c & (c - 1)) == 0,
+                      "synthesis: ToRGB %d does not match layer %d (cin=%d, cout=%d)", j, 2 * j, t.cin, c);
+    }
+    return GSB_OK;
+}
+static bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 }  // namespace gsb
 
@@ -410,31 +447,17 @@ extern "C" size_t gsb_synthesis_workspace_bytes(const gsb_styled_conv *layers, i
 
 namespace gsb {
 
-// layers[0 .. n_run) on per-layer latents d_w [w_layers][n][style_dim] (layer l reads entry min(l, w_layers - 1)); optional fp32
-// activation of the last layer (d_out), optional ToRGB chain: rgbs[j] follows layer 2j and reads latent entry 2j + 1.
+// run stage: layers[0 .. n_run) on the styles S[l] [n, cin_l]; optional fp32 activation of the last layer (d_out), optional ToRGB
+// chain: rgbs[j] follows layer 2j with style rgb_s[j] [n, cin_j].  The demodulation factors are derived from S here (model.py:239).
 static int synthesis_run(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int n_run, int style_dim,
-                         const gsb_to_rgb *rgbs, int n_rgb, const float *d_w, int w_layers, int64_t n, float *d_out, int64_t ld_out,
-                         float *d_rgb_out, void *d_workspace, size_t workspace_bytes, gsb_stream_t stream) {
-    if (int r = check_layers(layers, n_layers, style_dim)) return r;
-    GSB_CHECK_ARG(d_packed && d_w && d_workspace && (d_out || d_rgb_out), "synthesis: null pointer");
-    GSB_CHECK_ARG(n_run >= 1 && n_run <= n_layers && w_layers >= 1, "synthesis: n_run / w_layers out of range");
-    GSB_CHECK_ARG(n_rgb >= 0 && (n_rgb == 0 || (rgbs && d_rgb_out && 2 * (n_rgb - 1) <= n_run - 1)), "synthesis: bad ToRGB list");
-    if (n == 0) return GSB_OK;
-    const gsb_styled_conv &last = layers[n_run - 1];
-    const int ro_last = res_out_of(last);
-    GSB_CHECK_ARG(n > 0 && (!d_out || (ld_out >= (int64_t)ro_last * ro_last * last.cout && ld_out % 4 == 0)), "synthesis: bad n / ld_out");
-    SynthView v = synth_view(const_cast<void *>(d_packed), layers, n_layers, style_dim);
-    SynthWs w = synth_ws(d_workspace, layers, n_run, n, n_rgb > 0, style_dim);
-    if (workspace_bytes < w.bytes) { set_error("synthesis: workspace too small (%zu < %zu)", workspace_bytes, w.bytes); return GSB_ERR_WORKSPACE; }
+                         const gsb_to_rgb *rgbs, int n_rgb, const float *const *S, const float *const *rgb_s, int64_t n, float *d_out,
+                         int64_t ld_out, float *d_rgb_out, const SynthWs &w, gsb_stream_t stream) {
+    const SynthView v = synth_view(const_cast<void *>(d_packed), layers, n_layers, style_dim);
     cudaStream_t st = (cudaStream_t)stream;
-    auto latent = [&](int idx) { return d_w + (size_t)(idx < w_layers ? idx : w_layers - 1) * n * style_dim; };
-
-    // styles and demodulation factors of every layer that runs (model.py:234,239)
     for (int l = 0; l < n_run; ++l) {
         const gsb_styled_conv &c = layers[l];
-        if (int r = sy_linear(latent(l), v.L[l].modw, v.L[l].modb, w.S[l], n, c.cin, style_dim, stream)) return r;
         const int64_t cnt = n * c.cin;
-        sy_square_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, st>>>(w.S[l], cnt, w.s2);
+        sy_square_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, st>>>(S[l], cnt, w.s2);
         GSB_CHECK_LAUNCH();
         if (int r = sy_linear(w.s2, v.L[l].wsq, v.zeros, w.D[l], n, c.cout, c.cin, stream)) return r;
         const int64_t cnt2 = n * c.cout;
@@ -443,7 +466,7 @@ static int synthesis_run(const void *d_packed, const gsb_styled_conv *layers, in
     }
     {   // ConstantInput * style of conv1
         const int64_t total = n * 16 * (layers[0].cin / 4);
-        sy_const_modulate_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(v.const_nhwc, w.S[0], n, 16, layers[0].cin, w.act[0][0],
+        sy_const_modulate_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(v.const_nhwc, S[0], n, 16, layers[0].cin, w.act[0][0],
                                                                                 w.act[0][1], v.overflow);
         GSB_CHECK_LAUNCH();
     }
@@ -459,16 +482,9 @@ static int synthesis_run(const void *d_packed, const gsb_styled_conv *layers, in
         const bool with_rgb = (l % 2 == 0) && j < n_rgb;
         float *rgb_cur = nullptr;
         if (with_rgb) {
-            const gsb_to_rgb &t = rgbs[j];
-            GSB_CHECK_ARG(t.conv_weight && t.mod_weight && t.mod_bias && t.bias && t.cin == c.cout && (c.cout & (c.cout - 1)) == 0,
-                          "synthesis: ToRGB %d does not match layer %d (cin=%d, cout=%d)", j, l, t.cin, c.cout);
             rgb_cur = (j == n_rgb - 1) ? d_rgb_out : w.rgb[j & 1];
-            const float mscale = (float)(1.0 / sqrt((double)style_dim));
-            scale_copy_kernel<<<64, 256, 0, st>>>(t.mod_weight, (int64_t)c.cout * style_dim, mscale, nullptr, w.rgb_modw);
-            GSB_CHECK_LAUNCH();
-            if (int r = sy_linear(latent(2 * j + 1), w.rgb_modw, t.mod_bias, w.rgb_s, n, c.cout, style_dim, stream)) return r;
             const int64_t tot = n * hw_out;
-            sy_rgb_init_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(t.bias, rgb_prev, n, ro, rgb_cur);
+            sy_rgb_init_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(rgbs[j].bias, rgb_prev, n, ro, rgb_cur);
             GSB_CHECK_LAUNCH();
         }
         for (int64_t b0 = 0; b0 < n; b0 += spc) {
@@ -480,14 +496,14 @@ static int synthesis_run(const void *d_packed, const gsb_styled_conv *layers, in
             e.demod = w.D[l] + b0 * c.cout;
             e.noise = v.L[l].noise;
             e.bias = v.L[l].actb;
-            e.s_next = hooked ? nullptr : w.S[l + 1] + b0 * c.cout;
+            e.s_next = hooked ? nullptr : S[l + 1] + b0 * c.cout;
             e.out_hi = hooked ? nullptr : w.act[dst][0] + b0 * hw_out * c.cout;
             e.out_lo = hooked ? nullptr : w.act[dst][1] + b0 * hw_out * c.cout;
             e.out_f32 = (hooked && d_out) ? d_out + b0 * ld_out : nullptr;
             e.ld = ld_out;
             e.overflow = v.overflow;
             e.rgb_w = with_rgb ? rgbs[j].conv_weight : nullptr;
-            e.rgb_s = with_rgb ? w.rgb_s + b0 * c.cout : nullptr;
+            e.rgb_s = with_rgb ? rgb_s[j] + b0 * c.cout : nullptr;
             e.rgb_out = with_rgb ? rgb_cur + b0 * hw_out * 3 : nullptr;
             e.rgb_scale = (float)(1.0 / sqrt((double)c.cout));
             const int cq = c.cout / 4;
@@ -509,14 +525,51 @@ static int synthesis_run(const void *d_packed, const gsb_styled_conv *layers, in
     return GSB_OK;
 }
 
+// argument checks shared by the three chain entries; *w receives the workspace layout
+static int check_run(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int n_run, int style_dim, const gsb_to_rgb *rgbs,
+                     int n_rgb, bool need_mod, int64_t n, float *d_out, int64_t ld_out, float *d_rgb_out, void *d_workspace,
+                     size_t workspace_bytes, bool own_styles, SynthWs *w) {
+    if (int r = check_layers(layers, n_layers, style_dim)) return r;
+    GSB_CHECK_ARG(d_packed && d_workspace && (d_out || d_rgb_out), "synthesis: null pointer");
+    GSB_CHECK_ARG(n_run >= 1 && n_run <= n_layers, "synthesis: n_run out of range");
+    if (int r = check_rgbs(layers, n_run, rgbs, n_rgb, need_mod)) return r;
+    GSB_CHECK_ARG(n_rgb == 0 || d_rgb_out, "synthesis: ToRGB list without an image output");
+    GSB_CHECK_ARG(n >= 0, "synthesis: bad n");
+    if (n == 0) return GSB_OK;
+    const gsb_styled_conv &last = layers[n_run - 1];
+    const int ro_last = res_out_of(last);
+    GSB_CHECK_ARG(!d_out || (ld_out >= (int64_t)ro_last * ro_last * last.cout && ld_out % 4 == 0), "synthesis: bad n / ld_out");
+    *w = synth_ws(d_workspace, layers, n_run, n, n_rgb > 0, style_dim, own_styles);
+    if (workspace_bytes < w->bytes) { set_error("synthesis: workspace too small (%zu < %zu)", workspace_bytes, w->bytes); return GSB_ERR_WORKSPACE; }
+    return GSB_OK;
+}
+
+// style stage into the workspace, then the run stage (gsb_synthesis_forward / gsb_synthesis_render)
+static int synthesis_latents(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int n_run, int style_dim,
+                             const gsb_to_rgb *rgbs, int n_rgb, const float *d_w, int w_layers, int64_t n, float *d_out, int64_t ld_out,
+                             float *d_rgb_out, void *d_workspace, size_t workspace_bytes, gsb_stream_t stream) {
+    GSB_CHECK_ARG(d_w && w_layers >= 1, "synthesis: no latents");
+    SynthWs w;
+    if (int r = check_run(d_packed, layers, n_layers, n_run, style_dim, rgbs, n_rgb, true, n, d_out, ld_out, d_rgb_out, d_workspace,
+                          workspace_bytes, true, &w)) return r;
+    if (n == 0) return GSB_OK;
+    const SynthView v = synth_view(const_cast<void *>(d_packed), layers, n_layers, style_dim);
+    auto latent = [&](int idx) { return d_w + (size_t)(idx < w_layers ? idx : w_layers - 1) * n * style_dim; };
+    for (int l = 0; l < n_run; ++l)
+        if (int r = conv_style(v, layers[l], l, latent(l), n, style_dim, w.S[l], stream)) return r;
+    for (int j = 0; j < n_rgb; ++j)
+        if (int r = rgb_style(rgbs[j], latent(2 * j + 1), n, style_dim, w.rgb_modw, w.rgb_s[j], stream)) return r;
+    return synthesis_run(d_packed, layers, n_layers, n_run, style_dim, rgbs, n_rgb, w.S, w.rgb_s, n, d_out, ld_out, d_rgb_out, w, stream);
+}
+
 }  // namespace gsb
 
 extern "C" int gsb_synthesis_forward(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int n_run, int style_dim,
                                      const float *d_w, int64_t n, float *d_out, int64_t ld_out, void *d_workspace,
                                      size_t workspace_bytes, gsb_stream_t stream) {
     GSB_CHECK_ARG(d_out, "synthesis_forward: null output");
-    return gsb::synthesis_run(d_packed, layers, n_layers, n_run, style_dim, nullptr, 0, d_w, 1, n, d_out, ld_out, nullptr, d_workspace,
-                              workspace_bytes, stream);
+    return gsb::synthesis_latents(d_packed, layers, n_layers, n_run, style_dim, nullptr, 0, d_w, 1, n, d_out, ld_out, nullptr, d_workspace,
+                                  workspace_bytes, stream);
 }
 
 extern "C" size_t gsb_synthesis_render_workspace_bytes(const gsb_styled_conv *layers, int n_run, int64_t n, int style_dim) {
@@ -528,8 +581,58 @@ extern "C" size_t gsb_synthesis_render_workspace_bytes(const gsb_styled_conv *la
 extern "C" int gsb_synthesis_render(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int n_run, int style_dim,
                                     const gsb_to_rgb *rgbs, int n_rgb, const float *d_w, int w_layers, int64_t n, float *d_act_out,
                                     int64_t ld_act, float *d_rgb_out, void *d_workspace, size_t workspace_bytes, gsb_stream_t stream) {
-    return gsb::synthesis_run(d_packed, layers, n_layers, n_run, style_dim, rgbs, n_rgb, d_w, w_layers, n, d_act_out, ld_act, d_rgb_out,
-                              d_workspace, workspace_bytes, stream);
+    return gsb::synthesis_latents(d_packed, layers, n_layers, n_run, style_dim, rgbs, n_rgb, d_w, w_layers, n, d_act_out, ld_act,
+                                  d_rgb_out, d_workspace, workspace_bytes, stream);
+}
+
+extern "C" int gsb_synthesis_styles(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int style_dim,
+                                    const gsb_to_rgb *rgbs, int n_rgb, const float *d_w, int w_layers, int64_t n, float *const *d_S,
+                                    float *const *d_rgb_s, void *d_workspace, size_t workspace_bytes, gsb_stream_t stream) {
+    using namespace gsb;
+    if (int r = check_layers(layers, n_layers, style_dim)) return r;
+    GSB_CHECK_ARG(d_packed && d_w && w_layers >= 1 && n >= 0, "synthesis_styles: null pointer or bad n");
+    GSB_CHECK_ARG(n_rgb == 0 || d_rgb_s, "synthesis_styles: ToRGB list without outputs");
+    size_t need = 0;
+    for (int j = 0; j < n_rgb; ++j) {
+        if (!d_rgb_s[j]) continue;
+        if (int r = check_rgbs(layers, n_layers, rgbs, j + 1, true)) return r;
+        need = need > (size_t)rgbs[j].cin * style_dim * 4 ? need : (size_t)rgbs[j].cin * style_dim * 4;
+    }
+    GSB_CHECK_ARG(need == 0 || (d_workspace && workspace_bytes >= need), "synthesis_styles: workspace too small (%zu < %zu)",
+                  workspace_bytes, need);
+    if (n == 0) return GSB_OK;
+    const SynthView v = synth_view(const_cast<void *>(d_packed), layers, n_layers, style_dim);
+    auto latent = [&](int idx) { return d_w + (size_t)(idx < w_layers ? idx : w_layers - 1) * n * style_dim; };
+    for (int l = 0; d_S && l < n_layers; ++l)
+        if (d_S[l])
+            if (int r = conv_style(v, layers[l], l, latent(l), n, style_dim, d_S[l], stream)) return r;
+    for (int j = 0; j < n_rgb; ++j)
+        if (d_rgb_s[j])
+            if (int r = rgb_style(rgbs[j], latent(2 * j + 1), n, style_dim, (float *)d_workspace, d_rgb_s[j], stream)) return r;
+    return GSB_OK;
+}
+
+extern "C" size_t gsb_synthesis_render_styled_workspace_bytes(const gsb_styled_conv *layers, int n_run, int64_t n) {
+    if (!layers || n_run < 1 || n_run > gsb::SY_MAX_LAYERS || n < 1) return 0;
+    return gsb::synth_ws(nullptr, layers, n_run, n, true, 0, false).bytes;
+}
+
+extern "C" int gsb_synthesis_render_styled(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int n_run, int style_dim,
+                                           const gsb_to_rgb *rgbs, int n_rgb, const float *const *d_S, const float *const *d_rgb_s,
+                                           int64_t n, float *d_act_out, int64_t ld_act, float *d_rgb_out, void *d_workspace,
+                                           size_t workspace_bytes, gsb_stream_t stream) {
+    using namespace gsb;
+    SynthWs w;
+    if (int r = check_run(d_packed, layers, n_layers, n_run, style_dim, rgbs, n_rgb, false, n, d_act_out, ld_act, d_rgb_out, d_workspace,
+                          workspace_bytes, false, &w)) return r;
+    GSB_CHECK_ARG(d_S && (n_rgb == 0 || d_rgb_s), "synthesis_render_styled: null style list");
+    for (int l = 0; l < n_run; ++l)
+        GSB_CHECK_ARG(d_S[l] && aligned16(d_S[l]), "synthesis_render_styled: style of layer %d is null or not 16-byte aligned", l);
+    for (int j = 0; j < n_rgb; ++j)
+        GSB_CHECK_ARG(d_rgb_s[j] && aligned16(d_rgb_s[j]), "synthesis_render_styled: style of ToRGB %d is null or not 16-byte aligned", j);
+    if (n == 0) return GSB_OK;
+    return synthesis_run(d_packed, layers, n_layers, n_run, style_dim, rgbs, n_rgb, d_S, d_rgb_s, n, d_act_out, ld_act, d_rgb_out, w,
+                         stream);
 }
 
 extern "C" int gsb_synthesis_status(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int style_dim, unsigned *h_flags) {

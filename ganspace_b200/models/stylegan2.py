@@ -44,7 +44,11 @@ class EqualLinear(nn.Module):
         self.lr_mul = lr_mul
         self.pack_cache = _native.Repacked()
 
-    def forward(self, x):
+    def forward(self, x=None, _result=None):
+        if _result is not None:
+            # a ModulatedConv2d.modulation layer: its style rows come from the fused chain's style stage
+            # (models.wrappers.StyleGAN2); this call only hands them to the forward hooks, which may return edited rows
+            return _result
         if self.activation != "fused_lrelu" or self.weight.shape[0] != self.weight.shape[1]:
             raise NotImplementedError("EqualLinear outside the mapping network is not built yet (SURVEY 8 a5)")
         packed = self.pack_cache.get([self.weight, self.bias], lambda: _native.PackedMapping(
@@ -250,6 +254,38 @@ class Generator(nn.Module):
     def get_latent(self, z):
         return self.style(z)
 
+    def chain_layers(self):
+        """(name, module) of the StyledConv layers conv1, convs.0, ... and of the ToRGB layers to_rgb1, to_rgbs.0, ..."""
+        return ([("conv1", self.conv1)] + [(f"convs.{k}", m) for k, m in enumerate(self.convs)],
+                [("to_rgb1", self.to_rgb1)] + [(f"to_rgbs.{j}", m) for j, m in enumerate(self.to_rgbs)])
+
+    def style_layers(self):
+        """The style space: (name, chain, index, latent entry, width) of every modulation layer, in execution order.  ``chain`` is
+        'conv' (index 0 = conv1, k + 1 = convs.k) or 'rgb' (index 0 = to_rgb1, j + 1 = to_rgbs.j); the latent entry is the
+        [N, n_latent, 512] latent's column the layer reads (model.py:546-561); width = the layer's input channels."""
+        convs, rgbs = self.chain_layers()
+        out = []
+        for l, (name, m) in enumerate(convs):
+            out.append((f"{name}.conv.modulation", "conv", l, l, m.conv.in_channel))
+            if l % 2 == 0:
+                j = l // 2
+                out.append((f"{rgbs[j][0]}.conv.modulation", "rgb", j, 2 * j + 1, rgbs[j][1].conv.in_channel))
+        return out
+
+    def unhookable_layers(self):
+        """Sub-modules of the StyledConv and ToRGB layers that run inside the fused chain and have no output of their own to
+        hook: every one except the '.conv.modulation' style layers."""
+        convs, rgbs = self.chain_layers()
+        return [f"{name}.{c}" for name, m in convs + rgbs for c, _ in m.named_modules() if c and c != "conv.modulation"]
+
+    def latent(self, styles, inject_index=None, truncation=1, truncation_latent=None, input_is_w=False):
+        """The [N, n_latent, style_dim] per-layer latent of a forward call (model.py:511-552)."""
+        if not input_is_w:
+            styles = [self.style(s) for s in styles]
+        if truncation < 1:
+            styles = [truncation_latent + truncation * (s - truncation_latent) for s in styles]
+        return self.latents_per_layer(styles, inject_index)
+
     def latents_per_layer(self, styles, inject_index=None):
         """model.py:527-552: the [N, n_latent, style_dim] latent of a forward call from one, two or n_latent styles."""
         if len(styles) == 1:
@@ -272,11 +308,7 @@ class Generator(nn.Module):
         if _synthesis is None:
             raise NotImplementedError("Generator.forward needs the wrapper's packed synthesis chain (StyleGAN2.forward); "
                                       "randomised noise is not built")
-        if not input_is_w:
-            styles = [self.style(s) for s in styles]
-        if truncation < 1:
-            styles = [truncation_latent + truncation * (s - truncation_latent) for s in styles]
-        latent = self.latents_per_layer(styles, inject_index)                       # [N, n_latent, S]
+        latent = self.latent(styles, inject_index, truncation, truncation_latent, input_is_w)     # [N, n_latent, S]
         mods = [self.conv1] + list(self.convs)
         rgbs = [self.to_rgb1] + list(self.to_rgbs)
         w_layers = latent.permute(1, 0, 2).contiguous()

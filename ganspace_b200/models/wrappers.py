@@ -315,31 +315,115 @@ class StyleGAN2(_StyledGenerator):
     def forward(self, x):
         """wrappers.py:188-192: images in [0, 1] (before clamping) from one latent, a pair, or one latent per layer.  Hooked
         StyledConv / ToRGB layers receive their activations (retain_layer works); an edit installed on a hooked layer would
-        have to be re-fed into the fused chain, which is not built -- it raises instead of being silently ignored."""
+        have to be re-fed into the fused chain, which is not built -- it raises instead of being silently ignored.  Hooked style
+        layers ('*.conv.modulation') receive their style rows, and what their hooks return is what every chain run of the call
+        modulates with."""
+        self._reject_sub_module_hooks()
         x = x if isinstance(x, list) else [x]
         names = self.synthesis_layer_names()
+        target, rgb_upto = len(names) - 1, len(self.model.to_rgbs)
         syn = self._synthesis(len(names))
-        out, latent = self.model(x, noise=self.noise, truncation=self.truncation, truncation_latent=self.latent_avg,
-                                 input_is_w=self.w_primary, return_latents=True, _synthesis=syn)
-        self._fire_hooks(latent, len(names) - 1, rgb_upto=len(self.model.to_rgbs))
-        return 0.5 * (out + 1)
+        if not self._hooked_styles(target, rgb_upto):
+            out, latent = self.model(x, noise=self.noise, truncation=self.truncation, truncation_latent=self.latent_avg,
+                                     input_is_w=self.w_primary, return_latents=True, _synthesis=syn)
+            self._fire_hooks(latent, target, rgb_upto=rgb_upto)
+            return 0.5 * (out + 1)
+        latent = self.model.latent(x, truncation=self.truncation, truncation_latent=self.latent_avg, input_is_w=self.w_primary)
+        styles = self._styles(latent.permute(1, 0, 2).contiguous(), target, rgb_upto, True)
+        _, img = syn.render_styled([styles[0][l] for l in range(len(names))], [styles[1][j] for j in range(rgb_upto + 1)], len(names),
+                                   [r.describe() for _, r in self.model.chain_layers()[1]])
+        self._fire_hooks(None, target, rgb_upto=rgb_upto, styles=styles)
+        return 0.5 * (img.permute(0, 3, 1, 2) + 1)
 
-    def _fire_hooks(self, latent, target, rgb_upto=-1):
+    def _fire_hooks(self, latent, target, rgb_upto=-1, styles=None):
         """Hand the activations of hooked StyledConv layers 0..target (and hooked ToRGB layers 0..rgb_upto) to their hooks:
-        each gets its own run of the fused chain up to that layer."""
-        mods = [self.model.conv1] + list(self.model.convs)
-        rgbs = [self.model.to_rgb1] + list(self.model.to_rgbs)
-        names, rgb_names = self.synthesis_layer_names(), self._rgb_names()
-        w_layers = latent.permute(1, 0, 2).contiguous()
+        each gets its own run of the fused chain up to that layer, on the per-layer latents ``latent`` or, when given, on the
+        style rows ``styles`` (from ``_styles``)."""
+        convs, rgbs = self.model.chain_layers()
+        w_layers = latent.permute(1, 0, 2).contiguous() if styles is None else None
+
+        def run(n_run, n_rgb, want_act):
+            syn = self._synthesis(n_run)
+            descs = [r.describe() for _, r in rgbs[:n_rgb]]
+            if styles is None:
+                return syn, syn.render(w_layers, n_run, descs, want_act=want_act)
+            return syn, syn.render_styled([styles[0][l] for l in range(n_run)], [styles[1][j] for j in range(n_rgb)], n_run, descs,
+                                          want_act=want_act)
         for i in range(target + 1):
-            if len(mods[i]._forward_hooks):
-                syn = self._synthesis(i + 1)
-                act, _ = syn.render(w_layers, i + 1, [], want_act=True)
-                self._hand_off(mods[i], act, *syn.shapes[i], True, names[i])
+            if len(convs[i][1]._forward_hooks):
+                syn, (act, _) = run(i + 1, 0, True)
+                self._hand_off(convs[i][1], act, *syn.shapes[i], True, convs[i][0])
         for j in range(rgb_upto + 1):
-            if len(rgbs[j]._forward_hooks):
-                _, img = self._synthesis(2 * j + 1).render(w_layers, 2 * j + 1, [r.describe() for r in rgbs[:j + 1]])
-                self._hand_off(rgbs[j], img, img.shape[1], 3, True, rgb_names[j])
+            if len(rgbs[j][1]._forward_hooks):
+                _, (_, img) = run(2 * j + 1, j + 1, False)
+                self._hand_off(rgbs[j][1], img, img.shape[1], 3, True, rgbs[j][0])
+
+    # ---- style space: the modulation layers '*.conv.modulation' -----------------------------------------
+    def _style_modules(self, target, rgb_upto):
+        """(name, chain, index, module) of the style layers a run to StyledConv ``target`` and ToRGB ``rgb_upto`` executes."""
+        convs, rgbs = self.model.chain_layers()
+        return [(name, chain, i, (convs if chain == "conv" else rgbs)[i][1].conv.modulation)
+                for name, chain, i, _, _ in self.model.style_layers() if i <= (target if chain == "conv" else rgb_upto)]
+
+    def _hooked_styles(self, target, rgb_upto):
+        return any(len(m._forward_hooks) for *_, m in self._style_modules(target, rgb_upto))
+
+    def _styles(self, w_layers, target, rgb_upto, all_rows):
+        """Style rows for per-layer latents ``w_layers`` [Lw, n, 512], computed once; each hooked style layer up to StyledConv
+        ``target`` / ToRGB ``rgb_upto`` fires once with its rows and what it returns replaces them.  Returns ({conv l: rows},
+        {ToRGB j: rows}) with the rows of every layer in that range when ``all_rows`` (for chain runs), else of the hooked ones."""
+        mods = self._style_modules(target, rgb_upto)
+        want = mods if all_rows else [t for t in mods if len(t[3]._forward_hooks)]
+        rgbs = self.model.chain_layers()[1]
+        rgb_idx = [i for _, chain, i, _ in want if chain == "rgb"]
+        syn = self._synthesis(max([target + 1] + [2 * j + 1 for j in rgb_idx]))
+        S, R = syn.styles(w_layers, [i for _, chain, i, _ in want if chain == "conv"], rgb_idx,
+                          [r.describe() for _, r in rgbs[:max(rgb_idx, default=-1) + 1]])
+        for name, chain, i, m in want:
+            if len(m._forward_hooks):
+                rows = S if chain == "conv" else R
+                rows[i] = self._hand_style(m, rows[i], name)
+        return S, R
+
+    @staticmethod
+    def _hand_style(module, rows, name):
+        """Hands a style layer's rows [n, cin] to its hooks and returns what the chain uses: the rows, or the hooks' edit (a
+        [1, cin] edit applies to every sample, as nethook broadcasts it)."""
+        out = module(_result=rows)
+        if out is rows:
+            return rows
+        if out.dim() == 2 and out.shape[0] == 1:
+            out = out.expand(rows.shape[0], -1)
+        if tuple(out.shape) != tuple(rows.shape):
+            raise ValueError(f"an edit on '{name}' must keep the style's shape {tuple(rows.shape)} (or [1, {rows.shape[1]}]), got "
+                             f"{tuple(out.shape)}")
+        return out.to(device=rows.device, dtype=torch.float32).contiguous()
+
+    def _reject_sub_module_hooks(self):
+        guarded = getattr(self, "_guarded", None)
+        if guarded is None:
+            mods = dict(self.model.named_modules())
+            guarded = self._guarded = [(n, mods[n]) for n in self.model.unhookable_layers()]
+        for name, m in guarded:
+            if len(m._forward_hooks) or len(m._forward_pre_hooks):
+                raise NotImplementedError(self._unhookable_message(name))
+
+    def _unhookable_message(self, name):
+        return (f"StyleGAN2: a hook on '{name}' is not supported: the StyledConv and ToRGB layers run as one fused chain; the "
+                "hookable synthesis layers are conv1, convs.k, to_rgb1, to_rgbs.j and their style layers '<layer>.conv.modulation'")
+
+    def _stop(self, layer_name):
+        """(last StyledConv, last ToRGB) that partial_forward to ``layer_name`` runs (wrappers.py:228-255).  A style layer stops
+        at the StyledConv or ToRGB that contains it."""
+        base = layer_name[:-len(".conv.modulation")] if layer_name.endswith(".conv.modulation") else layer_name
+        names, rgb_names = self.synthesis_layer_names(), self._rgb_names()
+        if base in names:
+            t = names.index(base)
+            return t, (t - 1) // 2             # the reference computes every to_rgb that precedes the target as well
+        if base in rgb_names:
+            j = rgb_names.index(base)
+            return 2 * j, j
+        raise RuntimeError(f"Unknown layer '{layer_name}'")
 
     # ---- synthesis chain conv1, convs.0 .. convs.k (wrappers.py:224-255) ------------------------------------
     def synthesis_layer_names(self):
@@ -383,7 +467,11 @@ class StyleGAN2(_StyledGenerator):
 
     def partial_forward(self, x, layer_name):
         """wrappers.py:194-259: run up to (and including) the named layer; side effect = its hooks fire.  ``x``: one latent, a
-        pair (style mixing at a random index, as the reference) or one latent per layer."""
+        pair (style mixing at a random index, as the reference) or one latent per layer.  A style layer '<layer>.conv.modulation'
+        runs as far as <layer>; when no StyledConv or ToRGB on the way is hooked, only its style rows are computed."""
+        self._reject_sub_module_hooks()
+        if any(layer_name == n for n, _ in self._guarded):
+            raise NotImplementedError(self._unhookable_message(layer_name))
         styles = x if isinstance(x, list) else [x]
         if not self.w_primary:
             styles = [self.model.style(s) for s in styles]
@@ -391,31 +479,32 @@ class StyleGAN2(_StyledGenerator):
             # (the reference builds the [N, n_latent, 512] repeat + StridedStyle stack before this early exit, wrappers.py:202-222 --
             # 328 MB of traffic per 10k batch that nothing reads; skipped here)
             return
-        latent = self.model.latents_per_layer(styles)             # [N, n_latent, 512]
+        latent = None if (len(styles) == 1 and layer_name != "input") else self.model.latents_per_layer(styles)   # [N, n_latent, 512]
         if layer_name == "input":
             self.model.input(latent[:, 0])
             return
         names = self.synthesis_layer_names()
-        rgb_names = self._rgb_names()
-        rgb_hooked = any(len(m._forward_hooks) for m in [self.model.to_rgb1] + list(self.model.to_rgbs))
+        target, rgb_upto = self._stop(layer_name)
+        convs, rgbs = self.model.chain_layers()
+        if layer_name.endswith(".conv.modulation") or self._hooked_styles(target, rgb_upto):
+            chain_hooked = any(len(m._forward_hooks) for _, m in convs[:target + 1] + rgbs[:rgb_upto + 1])
+            w_layers = styles[0].reshape(1, -1, 512) if latent is None else latent.permute(1, 0, 2).contiguous()
+            st = self._styles(w_layers, target, rgb_upto, chain_hooked)
+            if chain_hooked:
+                self._fire_hooks(None, target, rgb_upto, styles=st)
+            return
+        if latent is None:
+            latent = self.model.latents_per_layer(styles)
+        rgb_hooked = any(len(m._forward_hooks) for _, m in rgbs)
         if layer_name in names and len(styles) == 1 and not rgb_hooked:
             # one global latent, no ToRGB hook: the decomposition's own call pattern -- the single-latent entry point
-            mods = [self.model.conv1] + list(self.model.convs)
-            target = names.index(layer_name)
             w = styles[0].reshape(-1, 512)
-            for i in [i for i in range(target) if len(mods[i]._forward_hooks)] + [target]:
+            for i in [i for i in range(target) if len(convs[i][1]._forward_hooks)] + [target]:
                 syn = self._synthesis(target + 1)
                 # (an edit on the target layer itself has nothing downstream inside partial_forward)
-                self._hand_off(mods[i], syn.forward(w, i + 1), *syn.shapes[i], i < target, names[i])
-        elif layer_name in names:
-            target = names.index(layer_name)
-            # the reference computes every to_rgb that precedes the target as well (wrappers.py:232-255)
-            self._fire_hooks(latent, target, rgb_upto=(target - 1) // 2 if target >= 1 else -1)
-        elif layer_name in rgb_names:
-            j = rgb_names.index(layer_name)
-            self._fire_hooks(latent, 2 * j, rgb_upto=j)
+                self._hand_off(convs[i][1], syn.forward(w, i + 1), *syn.shapes[i], i < target, names[i])
         else:
-            raise RuntimeError(f"Unknown layer '{layer_name}'")
+            self._fire_hooks(latent, target, rgb_upto=rgb_upto)
 
     def set_noise_seed(self, seed):
         # same generator stream as the reference (torch.manual_seed(seed); torch.randn per noise map),
@@ -759,7 +848,12 @@ def get_instrumented_model(name, output_class, layers, device, **kwargs):
             raise RuntimeError(f"Unknown layer '{layer_name}''")
     if hasattr(model, "use_z"):
         model.use_z()
-    inst = _annotate_shapes(InstrumentedModel(model), model, layers)
+    inst = InstrumentedModel(model)
+    try:
+        _annotate_shapes(inst, model, layers)
+    except Exception:
+        inst.close()                # a refused layer leaves no hook behind on the (cached) model
+        raise
     if kwargs.get("use_w", False):
         model.use_w()
     return inst
