@@ -75,6 +75,9 @@ SIGNATURES = {
     "gsb_stylegan_workspace_bytes": (_Z, [_P, _I, _L]),
     "gsb_stylegan_forward": (_I, [_P, _P, _I, _I, _I, _P, _I, _L, _P, _L, _P, _P, _Z, _P]),
     "gsb_stylegan_status": (_I, [_P, _P, _I, _I, _P]),
+    "gsb_stylegan_styles": (_I, [_P, _P, _I, _I, _P, _I, _L, _P, _I, _P, _P]),
+    "gsb_stylegan_forward_styled_workspace_bytes": (_Z, [_P, _I, _L]),
+    "gsb_stylegan_forward_styled": (_I, [_P, _P, _I, _I, _I, _P, _L, _P, _L, _P, _P, _Z, _P]),
     "gsb_biggan_conv_forward": (_I, [_P, _L, _P]),
     "gsb_biggan_bn_table": (_I, [_P, _L, _I, _P, _P, _P, _F, _I, _P, _P, _P]),
     "gsb_biggan_attn_pool": (_I, [_P, _L, _I, _I, _P, _P, _P]),
@@ -1072,6 +1075,53 @@ class PackedStyleGAN(_PackedTapGenerator):
             _check(lib.gsb_stylegan_forward(_ptr(self.packed), self.desc, self.n_layers, n_run, self.dlatent, _ptr(w3), Lw, n,
                                             C.c_void_p(act.data_ptr() if act is not None else 0), act.stride(0) if act is not None else 0,
                                             _ptr(rgb), _ptr(ws), ws.numel(), _stream()), "gsb_stylegan_forward")
+        instrument.count(1)
+        instrument.add_rows("stylegan", n)
+        return act, rgb
+
+    def style_width(self, l: int) -> int:
+        """Width 2 cout of layer ``l``'s style rows ([s0 | s1] of its StyleMod)."""
+        return 2 * self.shapes[l][1]
+
+    def styles(self, w: torch.Tensor, layers):
+        """The style-space rows (gsb_stylegan_styles): for dlatents ``w`` as in ``forward``, the StyleMod output [n, 2 cout] of every
+        layer in ``layers``.  Returns {layer: rows}.  The launch is the chain's own style GEMM, so the rows are bit-identical to the
+        ones ``forward`` consumes."""
+        lib = load()
+        assert w.is_cuda and w.dtype == torch.float32 and w.shape[-1] == self.dlatent and w.dim() in (2, 3)
+        w3 = (w[None] if w.dim() == 2 else w).contiguous()
+        Lw, n = int(w3.shape[0]), int(w3.shape[1])
+        layers = sorted(set(int(l) for l in layers))
+        assert layers and all(0 <= l < self.n_layers and (Lw == 1 or l < Lw) for l in layers), layers
+        S = {l: torch.empty((n, self.style_width(l)), dtype=torch.float32, device=self.device) for l in layers}
+        idx = (C.c_int * len(layers))(*layers)
+        ptrs = (C.c_void_p * len(layers))(*[S[l].data_ptr() for l in layers])
+        with torch.cuda.device(self.device), instrument.section("styles"):
+            _check(lib.gsb_stylegan_styles(_ptr(self.packed), self.desc, self.n_layers, self.dlatent, _ptr(w3), Lw, n, idx, len(layers),
+                                           ptrs, _stream()), "gsb_stylegan_styles")
+        instrument.count(1)
+        instrument.add_rows("styles", n)
+        return S
+
+    def forward_styled(self, S, n_run: int, out: torch.Tensor = None, want_act: bool = True, want_rgb: bool = False):
+        """``forward`` on caller-given styles (gsb_stylegan_forward_styled): ``S[l]`` [n, 2 cout] fp32 for the layers 0 .. n_run-1
+        (a list or a dict by layer).  Same outputs as ``forward``."""
+        lib = load()
+        rows = [S[l] for l in range(n_run)]
+        n = int(rows[0].shape[0])
+        for l, t in enumerate(rows):
+            assert t.is_cuda and t.dtype == torch.float32 and tuple(t.shape) == (n, self.style_width(l)), \
+                f"layer {l}: style rows [{n}, {self.style_width(l)}] fp32 on the device expected, got {tuple(t.shape)} {t.dtype}"
+        act, rgb = self._outputs(n, n_run, out, want_act, want_rgb, self.device)
+        if n == 0:
+            return act, rgb
+        S_run = torch.cat(rows, dim=1).contiguous()              # [n, s_run]: the chain's column order
+        ws = scratch.get("stylegan", lib.gsb_stylegan_forward_styled_workspace_bytes(self.desc, n_run, n), self.device)
+        with torch.cuda.device(self.device), instrument.section("stylegan"):
+            _check(lib.gsb_stylegan_forward_styled(_ptr(self.packed), self.desc, self.n_layers, n_run, self.dlatent, _ptr(S_run), n,
+                                                   C.c_void_p(act.data_ptr() if act is not None else 0),
+                                                   act.stride(0) if act is not None else 0, _ptr(rgb), _ptr(ws), ws.numel(), _stream()),
+                   "gsb_stylegan_forward_styled")
         instrument.count(1)
         instrument.add_rows("stylegan", n)
         return act, rgb

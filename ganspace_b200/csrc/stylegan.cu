@@ -23,7 +23,8 @@
 //     finish        one warp per (sample, channel): the tiles' sums in a fixed order -> mean and the affine
 //     apply         the affine -> the next layer's operand as fp16 hi/lo, and / or the hooked activation as fp32 NHWC rows with a
 //                   caller-given row stride, and / or (last layer) the 1x1 torgb conv
-// The StyleMod vectors of every layer come from one kernel before the first layer.  No float atomics; every reduction runs in
+// The StyleMod vectors of every layer come from one style GEMM launch before the first layer (the style stage); the rest is the
+// run stage, which gsb_stylegan_forward_styled runs on caller-given styles.  No float atomics; every reduction runs in
 // a fixed order inside one sample, so a sample's result does not depend on the batch it is part of.
 //
 // Channel counts: cin and cout are powers of two in [16, 512].  The 16-channel layers of the 1024-px generators run on the same
@@ -65,7 +66,6 @@ struct SgView {
     float *cst;               // [16, c0] NHWC
     float *style_wt;          // [dlatent, s_total]  A^T / sqrt(dlatent), all layers side by side
     float *style_b;           // [s_total]
-    int *style_layer;         // [s_total]  layer of each column
     int s_total;
     float *rgb_w;             // [3, c_last] / sqrt(c_last)
     float *rgb_b;             // [3]
@@ -83,7 +83,6 @@ static SgView sg_view(void *base, const gsb_stylegan_layer *layers, int n_layers
     v.cst = (float *)take((size_t)16 * layers[0].cout * 4);
     v.style_wt = (float *)take((size_t)dlatent * v.s_total * 4);
     v.style_b = (float *)take((size_t)v.s_total * 4);
-    v.style_layer = (int *)take((size_t)v.s_total * 4);
     v.rgb_w = (float *)take((size_t)3 * layers[n_layers - 1].cout * 4);
     v.rgb_b = (float *)take(16);
     int soff = 0;
@@ -120,31 +119,166 @@ static int sg_check(const gsb_stylegan_layer *layers, int n_layers, int dlatent)
 }
 
 // ---- pack kernels ---------------------------------------------------------------------------------------
-// A [rows, K] (StyleMod lin.weight) -> dst[k * ld + r] = A[r, k] * scale; column `layer` tag per row
-__global__ void sg_transpose_scale_kernel(const float *__restrict__ A, int rows, int K, float scale, float *__restrict__ dst, int64_t ld,
-                                          int *__restrict__ tag, int layer) {
+// A [rows, K] (StyleMod lin.weight) -> dst[k * ld + r] = A[r, k] * scale
+__global__ void sg_transpose_scale_kernel(const float *__restrict__ A, int rows, int K, float scale, float *__restrict__ dst, int64_t ld) {
     for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < (int64_t)rows * K; idx += (int64_t)gridDim.x * blockDim.x) {
         const int r = (int)(idx / K), k = (int)(idx % K);
         dst[(int64_t)k * ld + r] = A[idx] * scale;
-        if (k == 0) tag[r] = layer;
     }
 }
 
-// ---- forward kernels ------------------------------------------------------------------------------------
-// S[b, j] = w_{layer(j)}[b] . style_wt[:, j] + style_b[j] for columns j < s_run; one thread per (b, j), k in order.
-// w_layers == 1: one latent for every layer; otherwise w [w_layers, n, dlatent] and layer l reads latent l.
-__global__ void __launch_bounds__(256)
-sg_style_kernel(const float *__restrict__ w, int w_layers, int64_t n, int dlatent, const float *__restrict__ wt,
-                const float *__restrict__ bias, const int *__restrict__ tag, int s_total, int s_run, float *__restrict__ S) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    const int64_t b = blockIdx.y;
-    if (j >= s_run) return;
-    const int li = w_layers == 1 ? 0 : tag[j];
-    const float *wr = w + ((int64_t)li * n + b) * dlatent;
-    float acc = 0.f;
-    for (int k = 0; k < dlatent; ++k) acc = fmaf(wr[k], wt[(int64_t)k * s_total + j], acc);
-    S[b * s_run + j] = acc + bias[j];
+// ---- style GEMM -------------------------------------------------------------------------------------------
+// The StyleMod rows of a set of layers:  S_l[b, j] = w_{lat(l)}[b] . style_wt[:, col0(l) + j] + style_b[col0(l) + j],  every
+// element computed as  acc = 0; acc = fmaf(w[k], wt[k][j], acc) for k = 0 .. dlatent-1 in order; acc + bias  -- so a row does not
+// depend on the tile, the batch or the launch it is computed in.
+// Register-tiled FP32 GEMM: a CTA computes 32 TM rows x SGS_BN = 32 columns, 256 threads of TM rows x 4 columns; operands are
+// staged through shared memory in BK-deep slices by a cp.async double buffer.  Small batches (TM <= 2) take deeper slices and
+// four CTAs per SM: with little arithmetic per slice, the loads in flight -- the slices' latency -- set the kernel's time.  Every 2 cout is a multiple of
+// 32, so a column tile lies inside one layer and reads one latent per sample.  The grid is linear, column tiles fastest: the
+// CTAs that share a slice of latent rows run side by side (the rows come from L2 once per column tile, from HBM once).
+constexpr int SGS_BN = 32, SGS_THREADS = 256, SGS_PAD = 4;
+
+struct SgStyleJob {
+    const float *w;                       // [w_layers, n, dlatent]
+    const float *wt, *bias;               // packed: [dlatent, s_total], [s_total]
+    int64_t n;
+    int dlatent, s_total, n_sel;
+    int col0[SG_MAX_LAYERS];              // selected layer s: its first column in the packed style matrix
+    int tile0[SG_MAX_LAYERS + 1];         // its first column tile (prefix sums; tile0[n_sel] = all column tiles)
+    int lat[SG_MAX_LAYERS];               // the latent it reads
+    float *out[SG_MAX_LAYERS];            // its rows: out[s] + b * ld[s] + j
+    int64_t ld[SG_MAX_LAYERS];
+};
+
+__device__ __forceinline__ void sgs_cp16(float *dst, const float *src, bool valid) {
+    const unsigned sa = (unsigned)__cvta_generic_to_shared(dst);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(sa), "l"(src), "r"(valid ? 16 : 0) : "memory");
 }
+
+template <int TM, int BK>
+__global__ void __launch_bounds__(SGS_THREADS, TM <= 2 ? 4 : 2)
+sg_style_gemm_kernel(const __grid_constant__ SgStyleJob J) {
+    constexpr int BM = 32 * TM;
+    __shared__ __align__(16) float As[2][BM][BK + SGS_PAD];
+    __shared__ __align__(16) float Bs[2][BK][SGS_BN];
+    const int n_ct = J.tile0[J.n_sel];
+    const int ct = (int)(blockIdx.x % (unsigned)n_ct);
+    const int64_t r0 = (int64_t)(blockIdx.x / (unsigned)n_ct) * BM;
+    int s = 0;
+    while (ct >= J.tile0[s + 1]) ++s;
+    const int jl = (ct - J.tile0[s]) * SGS_BN;                      // first column of the tile inside its layer
+    const int jg = J.col0[s] + jl;                                  // ... in the packed style matrix
+    const float *wl = J.w + (int64_t)J.lat[s] * J.n * J.dlatent;
+    const int tid = threadIdx.x, tc = tid & 7, tr = tid >> 3;
+    const int nk = (J.dlatent + BK - 1) / BK;
+
+    auto load = [&](int kt, int buf) {
+        const int k0 = kt * BK;
+        for (int c = tid; c < BM * BK / 4; c += SGS_THREADS) {      // A: BM rows x BK/4 quads (rows past n are zero-filled)
+            const int row = c / (BK / 4), kq = (c % (BK / 4)) * 4;
+            const int64_t b = r0 + row < J.n ? r0 + row : J.n - 1;
+            const bool ok = k0 + kq < J.dlatent && r0 + row < J.n;
+            sgs_cp16(&As[buf][row][kq], wl + b * J.dlatent + (ok ? k0 + kq : 0), ok);
+        }
+        for (int c = tid; c < BK * SGS_BN / 4; c += SGS_THREADS) {  // B: BK rows x 8 quads
+            const int k = c >> 3, jq = (c & 7) * 4;
+            const bool ok = k0 + k < J.dlatent;
+            sgs_cp16(&Bs[buf][k][jq], J.wt + (int64_t)(ok ? k0 + k : 0) * J.s_total + jg + jq, ok);
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+
+    float acc[TM][4];
+#pragma unroll
+    for (int i = 0; i < TM; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+
+    load(0, 0);
+    for (int kt = 0; kt < nk; ++kt) {
+        const int buf = kt & 1;
+        if (kt + 1 < nk) {
+            load(kt + 1, buf ^ 1);
+            asm volatile("cp.async.wait_group 1;" ::: "memory");
+        } else {
+            asm volatile("cp.async.wait_group 0;" ::: "memory");
+        }
+        __syncthreads();
+        const int kmax = J.dlatent - kt * BK;                       // only the last slice of a dlatent % BK != 0 is partial
+        if (kmax >= BK) {
+#pragma unroll
+            for (int kq = 0; kq < BK; kq += 4) {
+                float4 bq[4];
+#pragma unroll
+                for (int q = 0; q < 4; ++q) bq[q] = *reinterpret_cast<const float4 *>(&Bs[buf][kq + q][tc * 4]);
+#pragma unroll
+                for (int i = 0; i < TM; ++i) {
+                    const float4 a = *reinterpret_cast<const float4 *>(&As[buf][tr + 32 * i][kq]);
+                    const float av[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) {
+                        acc[i][0] = fmaf(av[q], bq[q].x, acc[i][0]);
+                        acc[i][1] = fmaf(av[q], bq[q].y, acc[i][1]);
+                        acc[i][2] = fmaf(av[q], bq[q].z, acc[i][2]);
+                        acc[i][3] = fmaf(av[q], bq[q].w, acc[i][3]);
+                    }
+                }
+            }
+        } else {
+            for (int k = 0; k < kmax; ++k) {
+                const float4 bq = *reinterpret_cast<const float4 *>(&Bs[buf][k][tc * 4]);
+#pragma unroll
+                for (int i = 0; i < TM; ++i) {
+                    const float a = As[buf][tr + 32 * i][k];
+                    acc[i][0] = fmaf(a, bq.x, acc[i][0]);
+                    acc[i][1] = fmaf(a, bq.y, acc[i][1]);
+                    acc[i][2] = fmaf(a, bq.z, acc[i][2]);
+                    acc[i][3] = fmaf(a, bq.w, acc[i][3]);
+                }
+            }
+        }
+        __syncthreads();                                            // the slice is read before the next load overwrites it
+    }
+    const float4 bv = *reinterpret_cast<const float4 *>(J.bias + jg + tc * 4);
+#pragma unroll
+    for (int i = 0; i < TM; ++i) {
+        const int64_t b = r0 + tr + 32 * i;
+        if (b >= J.n) continue;
+        float *o = J.out[s] + b * J.ld[s] + jl + tc * 4;
+        o[0] = acc[i][0] + bv.x;
+        o[1] = acc[i][1] + bv.y;
+        o[2] = acc[i][2] + bv.z;
+        o[3] = acc[i][3] + bv.w;
+    }
+}
+
+// One launch of the style GEMM over the layers of `J` (n_sel, col0, lat, out, ld filled in by the caller); rows are tiled by the
+// smallest TM whose 32 TM rows hold n, at most 8.
+static int sg_style_launch(SgStyleJob &J, const SgView &v, const gsb_stylegan_layer *layers, const int *sel, cudaStream_t st) {
+    int t = 0;
+    for (int s = 0; s < J.n_sel; ++s) {
+        J.tile0[s] = t;
+        t += 2 * layers[sel[s]].cout / SGS_BN;
+    }
+    J.tile0[J.n_sel] = t;
+    J.wt = v.style_wt;
+    J.bias = v.style_b;
+    J.s_total = v.s_total;
+    if (J.n == 0 || t == 0) return GSB_OK;
+    const int TM = J.n <= 32 ? 1 : J.n <= 64 ? 2 : J.n <= 128 ? 4 : 8;
+    const int64_t blocks = (J.n + 32 * TM - 1) / (32 * TM) * t;
+    GSB_CHECK_ARG(blocks <= 0x7fffffff, "stylegan: %lld style tiles exceed one launch", (long long)blocks);
+    switch (TM) {
+        case 1: sg_style_gemm_kernel<1, 64><<<(unsigned)blocks, SGS_THREADS, 0, st>>>(J); break;
+        case 2: sg_style_gemm_kernel<2, 32><<<(unsigned)blocks, SGS_THREADS, 0, st>>>(J); break;
+        case 4: sg_style_gemm_kernel<4, 16><<<(unsigned)blocks, SGS_THREADS, 0, st>>>(J); break;
+        default: sg_style_gemm_kernel<8, 16><<<(unsigned)blocks, SGS_THREADS, 0, st>>>(J); break;
+    }
+    GSB_CHECK_LAUNCH();
+    return GSB_OK;
+}
+
+// ---- forward kernels ------------------------------------------------------------------------------------
 
 // the 3x3 conv outputs of an up-conv layer (before the blur), from Y at the input resolution R/2 with row length np.  One thread
 // per 4 channels of an output pixel.
@@ -297,7 +431,7 @@ sg_apply_kernel(SgApply e, int64_t nb, int hw, int c) {
 
 // ---- workspace --------------------------------------------------------------------------------------------
 struct SgWs {
-    float *S;               // [n, s_run]
+    float *S;               // [n, s_run]  (gsb_stylegan_forward only: the styled run reads the caller's)
     __half *act[2][2];      // [ping-pong][hi/lo]
     float *Y, *U, *A;
     double *part;
@@ -305,7 +439,7 @@ struct SgWs {
     unsigned *queue;        // tile queue of the tap GEMM launches
     size_t bytes;
 };
-static SgWs sg_ws(void *base, const gsb_stylegan_layer *layers, int n_run, int64_t n) {
+static SgWs sg_ws(void *base, const gsb_stylegan_layer *layers, int n_run, int64_t n, bool own_styles) {
     SgWs w;
     char *p = reinterpret_cast<char *>(base);
     size_t off = 0;
@@ -323,7 +457,7 @@ static SgWs sg_ws(void *base, const gsb_stylegan_layer *layers, int n_run, int64
         part_elems = part_elems > pe ? part_elems : pe;
         aff_elems = aff_elems > spc * c.cout ? aff_elems : spc * c.cout;
     }
-    w.S = (float *)take((size_t)n * s_run * 4);
+    w.S = own_styles ? (float *)take((size_t)n * s_run * 4) : nullptr;
     for (int a = 0; a < 2; ++a)
         for (int h = 0; h < 2; ++h) w.act[a][h] = (__half *)take(act_elems * 2);
     w.Y = (float *)take(y_elems * 4);
@@ -334,6 +468,83 @@ static SgWs sg_ws(void *base, const gsb_stylegan_layer *layers, int n_run, int64
     w.queue = (unsigned *)take(sizeof(unsigned));
     w.bytes = off;
     return w;
+}
+
+static int sg_s_run(const gsb_stylegan_layer *layers, int n_run) {
+    int s_run = 0;
+    for (int l = 0; l < n_run; ++l) s_run += 2 * layers[l].cout;
+    return s_run;
+}
+
+// The arguments gsb_stylegan_forward and gsb_stylegan_forward_styled share.
+static int sg_run_check(const gsb_stylegan_layer *layers, int n_layers, int n_run, int dlatent, int64_t n, const float *d_act_out,
+                        int64_t ld_act, const float *d_rgb_out) {
+    if (int r = sg_check(layers, n_layers, dlatent)) return r;
+    GSB_CHECK_ARG(n_run >= 1 && n_run <= n_layers && n >= 0, "stylegan: n_run / n out of range");
+    GSB_CHECK_ARG(!d_rgb_out || n_run == n_layers, "stylegan: the image needs every layer (n_run == n_layers)");
+    if (n == 0) return GSB_OK;
+    GSB_CHECK_ARG(n <= 65535, "stylegan: at most 65535 samples per call (n = %lld)", (long long)n);
+    const gsb_stylegan_layer &last = layers[n_run - 1];
+    GSB_CHECK_ARG(!d_act_out || (ld_act >= (int64_t)last.res_out * last.res_out * last.cout && ld_act % 4 == 0), "stylegan: bad ld_act");
+    return GSB_OK;
+}
+
+// The style GEMM's operand rules: 16-byte cp.async slices of the latent rows.
+static int sg_latents_check(const float *d_w, int dlatent) {
+    GSB_CHECK_ARG(dlatent % 4 == 0 && ((uintptr_t)d_w & 15) == 0,
+                  "stylegan: the style GEMM needs dlatent %% 4 == 0 and 16-byte aligned latents (dlatent = %d)", dlatent);
+    return GSB_OK;
+}
+
+// The run stage: layers 0 .. n_run-1 on the styles S [n, s_run] (the chain's column order).
+static int sg_run(const SgView &v, const SgWs &w, const gsb_stylegan_layer *layers, int n_run, const float *S, int64_t n, float *d_act_out,
+                  int64_t ld_act, float *d_rgb_out, cudaStream_t st) {
+    const int s_run = sg_s_run(layers, n_run);
+    for (int l = 0; l < n_run; ++l) {
+        const gsb_stylegan_layer &c = layers[l];
+        const int dst = l & 1;                                         // layer l reads act[dst ^ 1], writes act[dst]
+        const __half *a_hi = w.act[dst ^ 1][0], *a_lo = w.act[dst ^ 1][1];
+        const bool is_last = (l == n_run - 1);
+        const int R = c.res_out, H = sg_res_in(c), hw = R * R, hw_in = H * H, np = sg_np(c), tile = sg_tile_px(c), tiles = hw / tile;
+        const int64_t spc = sg_chunk_samples(c);
+        for (int64_t b0 = 0; b0 < n; b0 += spc) {
+            const int64_t nb = (b0 + spc <= n) ? spc : (n - b0);
+            const dim3 egrid((unsigned)tiles, (unsigned)nb);
+            if (!c.conv_weight) {
+                sg_epilogue_kernel<0><<<egrid, 256, 0, st>>>(v.cst, R, c.cout, 0, tile, v.L[l].bias, v.L[l].noise_w, v.L[l].noise, w.A, w.part);
+            } else {
+                if (int r = tc_gemm_plain(a_hi + b0 * hw_in * c.cin, a_lo + b0 * hw_in * c.cin, nb * hw_in, c.cin, v.L[l].w_hi, v.L[l].w_lo,
+                                          np, v.L[l].scal, w.Y, v.overflow, w.queue, 0, st)) return r;
+                if (c.upsample) {
+                    const int64_t total = nb * hw * (c.cout / 4);
+                    sg_up_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(w.Y, nb, R, c.cout, np, w.U);
+                    GSB_CHECK_LAUNCH();
+                    sg_epilogue_kernel<2><<<egrid, 256, 0, st>>>(w.U, R, c.cout, np, tile, v.L[l].bias, v.L[l].noise_w, v.L[l].noise, w.A, w.part);
+                } else {
+                    sg_epilogue_kernel<1><<<egrid, 256, 0, st>>>(w.Y, R, c.cout, np, tile, v.L[l].bias, v.L[l].noise_w, v.L[l].noise, w.A, w.part);
+                }
+            }
+            GSB_CHECK_LAUNCH();
+            sg_finish_kernel<<<(unsigned)((nb * c.cout + 7) / 8), 256, 0, st>>>(w.part, nb, c.cout, tiles, hw, S + b0 * s_run, s_run,
+                                                                               v.L[l].style_off, w.aff);
+            GSB_CHECK_LAUNCH();
+            SgApply e;
+            e.A = w.A;
+            e.aff = w.aff;
+            e.out_hi = is_last ? nullptr : w.act[dst][0] + b0 * hw * c.cout;
+            e.out_lo = is_last ? nullptr : w.act[dst][1] + b0 * hw * c.cout;
+            e.out_f32 = (is_last && d_act_out) ? d_act_out + b0 * ld_act : nullptr;
+            e.ld = ld_act;
+            e.rgb_w = (is_last && d_rgb_out) ? v.rgb_w : nullptr;
+            e.rgb_b = v.rgb_b;
+            e.rgb_out = (is_last && d_rgb_out) ? d_rgb_out + b0 * hw * 3 : nullptr;
+            e.overflow = v.overflow;
+            const int64_t total = nb * hw * (c.cout / 4);
+            sg_apply_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(e, nb, hw, c.cout);
+            GSB_CHECK_LAUNCH();
+        }
+    }
+    return GSB_OK;
 }
 
 }  // namespace gsb
@@ -374,7 +585,7 @@ extern "C" int gsb_stylegan_pack(const gsb_stylegan_layer *layers, int n_layers,
         GSB_CHECK_LAUNCH();
         // StyleMod lin: MyLinear(dlatent, 2 cout, gain 1, use_wscale): w_mul = 1 / sqrt(dlatent), b_mul = 1 (model.py:121-131)
         sg_transpose_scale_kernel<<<256, 256, 0, st>>>(c.style_weight, 2 * c.cout, dlatent, (float)(1.0 / sqrt((double)dlatent)),
-                                                       v.style_wt + v.L[l].style_off, v.s_total, v.style_layer + v.L[l].style_off, l);
+                                                       v.style_wt + v.L[l].style_off, v.s_total);
         GSB_CHECK_LAUNCH();
         scale_copy_kernel<<<4, 256, 0, st>>>(c.style_bias, 2 * c.cout, 1.0f, nullptr, v.style_b + v.L[l].style_off);
         GSB_CHECK_LAUNCH();
@@ -390,77 +601,88 @@ extern "C" int gsb_stylegan_pack(const gsb_stylegan_layer *layers, int n_layers,
 
 extern "C" size_t gsb_stylegan_workspace_bytes(const gsb_stylegan_layer *layers, int n_run, int64_t n) {
     if (!layers || n_run < 1 || n_run > gsb::SG_MAX_LAYERS || n < 1) return 0;
-    return gsb::sg_ws(nullptr, layers, n_run, n).bytes;
+    return gsb::sg_ws(nullptr, layers, n_run, n, true).bytes;
+}
+
+extern "C" size_t gsb_stylegan_forward_styled_workspace_bytes(const gsb_stylegan_layer *layers, int n_run, int64_t n) {
+    if (!layers || n_run < 1 || n_run > gsb::SG_MAX_LAYERS || n < 1) return 0;
+    return gsb::sg_ws(nullptr, layers, n_run, n, false).bytes;
 }
 
 extern "C" int gsb_stylegan_forward(const void *d_packed, const gsb_stylegan_layer *layers, int n_layers, int n_run, int dlatent,
                                     const float *d_w, int w_layers, int64_t n, float *d_act_out, int64_t ld_act, float *d_rgb_out,
                                     void *d_workspace, size_t workspace_bytes, gsb_stream_t stream) {
     using namespace gsb;
-    if (int r = sg_check(layers, n_layers, dlatent)) return r;
+    if (int r = sg_run_check(layers, n_layers, n_run, dlatent, n, d_act_out, ld_act, d_rgb_out)) return r;
     GSB_CHECK_ARG(d_packed && d_w && d_workspace && (d_act_out || d_rgb_out), "stylegan: null pointer");
-    GSB_CHECK_ARG(n_run >= 1 && n_run <= n_layers && n >= 0, "stylegan: n_run / n out of range");
     GSB_CHECK_ARG(w_layers == 1 || w_layers >= n_run, "stylegan: w_layers must be 1 or cover every layer run (%d < %d)", w_layers, n_run);
-    GSB_CHECK_ARG(!d_rgb_out || n_run == n_layers, "stylegan: the image needs every layer (n_run == n_layers)");
     if (n == 0) return GSB_OK;
-    GSB_CHECK_ARG(n <= 65535, "stylegan: at most 65535 samples per call (n = %lld)", (long long)n);
-    const gsb_stylegan_layer &last = layers[n_run - 1];
-    GSB_CHECK_ARG(!d_act_out || (ld_act >= (int64_t)last.res_out * last.res_out * last.cout && ld_act % 4 == 0), "stylegan: bad ld_act");
+    if (int r = sg_latents_check(d_w, dlatent)) return r;
     SgView v = sg_view(const_cast<void *>(d_packed), layers, n_layers, dlatent);
-    SgWs w = sg_ws(d_workspace, layers, n_run, n);
+    SgWs w = sg_ws(d_workspace, layers, n_run, n, true);
     if (workspace_bytes < w.bytes) { set_error("stylegan: workspace too small (%zu < %zu)", workspace_bytes, w.bytes); return GSB_ERR_WORKSPACE; }
     cudaStream_t st = (cudaStream_t)stream;
 
-    int s_run = 0;
-    for (int l = 0; l < n_run; ++l) s_run += 2 * layers[l].cout;
-    sg_style_kernel<<<dim3((unsigned)((s_run + 255) / 256), (unsigned)n), 256, 0, st>>>(d_w, w_layers, n, dlatent, v.style_wt, v.style_b,
-                                                                                       v.style_layer, v.s_total, s_run, w.S);
-    GSB_CHECK_LAUNCH();
+    // the style stage: every layer run, in the chain's column order, into S [n, s_run]
+    SgStyleJob J;
+    J.w = d_w;
+    J.n = n;
+    J.dlatent = dlatent;
+    J.n_sel = n_run;
+    int sel[SG_MAX_LAYERS];
+    const int s_run = sg_s_run(layers, n_run);
     for (int l = 0; l < n_run; ++l) {
-        const gsb_stylegan_layer &c = layers[l];
-        const int dst = l & 1;                                         // layer l reads act[dst ^ 1], writes act[dst]
-        const __half *a_hi = w.act[dst ^ 1][0], *a_lo = w.act[dst ^ 1][1];
-        const bool is_last = (l == n_run - 1);
-        const int R = c.res_out, H = sg_res_in(c), hw = R * R, hw_in = H * H, np = sg_np(c), tile = sg_tile_px(c), tiles = hw / tile;
-        const int64_t spc = sg_chunk_samples(c);
-        for (int64_t b0 = 0; b0 < n; b0 += spc) {
-            const int64_t nb = (b0 + spc <= n) ? spc : (n - b0);
-            const dim3 egrid((unsigned)tiles, (unsigned)nb);
-            if (!c.conv_weight) {
-                sg_epilogue_kernel<0><<<egrid, 256, 0, st>>>(v.cst, R, c.cout, 0, tile, v.L[l].bias, v.L[l].noise_w, v.L[l].noise, w.A, w.part);
-            } else {
-                if (int r = tc_gemm_plain(a_hi + b0 * hw_in * c.cin, a_lo + b0 * hw_in * c.cin, nb * hw_in, c.cin, v.L[l].w_hi, v.L[l].w_lo,
-                                          np, v.L[l].scal, w.Y, v.overflow, w.queue, 0, st)) return r;
-                if (c.upsample) {
-                    const int64_t total = nb * hw * (c.cout / 4);
-                    sg_up_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(w.Y, nb, R, c.cout, np, w.U);
-                    GSB_CHECK_LAUNCH();
-                    sg_epilogue_kernel<2><<<egrid, 256, 0, st>>>(w.U, R, c.cout, np, tile, v.L[l].bias, v.L[l].noise_w, v.L[l].noise, w.A, w.part);
-                } else {
-                    sg_epilogue_kernel<1><<<egrid, 256, 0, st>>>(w.Y, R, c.cout, np, tile, v.L[l].bias, v.L[l].noise_w, v.L[l].noise, w.A, w.part);
-                }
-            }
-            GSB_CHECK_LAUNCH();
-            sg_finish_kernel<<<(unsigned)((nb * c.cout + 7) / 8), 256, 0, st>>>(w.part, nb, c.cout, tiles, hw, w.S + b0 * s_run, s_run,
-                                                                               v.L[l].style_off, w.aff);
-            GSB_CHECK_LAUNCH();
-            SgApply e;
-            e.A = w.A;
-            e.aff = w.aff;
-            e.out_hi = is_last ? nullptr : w.act[dst][0] + b0 * hw * c.cout;
-            e.out_lo = is_last ? nullptr : w.act[dst][1] + b0 * hw * c.cout;
-            e.out_f32 = (is_last && d_act_out) ? d_act_out + b0 * ld_act : nullptr;
-            e.ld = ld_act;
-            e.rgb_w = (is_last && d_rgb_out) ? v.rgb_w : nullptr;
-            e.rgb_b = v.rgb_b;
-            e.rgb_out = (is_last && d_rgb_out) ? d_rgb_out + b0 * hw * 3 : nullptr;
-            e.overflow = v.overflow;
-            const int64_t total = nb * hw * (c.cout / 4);
-            sg_apply_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(e, nb, hw, c.cout);
-            GSB_CHECK_LAUNCH();
-        }
+        sel[l] = l;
+        J.col0[l] = v.L[l].style_off;
+        J.lat[l] = w_layers == 1 ? 0 : l;
+        J.out[l] = w.S + v.L[l].style_off;
+        J.ld[l] = s_run;
     }
-    return GSB_OK;
+    if (int r = sg_style_launch(J, v, layers, sel, st)) return r;
+    return sg_run(v, w, layers, n_run, w.S, n, d_act_out, ld_act, d_rgb_out, st);
+}
+
+extern "C" int gsb_stylegan_forward_styled(const void *d_packed, const gsb_stylegan_layer *layers, int n_layers, int n_run, int dlatent,
+                                           const float *d_S, int64_t n, float *d_act_out, int64_t ld_act, float *d_rgb_out,
+                                           void *d_workspace, size_t workspace_bytes, gsb_stream_t stream) {
+    using namespace gsb;
+    if (int r = sg_run_check(layers, n_layers, n_run, dlatent, n, d_act_out, ld_act, d_rgb_out)) return r;
+    GSB_CHECK_ARG(d_packed && d_S && d_workspace && (d_act_out || d_rgb_out), "stylegan_forward_styled: null pointer");
+    if (n == 0) return GSB_OK;
+    SgView v = sg_view(const_cast<void *>(d_packed), layers, n_layers, dlatent);
+    SgWs w = sg_ws(d_workspace, layers, n_run, n, false);
+    if (workspace_bytes < w.bytes) {
+        set_error("stylegan_forward_styled: workspace too small (%zu < %zu)", workspace_bytes, w.bytes);
+        return GSB_ERR_WORKSPACE;
+    }
+    return sg_run(v, w, layers, n_run, d_S, n, d_act_out, ld_act, d_rgb_out, (cudaStream_t)stream);
+}
+
+extern "C" int gsb_stylegan_styles(const void *d_packed, const gsb_stylegan_layer *layers, int n_layers, int dlatent, const float *d_w,
+                                   int w_layers, int64_t n, const int *layer_idx, int n_idx, float *const *d_S, gsb_stream_t stream) {
+    using namespace gsb;
+    if (int r = sg_check(layers, n_layers, dlatent)) return r;
+    GSB_CHECK_ARG(d_packed && (d_w || n == 0) && n >= 0 && w_layers >= 1, "stylegan_styles: null pointer or bad n / w_layers");
+    GSB_CHECK_ARG(n_idx >= 1 && n_idx <= n_layers && layer_idx && d_S, "stylegan_styles: need 1..%d layers (n_idx = %d)", n_layers, n_idx);
+    SgStyleJob J;
+    J.w = d_w;
+    J.n = n;
+    J.dlatent = dlatent;
+    J.n_sel = n_idx;
+    SgView v = sg_view(const_cast<void *>(d_packed), layers, n_layers, dlatent);
+    for (int s = 0; s < n_idx; ++s) {
+        const int l = layer_idx[s];
+        GSB_CHECK_ARG(l >= 0 && l < n_layers, "stylegan_styles: layer index %d out of [0, %d)", l, n_layers);
+        GSB_CHECK_ARG(d_S[s] || n == 0, "stylegan_styles: null output for layer %d", l);
+        GSB_CHECK_ARG(w_layers == 1 || l < w_layers, "stylegan_styles: layer %d needs latent %d (w_layers = %d)", l, l, w_layers);
+        J.col0[s] = v.L[l].style_off;
+        J.lat[s] = w_layers == 1 ? 0 : l;
+        J.out[s] = d_S[s];
+        J.ld[s] = 2 * layers[l].cout;
+    }
+    if (n == 0) return GSB_OK;
+    if (int r = sg_latents_check(d_w, dlatent)) return r;
+    return sg_style_launch(J, v, layers, layer_idx, (cudaStream_t)stream);
 }
 
 extern "C" int gsb_stylegan_status(const void *d_packed, const gsb_stylegan_layer *layers, int n_layers, int dlatent, unsigned *h_flags) {

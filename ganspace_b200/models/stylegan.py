@@ -5,8 +5,8 @@
 The arithmetic is not here.  ``g_mapping`` runs the packed mapping kernels (csrc/mapping*.cu): v1's layer
 ``lrelu(x (W w_mul)^T + b 0.01)`` with ``w_mul = sqrt2 0.01 / sqrt512`` equals ``sqrt2 lrelu(x (W 0.01 / sqrt512)^T + (b / sqrt2) 0.01)``
 (leaky-ReLU is positively homogeneous), which is the StyleGAN2 layer the kernels compute, with the bias divided by sqrt2 on the host.
-The synthesis network runs in ``_native.PackedStyleGAN`` (csrc/stylegan.cu); a block's ``forward(_result=act)`` only hands the
-chain's result to the forward hooks.  Every other module has no stand-alone forward and raises.
+The synthesis network runs in ``_native.PackedStyleGAN`` (csrc/stylegan.cu); a block's ``forward(_result=act)`` and a StyleMod
+``lin``'s ``forward(_result=rows)`` only hand the chain's result to the forward hooks.  Every other module has no stand-alone forward and raises.
 """
 from __future__ import annotations
 
@@ -29,7 +29,9 @@ class _NotBuilt(nn.Module):
 
 
 class MyLinear(_NotBuilt):
-    """model.py:26-48, parameters only (equalized learning rate: ``weight * w_mul``, ``bias * b_mul``)."""
+    """model.py:26-48, parameters only (equalized learning rate: ``weight * w_mul``, ``bias * b_mul``).  A StyleMod's ``lin`` is a
+    style layer: StyleGAN.forward / partial_forward compute its rows [n, 2C] on the device and ``forward(_result=rows)`` hands them
+    to the forward hooks, returning what the hooks return (an edit replaces the style)."""
 
     def __init__(self, input_size, output_size, gain=2 ** 0.5, use_wscale=True, lrmul=1.0):
         super().__init__()
@@ -39,6 +41,11 @@ class MyLinear(_NotBuilt):
         self.weight = nn.Parameter(torch.randn(output_size, input_size) * init_std)
         self.bias = nn.Parameter(torch.zeros(output_size))
         self.b_mul = lrmul
+
+    def forward(self, *a, _result=None, **k):
+        if _result is None:
+            return super().forward(*a, **k)
+        return _result
 
 
 class Upscale2d(_NotBuilt):
@@ -216,6 +223,15 @@ class StyleGAN_G(nn.Sequential):
 
     def block_names(self):
         return [f"g_synthesis.blocks.{n}" for n in self.g_synthesis.blocks]
+
+    def style_layers(self):
+        """(name, chain layer, latent index, width 2C) of every style layer ``g_synthesis.blocks.RxR.epi{1,2}.style_mod.lin``, in
+        execution order: chain layer l is the l-th epilogue and reads latent l of an 18-latent input."""
+        out = []
+        for l, (_, epi, _, _) in enumerate(self.g_synthesis.layer_modules()):
+            blk = self.block_names()[l // 2]
+            out.append((f"{blk}.epi{l % 2 + 1}.style_mod.lin", l, l, epi.style_mod.lin.weight.shape[0]))
+        return out
 
 
 def synthesis_fill(net, seed):

@@ -167,6 +167,20 @@ class _StyledGenerator(_DeviceGenerator):
         # a module call: the mapping network's hooks fire here in W mode, as in the reference
         return self._mapping()(z) if self.w_primary else z
 
+    @staticmethod
+    def _hand_style(module, rows, name):
+        """Hands a style layer's rows [n, width] to its hooks and returns what the chain uses: the rows, or the hooks' edit (a
+        [1, width] edit applies to every sample, as nethook broadcasts it)."""
+        out = module(_result=rows)
+        if out is rows:
+            return rows
+        if out.dim() == 2 and out.shape[0] == 1:
+            out = out.expand(rows.shape[0], -1)
+        if tuple(out.shape) != tuple(rows.shape):
+            raise ValueError(f"an edit on '{name}' must keep the style's shape {tuple(rows.shape)} (or [1, {rows.shape[1]}]), got "
+                             f"{tuple(out.shape)}")
+        return out.to(device=rows.device, dtype=torch.float32).contiguous()
+
     def draw_z_async(self, n_samples, seed):
         """The Z stream of ``sample_latent(n_samples, seed=seed)`` generated on a side stream; returns a callable that makes
         the current stream wait for it and hands back z [n_samples, 512]."""
@@ -385,20 +399,6 @@ class StyleGAN2(_StyledGenerator):
                 rows[i] = self._hand_style(m, rows[i], name)
         return S, R
 
-    @staticmethod
-    def _hand_style(module, rows, name):
-        """Hands a style layer's rows [n, cin] to its hooks and returns what the chain uses: the rows, or the hooks' edit (a
-        [1, cin] edit applies to every sample, as nethook broadcasts it)."""
-        out = module(_result=rows)
-        if out is rows:
-            return rows
-        if out.dim() == 2 and out.shape[0] == 1:
-            out = out.expand(rows.shape[0], -1)
-        if tuple(out.shape) != tuple(rows.shape):
-            raise ValueError(f"an edit on '{name}' must keep the style's shape {tuple(rows.shape)} (or [1, {rows.shape[1]}]), got "
-                             f"{tuple(out.shape)}")
-        return out.to(device=rows.device, dtype=torch.float32).contiguous()
-
     def _reject_sub_module_hooks(self):
         guarded = getattr(self, "_guarded", None)
         if guarded is None:
@@ -615,7 +615,8 @@ class ProGAN(_DeviceGenerator):
 
 class StyleGAN(_StyledGenerator):
     """wrappers.py:270-436 (StyleGAN v1).  ``g_mapping`` runs the packed mapping kernels, the synthesis blocks the fused chain of
-    csrc/stylegan.cu.  Hookable layers: ``g_mapping`` and the blocks ``g_synthesis.blocks.RxR``.  Checkpoint:
+    csrc/stylegan.cu.  Hookable layers: ``g_mapping``, the blocks ``g_synthesis.blocks.RxR`` and their style layers
+    ``g_synthesis.blocks.RxR.epi{1,2}.style_mod.lin`` (the StyleMod rows [n, 2C], which an edit replaces).  Checkpoint:
     ``$GANCONTROL_CHECKPOINT_DIR/stylegan/stylegan_<class>_<res>.pt`` (the reference's ``StyleGAN_G`` state dict; there is no network
     to download it and no TensorFlow to convert a ``.pkl``); without one, ``random_init=<seed>`` (or env GANSPACE_B200_RANDOM_INIT)
     builds ``stylegan.random_init(seed)``."""
@@ -703,7 +704,7 @@ class StyleGAN(_StyledGenerator):
 
     # ---- synthesis ----------------------------------------------------------------------------------------
     def _hookable(self):
-        return ["g_mapping"] + self.model.block_names()
+        return ["g_mapping"] + self.model.block_names() + [t[0] for t in self.model.style_layers()]
 
     def _reject_sub_module_hooks(self):
         hookable = set(self._hookable())
@@ -721,27 +722,60 @@ class StyleGAN(_StyledGenerator):
         w = x if self.w_primary else self.model.g_mapping(x)
         return w.reshape(1, -1, 512).float()
 
-    def _run(self, w_layers, target, want_rgb):
+    def _run(self, w_layers, target, want_rgb, styles=None):
         """Blocks 0 .. ``target`` with the forward hooks of every hooked block on the way (a hooked earlier block gets its own run
-        of the chain); the image when ``want_rgb``."""
+        of the chain); the image when ``want_rgb``.  With ``styles`` ({layer: rows}, from ``_styles``) every run takes its styles
+        from there instead of from ``w_layers``."""
         packed = self.model.g_synthesis.packed()
         blocks = list(self.model.g_synthesis.blocks.values())
         names = self.model.block_names()
         w_layers = w_layers[:2 * (target + 1)] if w_layers.shape[0] > 1 else w_layers
+
+        def run(n_run, **kw):
+            if styles is not None:
+                return packed.forward_styled(styles, n_run, **kw)
+            return packed.forward(w_layers[:n_run] if w_layers.shape[0] > 1 else w_layers, n_run, **kw)
         hand = lambda i, act: self._hand_off(blocks[i], act, *packed.shapes[2 * i + 1], i < target or want_rgb, names[i])
         for i in [i for i in range(target) if len(blocks[i]._forward_hooks)]:
-            hand(i, packed.forward(w_layers[:2 * (i + 1)] if w_layers.shape[0] > 1 else w_layers, 2 * (i + 1))[0])
+            hand(i, run(2 * (i + 1))[0])
         want_act = len(blocks[target]._forward_hooks) > 0
-        act, rgb = packed.forward(w_layers, 2 * (target + 1), want_act=want_act or not want_rgb, want_rgb=want_rgb)
+        act, rgb = run(2 * (target + 1), want_act=want_act or not want_rgb, want_rgb=want_rgb)
         if want_act:
             hand(target, act)
         return rgb
 
+    # ---- style space: the StyleMod layers 'g_synthesis.blocks.RxR.epi{1,2}.style_mod.lin' --------------------
+    def _style_modules(self, n_run):
+        """(name, chain layer, module) of the style layers of chain layers 0 .. n_run-1."""
+        epis = self.model.g_synthesis.layer_modules()
+        return [(name, l, epis[l][1].style_mod.lin) for name, l, _, _ in self.model.style_layers() if l < n_run]
+
+    def _hooked_styles(self, n_run):
+        return any(len(m._forward_hooks) for *_, m in self._style_modules(n_run))
+
+    def _styles(self, w_layers, n_run, all_rows):
+        """Style rows for per-layer dlatents ``w_layers`` [Lw, n, 512], computed once; each hooked style layer of chain layers
+        0 .. n_run-1 fires once with its rows, and what it returns replaces them.  Returns {layer: rows} with the rows of every
+        layer in that range when ``all_rows`` (for chain runs), else of the hooked ones."""
+        mods = self._style_modules(n_run)
+        want = mods if all_rows else [t for t in mods if len(t[2]._forward_hooks)]
+        if not want:
+            return {}
+        S = self.model.g_synthesis.packed().styles(w_layers, [l for _, l, _ in want])
+        for name, l, m in want:
+            if len(m._forward_hooks):
+                S[l] = self._hand_style(m, S[l], name)
+        return S
+
     def forward(self, x):
-        """wrappers.py:375-377: images ``0.5 (torgb + 1)`` (unclamped) from one latent or a list of 18; hooked blocks fire."""
+        """wrappers.py:375-377: images ``0.5 (torgb + 1)`` (unclamped) from one latent or a list of 18; hooked blocks fire.  Hooked
+        style layers receive their rows once per call, and what their hooks return is what every chain run of the call uses."""
         self._reject_sub_module_hooks()
         w_layers = self._w_layers(x)
-        rgb = self._run(w_layers, len(self.model.g_synthesis.blocks) - 1, True)
+        target = len(self.model.g_synthesis.blocks) - 1
+        n_layers = 2 * (target + 1)
+        styles = self._styles(w_layers, n_layers, True) if self._hooked_styles(n_layers) else None
+        rgb = self._run(w_layers, target, True, styles=styles)
         return 0.5 * (rgb.permute(0, 3, 1, 2) + 1)
 
     def _target_block(self, layer_name):
@@ -753,6 +787,8 @@ class StyleGAN(_StyledGenerator):
         raise RuntimeError(f"Layer {layer_name} not encountered in partial_forward")
 
     def partial_forward(self, x, layer_name):
+        """wrappers.py:379-417: the blocks up to the one the stop rule names; hooks on the way fire.  To a style layer with no block
+        on the way hooked, only the hooked style layers' rows are computed (no synthesis launch)."""
         self._reject_sub_module_hooks()
         if not self.w_primary:
             x = [self.model.g_mapping(l) for l in x] if isinstance(x, list) else self.model.g_mapping(x)
@@ -763,7 +799,15 @@ class StyleGAN(_StyledGenerator):
             w_layers = self._w_layers(x)
         finally:
             self.w_primary = w_primary
-        self._run(w_layers, self._target_block(layer_name), False)
+        target = self._target_block(layer_name)
+        n_run = 2 * (target + 1)
+        if not (layer_name.endswith(".style_mod.lin") or self._hooked_styles(n_run)):
+            self._run(w_layers, target, False)
+            return
+        blocks_hooked = any(len(b._forward_hooks) for b in list(self.model.g_synthesis.blocks.values())[:target + 1])
+        styles = self._styles(w_layers, n_run, blocks_hooked)
+        if blocks_hooked:
+            self._run(w_layers, target, False, styles=styles)
 
     def feature_layout(self, layer_name):
         names = self.model.block_names()
