@@ -59,12 +59,13 @@ SIGNATURES = {
     "gsb_linreg_solve_pinv": (_I, [_P, _I, _I, _P, _P, _D, _P, _P]),
     "gsb_ipca_set_chain_mode": (_I, [_I]),
     "gsb_synthesis_packed_bytes": (_Z, [_P, _I, _I]),
-    "gsb_synthesis_pack": (_I, [_P, _I, _I, _P, _P, _Z, _P]),
-    "gsb_synthesis_workspace_bytes": (_Z, [_P, _I, _L]),
-    "gsb_synthesis_forward": (_I, [_P, _P, _I, _I, _I, _P, _L, _P, _L, _P, _Z, _P]),
+    "gsb_synthesis_pack": (_I, [_P, _I, _I, _P, _P, _P, _Z, _P]),
+    "gsb_synthesis_workspace_bytes": (_Z, [_P, _I, _I, _L]),
+    "gsb_synthesis_forward": (_I, [_P, _P, _I, _I, _I, _I, _P, _I, _L, _P, _L, _P, _P, _Z, _P]),
     "gsb_synthesis_status": (_I, [_P, _P, _I, _I, _P]),
-    "gsb_synthesis_render_workspace_bytes": (_Z, [_P, _I, _L, _I]),
-    "gsb_synthesis_render": (_I, [_P, _P, _I, _I, _I, _P, _I, _P, _I, _L, _P, _L, _P, _P, _Z, _P]),
+    "gsb_synthesis_styles": (_I, [_P, _P, _I, _I, _P, _I, _L, _P, _P, _P]),
+    "gsb_synthesis_forward_styled_workspace_bytes": (_Z, [_P, _I, _I, _L]),
+    "gsb_synthesis_forward_styled": (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _L, _P, _L, _P, _P, _Z, _P]),
     "gsb_progan_packed_bytes": (_Z, [_P, _I]),
     "gsb_progan_pack": (_I, [_P, _I, _P, _P, _P, _Z, _P]),
     "gsb_progan_workspace_bytes": (_Z, [_P, _I, _L]),
@@ -100,9 +101,6 @@ SIGNATURES = {
     "gsb_fbpca_workspace_bytes": (_Z, [_I, _I, _I]),
     "gsb_fbpca_solve": (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _Z, _P]),
     "gsb_fbpca_status": (_I, [_P, _I, _P, _P]),
-    "gsb_synthesis_styles": (_I, [_P, _P, _I, _I, _P, _I, _P, _I, _L, _P, _P, _P, _Z, _P]),
-    "gsb_synthesis_render_styled_workspace_bytes": (_Z, [_P, _I, _L]),
-    "gsb_synthesis_render_styled": (_I, [_P, _P, _I, _I, _I, _P, _I, _P, _P, _L, _P, _L, _P, _P, _Z, _P]),
 }
 
 
@@ -772,17 +770,38 @@ class _PackedTapGenerator:
         r, co = self.shapes[n_run - 1]
         return r * r * co
 
-    def _outputs(self, n: int, n_run: int, out, want_act: bool, want_rgb: bool, device):
-        """(activation rows [n, out_dims] -- ``out`` if given -- or None, image [n, res, res, 3] or None)."""
+    def _rgb_after(self, n_rgb: int) -> int:
+        """The layer whose resolution the image after ``n_rgb`` ToRGBs has: the last one (one ToRGB after the last layer)."""
+        return -1
+
+    def _outputs(self, n: int, n_run: int, out, want_act: bool, n_rgb: int, device):
+        """(activation rows [n, out_dims] -- ``out`` if given -- or None, image [n, res, res, 3] after ``n_rgb`` ToRGBs or None).
+        The generators with one ToRGB after the last layer pass their ``want_rgb``."""
         act = rgb = None
         if want_act:
             d = self.out_dims(n_run)
             act = torch.empty((n, d), dtype=torch.float32, device=device) if out is None else out
             assert act.is_cuda and act.dtype == torch.float32 and act.shape == (n, d) and act.stride(1) == 1
-        if want_rgb:
-            res = self.shapes[-1][0]
+        if n_rgb:
+            res = self.shapes[self._rgb_after(n_rgb)][0]
             rgb = torch.empty((n, res, res, 3), dtype=torch.float32, device=device)
         return act, rgb
+
+    @staticmethod
+    def _latents(w: torch.Tensor, dim: int) -> torch.Tensor:
+        """[Lw, n, dim] contiguous latents from ``w`` [n, dim] (one latent for every layer) or [Lw, n, dim] (per-layer latents)."""
+        assert w.is_cuda and w.dtype == torch.float32 and w.shape[-1] == dim and w.dim() in (2, 3)
+        return (w[None] if w.dim() == 2 else w).contiguous()
+
+    def _style_rows(self, S, keys):
+        """(the rows S[k] of the style layers ``keys``, contiguous; their row count n), each checked to be [n, style_width(k)] fp32
+        on the device."""
+        rows = [S[k] for k in keys]
+        n = int(rows[0].shape[0])
+        for k, t in zip(keys, rows):
+            assert t.is_cuda and t.dtype == torch.float32 and tuple(t.shape) == (n, self.style_width(k)), \
+                f"style layer {k}: rows [{n}, {self.style_width(k)}] fp32 on the device expected, got {tuple(t.shape)} {t.dtype}"
+        return [t.contiguous() for t in rows], n
 
     def check(self):
         flags = C.c_uint(0)
@@ -793,25 +812,32 @@ class _PackedTapGenerator:
 
 
 class PackedSynthesis(_PackedTapGenerator):
-    """StyleGAN2 synthesis layers conv1, convs.0 .. convs.k packed for the tap-GEMM kernels (gsb_synthesis_pack).
+    """StyleGAN2 synthesis layers conv1, convs.0 .. convs.k and the ToRGBs that follow them, packed for the tap-GEMM kernels
+    (gsb_synthesis_pack).
 
     ``layers``: dicts with conv_weight [co,ci,3,3], mod_weight [ci,S], mod_bias [ci], act_bias [co], noise [r,r],
-    noise_weight [1] (fp32 CUDA tensors) and upsample (bool), res_in (int), in execution order."""
+    noise_weight [1] (fp32 CUDA tensors) and upsample (bool), res_in (int), in execution order.  ``rgbs``: dicts with conv_weight
+    [3,ci], mod_weight [ci,S], mod_bias [ci] and bias [3] of to_rgb1, to_rgbs.0, ...: the (len(layers) + 1) // 2 that follow the
+    layers (ToRGB j follows layer 2j).  Style layers are keyed by their position in execution order (conv1, to_rgb1, convs.0,
+    convs.1, to_rgbs.0, ...), the order of ``Generator.style_layers()``."""
 
     NAME = "synthesis"
 
-    def __init__(self, const_input: torch.Tensor, layers, style_dim: int):
+    def __init__(self, const_input: torch.Tensor, layers, rgbs, style_dim: int):
         lib = load()
         self.device = require_cuda(const_input.device)
         self.style_dim = int(style_dim)
-        self.n_layers = len(layers)
-        self._keep = []
+        self.n_layers, self.n_rgb = len(layers), (len(layers) + 1) // 2
+        assert len(rgbs) == self.n_rgb, f"{self.n_layers} layers are followed by {self.n_rgb} ToRGBs, got {len(rgbs)}"
         self.desc = (StyledConvDesc * self.n_layers)()
+        self.rgb_desc = (ToRGBDesc * self.n_rgb)()
         self.shapes = []                        # (res_out, cout) per layer
+        self.slots = []                         # style layer -> ("conv", l) or ("rgb", j), in execution order
         f32 = lambda t: t.detach().to(self.device, torch.float32).contiguous()
+        keep = []
         for i, L in enumerate(layers):
             ts = {k: f32(L[k]) for k in ("conv_weight", "mod_weight", "mod_bias", "act_bias", "noise", "noise_weight")}
-            self._keep.append(ts)
+            keep.append(ts)
             co, ci = ts["conv_weight"].shape[0], ts["conv_weight"].shape[1]
             assert ts["conv_weight"].shape == (co, ci, 3, 3) and ts["mod_weight"].shape == (ci, self.style_dim)
             res_in, up = int(L["res_in"]), bool(L["upsample"])
@@ -822,142 +848,98 @@ class PackedSynthesis(_PackedTapGenerator):
                 setattr(d, k, t.data_ptr())
             d.cin, d.cout, d.upsample, d.res_in = ci, co, int(up), res_in
             self.shapes.append((res_out, co))
+            self.slots.append(("conv", i))
+            if i % 2 == 0:
+                self.slots.append(("rgb", i // 2))
+        for j, R in enumerate(rgbs):
+            ts = {k: f32(R[k]) for k in ("conv_weight", "mod_weight", "mod_bias", "bias")}
+            keep.append(ts)
+            ci = self.shapes[2 * j][1]
+            assert ts["conv_weight"].numel() == 3 * ci and ts["mod_weight"].shape == (ci, self.style_dim) and ts["bias"].numel() == 3
+            for k, t in ts.items():
+                setattr(self.rgb_desc[j], k, t.data_ptr())
+            self.rgb_desc[j].cin = ci
+        self.slot_of = {s: k for k, s in enumerate(self.slots)}
         cst = f32(const_input).reshape(-1, 4, 4)
         self._pack(lib.gsb_synthesis_packed_bytes(self.desc, self.n_layers, self.style_dim),
-                   lambda packed, nbytes, st: lib.gsb_synthesis_pack(self.desc, self.n_layers, self.style_dim, _ptr(cst), packed,
-                                                                     nbytes, st))
+                   lambda packed, nbytes, st: lib.gsb_synthesis_pack(self.desc, self.n_layers, self.style_dim, self.rgb_desc, _ptr(cst),
+                                                                     packed, nbytes, st))
 
-    def forward(self, w: torch.Tensor, n_run: int, out: torch.Tensor = None) -> torch.Tensor:
-        """Activation of layer ``n_run - 1`` for w[n, style_dim]: fp32 NHWC rows [n, res*res*cout] (``out`` may be a
-        row-strided 2-D view, e.g. the batch rows of the large-d IPCA buffer)."""
+    def _rgb_after(self, n_rgb: int) -> int:
+        return 2 * (n_rgb - 1)
+
+    def style_width(self, k: int) -> int:
+        """Width of style layer ``k``'s rows: the input channels of its StyledConv or ToRGB."""
+        chain, i = self.slots[k]
+        return self.desc[i].cin if chain == "conv" else self.shapes[2 * i][1]
+
+    def forward(self, w: torch.Tensor, n_run: int, out: torch.Tensor = None, want_act: bool = True, n_rgb: int = 0):
+        """Layers 0 .. n_run-1 and ToRGBs 0 .. n_rgb-1 (n_rgb <= (n_run + 1) // 2) for latents ``w`` [n, style_dim] (one latent for
+        every layer) or [Lw, n, style_dim] (layer l reads latent min(l, Lw-1), ToRGB j latent min(2j+1, Lw-1)).  Returns (activation
+        of layer n_run-1 as fp32 NHWC rows [n, res*res*cout] or None, skip image after ToRGB n_rgb-1 as fp32 NHWC [n, res, res, 3]
+        or None).  ``out`` may be a row-strided 2-D view, e.g. the batch rows of the large-d IPCA buffer."""
         lib = load()
-        assert w.is_cuda and w.dtype == torch.float32 and w.dim() == 2 and w.shape[1] == self.style_dim
-        w = w.contiguous()
-        n = w.shape[0]
-        out = self._outputs(n, n_run, out, True, False, w.device)[0]
-        ws_bytes = lib.gsb_synthesis_workspace_bytes(self.desc, n_run, n)
-        ws = scratch.get("synthesis", ws_bytes, w.device)
-        with torch.cuda.device(w.device), instrument.section("synthesis"):
-            _check(lib.gsb_synthesis_forward(_ptr(self.packed), self.desc, self.n_layers, n_run, self.style_dim, _ptr(w), n,
-                                             C.c_void_p(out.data_ptr()), out.stride(0), _ptr(ws), ws.numel(), _stream()),
-                   "gsb_synthesis_forward")
-        # per layer: 4 style/demod launches; per chunk of samples: 1 GEMM + 1 (stride-1) or 2 (upsample) epilogue launches
-        launches = 1
+        w3 = self._latents(w, self.style_dim)
+        Lw, n = int(w3.shape[0]), int(w3.shape[1])
+        act, rgb = self._outputs(n, n_run, out, want_act, n_rgb, self.device)
+        ws = scratch.get("synthesis", lib.gsb_synthesis_workspace_bytes(self.desc, n_run, n_rgb, n), self.device)
+        with torch.cuda.device(self.device), instrument.section("synthesis"):
+            _check(lib.gsb_synthesis_forward(_ptr(self.packed), self.desc, self.n_layers, n_run, n_rgb, self.style_dim, _ptr(w3), Lw, n,
+                                             C.c_void_p(act.data_ptr() if act is not None else 0), act.stride(0) if act is not None else 0,
+                                             _ptr(rgb), _ptr(ws), ws.numel(), _stream()), "gsb_synthesis_forward")
+        self._count(n, n_run, n_rgb)
+        return act, rgb
+
+    def styles(self, w: torch.Tensor, keys):
+        """The style-space rows (gsb_synthesis_styles): for latents ``w`` as in ``forward``, the modulation output [n, width] of every
+        style layer in ``keys`` (positions in execution order).  Returns {key: rows}.  The launches are the chain's own style stage,
+        so at the same n the rows are the ones it consumes."""
+        lib = load()
+        w3 = self._latents(w, self.style_dim)
+        Lw, n = int(w3.shape[0]), int(w3.shape[1])
+        keys = sorted(set(int(k) for k in keys))
+        assert all(0 <= k < len(self.slots) for k in keys), keys
+        S = {k: torch.empty((n, self.style_width(k)), dtype=torch.float32, device=self.device) for k in keys}
+        ptrs = {"conv": [None] * self.n_layers, "rgb": [None] * self.n_rgb}
+        for k in keys:
+            chain, i = self.slots[k]
+            ptrs[chain][i] = S[k].data_ptr()
+        with torch.cuda.device(self.device), instrument.section("styles"):
+            _check(lib.gsb_synthesis_styles(_ptr(self.packed), self.desc, self.n_layers, self.style_dim, _ptr(w3), Lw, n,
+                                            (C.c_void_p * self.n_layers)(*ptrs["conv"]), (C.c_void_p * self.n_rgb)(*ptrs["rgb"]),
+                                            _stream()), "gsb_synthesis_styles")
+        instrument.count(len(keys))
+        instrument.add_rows("styles", n)
+        return S
+
+    def forward_styled(self, S, n_run: int, out: torch.Tensor = None, want_act: bool = True, n_rgb: int = 0):
+        """``forward`` on caller-given styles (gsb_synthesis_forward_styled): ``S`` {style layer: rows [n, width] fp32} holding the
+        layers 0 .. n_run-1 and the ToRGBs 0 .. n_rgb-1.  Same outputs as ``forward``."""
+        lib = load()
+        keys = [self.slot_of["conv", l] for l in range(n_run)] + [self.slot_of["rgb", j] for j in range(n_rgb)]
+        rows, n = self._style_rows(S, keys)
+        act, rgb = self._outputs(n, n_run, out, want_act, n_rgb, self.device)
+        S_ptrs = (C.c_void_p * n_run)(*[t.data_ptr() for t in rows[:n_run]])
+        R_ptrs = (C.c_void_p * max(1, n_rgb))(*[t.data_ptr() for t in rows[n_run:]])
+        ws = scratch.get("synthesis", lib.gsb_synthesis_forward_styled_workspace_bytes(self.desc, n_run, n_rgb, n), self.device)
+        with torch.cuda.device(self.device), instrument.section("synthesis"):
+            _check(lib.gsb_synthesis_forward_styled(_ptr(self.packed), self.desc, self.n_layers, n_run, n_rgb, self.style_dim, S_ptrs,
+                                                    R_ptrs, n, C.c_void_p(act.data_ptr() if act is not None else 0),
+                                                    act.stride(0) if act is not None else 0, _ptr(rgb), _ptr(ws), ws.numel(), _stream()),
+                   "gsb_synthesis_forward_styled")
+        self._count(n, n_run, n_rgb)
+        return act, rgb
+
+    def _count(self, n, n_run, n_rgb):
+        # per layer: 4 style/demod launches; per chunk of samples: 1 GEMM + 1 (stride-1) or 2 (upsample) epilogue launches;
+        # per ToRGB: its style and its skip-image launch
+        launches = 1 + 2 * n_rgb
         for i in range(n_run):
             res_in = self.desc[i].res_in
             chunks = -(-n // max(1, 4096 // (res_in * res_in)))
             launches += 4 + chunks * (3 if self.desc[i].upsample else 2)
         instrument.count(launches)
         instrument.add_rows("synthesis", n)
-        return out
-
-    def render(self, w_layers: torch.Tensor, n_run: int, rgbs, want_act: bool = False):
-        """Generator.forward on the fused chain (gsb_synthesis_render): ``w_layers`` [Lw, n, style_dim] per-layer latents (Lw = 1:
-        one global latent), ``rgbs``: list of dicts (conv_weight [3,cin], mod_weight, mod_bias, bias [3]) for to_rgb1,
-        to_rgbs.0, ... up to the one that follows layer n_run-1 or earlier.  Returns (activation of layer n_run-1 as fp32 NHWC
-        rows or None, skip image after the last ToRGB as fp32 NHWC [n, res, res, 3] or None)."""
-        lib = load()
-        w_layers = self._latents(w_layers)
-        Lw, n = int(w_layers.shape[0]), int(w_layers.shape[1])
-        descs, keep = self._rgb_descs(rgbs)
-        act, rgb = self._render_outputs(n, n_run, len(rgbs), want_act)
-        ws_bytes = lib.gsb_synthesis_render_workspace_bytes(self.desc, n_run, n, self.style_dim)
-        ws = scratch.get("synthesis", ws_bytes, self.device)
-        with torch.cuda.device(self.device), instrument.section("synthesis"):
-            _check(lib.gsb_synthesis_render(_ptr(self.packed), self.desc, self.n_layers, n_run, self.style_dim, descs, len(rgbs),
-                                            _ptr(w_layers), Lw, n, _ptr(act), act.stride(0) if act is not None else 0, _ptr(rgb),
-                                            _ptr(ws), ws.numel(), _stream()), "gsb_synthesis_render")
-            if keep:
-                torch.cuda.current_stream().synchronize()      # the temporary parameter copies may be freed after this
-        instrument.count(1)
-        instrument.add_rows("synthesis", n)
-        return act, rgb
-
-    def styles(self, w_layers: torch.Tensor, conv_idx, rgb_idx=(), rgbs=()):
-        """The style-space rows (gsb_synthesis_styles): for per-layer latents ``w_layers`` [Lw, n, style_dim] (entries as in
-        ``render``), the modulation output [n, cin] of every chain layer in ``conv_idx`` and of every ToRGB in ``rgb_idx`` (0 =
-        to_rgb1, j + 1 = to_rgbs.j; ``rgbs`` describes ToRGBs 0 .. max(rgb_idx) as in ``render``).  Returns ({layer: rows},
-        {ToRGB: rows}).  The launches are the chain's own style stage, so at the same n the rows are the ones it consumes."""
-        lib = load()
-        w_layers = self._latents(w_layers)
-        Lw, n = int(w_layers.shape[0]), int(w_layers.shape[1])
-        conv_idx, rgb_idx = sorted(set(conv_idx)), sorted(set(rgb_idx))
-        assert all(0 <= l < self.n_layers for l in conv_idx) and all(0 <= j < len(rgbs) for j in rgb_idx)
-        new = lambda c: torch.empty((n, c), dtype=torch.float32, device=self.device)
-        S = {l: new(self.desc[l].cin) for l in conv_idx}
-        R = {j: new(self.desc[2 * j].cout) for j in rgb_idx}
-        S_ptrs = (C.c_void_p * self.n_layers)(*[S[l].data_ptr() if l in S else None for l in range(self.n_layers)])
-        n_rgb = rgb_idx[-1] + 1 if rgb_idx else 0
-        R_ptrs = (C.c_void_p * max(1, n_rgb))(*[R[j].data_ptr() if j in R else None for j in range(n_rgb)])
-        descs, keep = self._rgb_descs(list(rgbs)[:n_rgb])
-        ws = scratch.get("synthesis_styles", max([self.desc[2 * j].cout for j in rgb_idx], default=0) * self.style_dim * 4,
-                         self.device)
-        with torch.cuda.device(self.device), instrument.section("styles"):
-            _check(lib.gsb_synthesis_styles(_ptr(self.packed), self.desc, self.n_layers, self.style_dim, descs, n_rgb, _ptr(w_layers),
-                                            Lw, n, S_ptrs, R_ptrs, _ptr(ws), ws.numel(), _stream()), "gsb_synthesis_styles")
-            if keep:
-                torch.cuda.current_stream().synchronize()
-        instrument.count(len(conv_idx) + 2 * len(rgb_idx))
-        instrument.add_rows("styles", n)
-        return S, R
-
-    def render_styled(self, S, rgb_S, n_run: int, rgbs, want_act: bool = False):
-        """``render`` on caller-given styles (gsb_synthesis_render_styled): ``S[l]`` [n, cin] for the chain layers 0 .. n_run-1 and
-        ``rgb_S[j]`` [n, cin] for every ToRGB in ``rgbs`` (only their conv_weight and bias are read).  Same outputs as ``render``."""
-        lib = load()
-        S = [self._style_rows(t, self.desc[l].cin) for l, t in enumerate(S[:n_run])]
-        assert len(S) == n_run and len(rgb_S) == len(rgbs)
-        n = S[0].shape[0]
-        rgb_S = [self._style_rows(t, self.desc[2 * j].cout) for j, t in enumerate(rgb_S)]
-        assert all(t.shape[0] == n for t in S + rgb_S), "every style needs the same number of rows"
-        descs, keep = self._rgb_descs(rgbs)
-        act, rgb = self._render_outputs(n, n_run, len(rgbs), want_act)
-        S_ptrs = (C.c_void_p * n_run)(*[t.data_ptr() for t in S])
-        R_ptrs = (C.c_void_p * max(1, len(rgb_S)))(*[t.data_ptr() for t in rgb_S])
-        ws_bytes = lib.gsb_synthesis_render_styled_workspace_bytes(self.desc, n_run, n)
-        ws = scratch.get("synthesis", ws_bytes, self.device)
-        with torch.cuda.device(self.device), instrument.section("synthesis"):
-            _check(lib.gsb_synthesis_render_styled(_ptr(self.packed), self.desc, self.n_layers, n_run, self.style_dim, descs, len(rgbs),
-                                                   S_ptrs, R_ptrs, n, _ptr(act), act.stride(0) if act is not None else 0, _ptr(rgb),
-                                                   _ptr(ws), ws.numel(), _stream()), "gsb_synthesis_render_styled")
-            if keep:
-                torch.cuda.current_stream().synchronize()
-        instrument.count(1)
-        instrument.add_rows("synthesis", n)
-        return act, rgb
-
-    def _latents(self, w_layers):
-        assert w_layers.is_cuda and w_layers.dtype == torch.float32 and w_layers.dim() == 3 and w_layers.shape[2] == self.style_dim
-        return w_layers.contiguous()
-
-    def _style_rows(self, t, width):
-        assert t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and t.shape[1] == width, \
-            f"style rows [n, {width}] fp32 on the device expected, got {tuple(t.shape)} {t.dtype}"
-        return t.contiguous()
-
-    def _rgb_descs(self, rgbs):
-        """(ToRGBDesc array, the fp32 device copies it points to) for the ToRGB dicts ``rgbs``; parameters that already are
-        contiguous fp32 device tensors are used in place."""
-        keep = []
-        descs = (ToRGBDesc * max(1, len(rgbs)))()
-        for j, r in enumerate(rgbs):
-            ts = {k: r[k].detach().to(self.device, torch.float32).contiguous() for k in ("conv_weight", "mod_weight", "mod_bias", "bias")}
-            keep += [t for k, t in ts.items() if t.data_ptr() != r[k].data_ptr()]
-            cin = ts["conv_weight"].shape[-1]
-            assert ts["conv_weight"].numel() == 3 * cin and ts["bias"].numel() == 3
-            for k, t in ts.items():
-                setattr(descs[j], k, t.data_ptr())
-            descs[j].cin = int(cin)
-        return descs, keep
-
-    def _render_outputs(self, n, n_run, n_rgb, want_act):
-        act = rgb = None
-        if want_act:
-            act = torch.empty((n, self.out_dims(n_run)), dtype=torch.float32, device=self.device)
-        if n_rgb:
-            res = self.shapes[2 * (n_rgb - 1)][0]
-            rgb = torch.empty((n, res, res, 3), dtype=torch.float32, device=self.device)
-        return act, rgb
 
     def _status(self, flags):
         return load().gsb_synthesis_status(_ptr(self.packed), self.desc, self.n_layers, self.style_dim, flags)
@@ -1064,8 +1046,7 @@ class PackedStyleGAN(_PackedTapGenerator):
         [n, res, res, 3] or None; the image needs n_run == n_layers).  ``out`` may be a row-strided 2-D view, e.g. the batch rows
         of the large-d IPCA buffer."""
         lib = load()
-        assert w.is_cuda and w.dtype == torch.float32 and w.shape[-1] == self.dlatent and w.dim() in (2, 3)
-        w3 = (w[None] if w.dim() == 2 else w).contiguous()
+        w3 = self._latents(w, self.dlatent)
         Lw, n = int(w3.shape[0]), int(w3.shape[1])
         act, rgb = self._outputs(n, n_run, out, want_act, want_rgb, w.device)
         if n == 0:
@@ -1088,8 +1069,7 @@ class PackedStyleGAN(_PackedTapGenerator):
         layer in ``layers``.  Returns {layer: rows}.  The launch is the chain's own style GEMM, so the rows are bit-identical to the
         ones ``forward`` consumes."""
         lib = load()
-        assert w.is_cuda and w.dtype == torch.float32 and w.shape[-1] == self.dlatent and w.dim() in (2, 3)
-        w3 = (w[None] if w.dim() == 2 else w).contiguous()
+        w3 = self._latents(w, self.dlatent)
         Lw, n = int(w3.shape[0]), int(w3.shape[1])
         layers = sorted(set(int(l) for l in layers))
         assert layers and all(0 <= l < self.n_layers and (Lw == 1 or l < Lw) for l in layers), layers
@@ -1107,11 +1087,7 @@ class PackedStyleGAN(_PackedTapGenerator):
         """``forward`` on caller-given styles (gsb_stylegan_forward_styled): ``S[l]`` [n, 2 cout] fp32 for the layers 0 .. n_run-1
         (a list or a dict by layer).  Same outputs as ``forward``."""
         lib = load()
-        rows = [S[l] for l in range(n_run)]
-        n = int(rows[0].shape[0])
-        for l, t in enumerate(rows):
-            assert t.is_cuda and t.dtype == torch.float32 and tuple(t.shape) == (n, self.style_width(l)), \
-                f"layer {l}: style rows [{n}, {self.style_width(l)}] fp32 on the device expected, got {tuple(t.shape)} {t.dtype}"
+        rows, n = self._style_rows(S, range(n_run))
         act, rgb = self._outputs(n, n_run, out, want_act, want_rgb, self.device)
         if n == 0:
             return act, rgb

@@ -26,6 +26,7 @@
 namespace gsb {
 
 constexpr int SY_MAX_LAYERS = 24;
+constexpr int SY_MAX_RGB = SY_MAX_LAYERS / 2 + 1;
 constexpr int SY_CHUNK_ROWS = 2048;       // GEMM rows per launch: 2048 x 9*512 fp32 tap planes = 38 MB (fits the 50 MB L2)
 
 // ---- packed layout ----------------------------------------------------------------------------------------
@@ -38,14 +39,22 @@ struct SynthLayerView {
     float *actb;              // [cout]
     float *noise;             // [res_out^2]  noise_weight * noise
 };
+struct SynthRgbView {         // the ToRGB that follows layer 2j (cin = that layer's cout)
+    float *modw;              // [cin, style_dim]  modulation.weight * (1/sqrt(style_dim))
+    float *modb;              // [cin]
+    float *convw;             // [3, cin]  conv.weight (unscaled)
+    float *bias;              // [3]
+};
 struct SynthView {
     float *const_nhwc;        // [16, c0]
     float *zeros;             // [max channels]
     unsigned *overflow;
     SynthLayerView L[SY_MAX_LAYERS];
+    SynthRgbView R[SY_MAX_RGB];
     size_t bytes;
 };
 static int res_out_of(const gsb_styled_conv &l) { return l.upsample ? 2 * l.res_in : l.res_in; }
+static int rgbs_of(int n_layers) { return (n_layers + 1) / 2; }    // ToRGB j follows layer 2j
 
 static SynthView synth_view(void *base, const gsb_styled_conv *layers, int n_layers, int style_dim) {
     SynthView v;
@@ -68,6 +77,13 @@ static SynthView synth_view(void *base, const gsb_styled_conv *layers, int n_lay
         v.L[l].modb = (float *)take((size_t)c.cin * 4);
         v.L[l].actb = (float *)take((size_t)c.cout * 4);
         v.L[l].noise = (float *)take((size_t)ro * ro * 4);
+    }
+    for (int j = 0; j < rgbs_of(n_layers); ++j) {
+        const size_t cin = layers[2 * j].cout;
+        v.R[j].modw = (float *)take(cin * style_dim * 4);
+        v.R[j].modb = (float *)take(cin * 4);
+        v.R[j].convw = (float *)take(3 * cin * 4);
+        v.R[j].bias = (float *)take(3 * 4);
     }
     v.bytes = off;
     return v;
@@ -310,25 +326,23 @@ sy_blur_epilogue_kernel(const float *__restrict__ T, int64_t nb, int H2, int W2,
 }
 
 // ---- workspace --------------------------------------------------------------------------------------------
-constexpr int SY_MAX_RGB = SY_MAX_LAYERS / 2 + 1;
 struct SynthWs {
     float *S[SY_MAX_LAYERS], *D[SY_MAX_LAYERS];
     float *s2;
     __half *act[2][2];     // [ping-pong][hi/lo]
     float *Y, *T;
     unsigned *queue;        // tile queue of the tap GEMM launches
-    float *rgb[2];          // render path: skip images (ping-pong)
-    float *rgb_s[SY_MAX_RGB], *rgb_modw;   // with the style stage: ToRGB styles, scaled ToRGB modulation weight
+    float *rgb[2];          // with ToRGBs: skip images (ping-pong)
+    float *rgb_s[SY_MAX_RGB];   // with the style stage: ToRGB styles
     size_t bytes;
 };
 static int chunk_samples(const gsb_styled_conv &c) {
     int spc = SY_CHUNK_ROWS / (c.res_in * c.res_in);
     return spc < 1 ? 1 : spc;
 }
-// own_styles: the workspace also holds the styles S[l] (and, with_rgb, those of the ToRGBs that can follow layers[0..n_run)) that
-// the style stage writes; without it the caller passes them (gsb_synthesis_render_styled)
-static SynthWs synth_ws(void *base, const gsb_styled_conv *layers, int n_run, int64_t n, bool with_rgb = false, int style_dim = 0,
-                        bool own_styles = true) {
+// own_styles: the workspace also holds the styles S[l] and rgb_s[j] (j < n_rgb) that the style stage writes; without it the caller
+// passes them (gsb_synthesis_forward_styled)
+static SynthWs synth_ws(void *base, const gsb_styled_conv *layers, int n_run, int n_rgb, int64_t n, bool own_styles) {
     SynthWs w;
     char *p = reinterpret_cast<char *>(base);
     size_t off = 0;
@@ -355,45 +369,24 @@ static SynthWs synth_ws(void *base, const gsb_styled_conv *layers, int n_run, in
     w.Y = (float *)take(y_elems * 4);
     w.T = (float *)take((t_elems ? t_elems : 64) * 4);
     w.queue = (unsigned *)take(sizeof(unsigned));
-    w.rgb[0] = w.rgb[1] = w.rgb_modw = nullptr;
+    w.rgb[0] = w.rgb[1] = nullptr;
     for (int j = 0; j < SY_MAX_RGB; ++j) w.rgb_s[j] = nullptr;
-    if (with_rgb) {
+    if (n_rgb > 0) {
         const int ro = res_out_of(layers[n_run - 1]);
         for (int a = 0; a < 2; ++a) w.rgb[a] = (float *)take((size_t)n * ro * ro * 3 * 4);
-        if (own_styles) {
-            size_t cm = 0;
-            for (int j = 0; 2 * j < n_run; ++j) {
-                w.rgb_s[j] = (float *)take((size_t)n * layers[2 * j].cout * 4);
-                cm = cm > (size_t)layers[2 * j].cout ? cm : (size_t)layers[2 * j].cout;
-            }
-            w.rgb_modw = (float *)take(cm * (size_t)style_dim * 4);
-        }
+        for (int j = 0; own_styles && j < n_rgb; ++j) w.rgb_s[j] = (float *)take((size_t)n * layers[2 * j].cout * 4);
     }
     w.bytes = off;
     return w;
 }
 
-// ---- style stage (model.py:226,234) ----------------------------------------------------------------------
-// StyledConv layer l: s = w modw^T + modb with the modulation weight scaled at pack time
-static int conv_style(const SynthView &v, const gsb_styled_conv &c, int l, const float *w, int64_t n, int style_dim, float *s,
-                      gsb_stream_t stream) {
-    return sy_linear(w, v.L[l].modw, v.L[l].modb, s, n, c.cin, style_dim, stream);
-}
-// ToRGB: the modulation weight is scaled per call into modw (cin * style_dim floats)
-static int rgb_style(const gsb_to_rgb &t, const float *w, int64_t n, int style_dim, float *modw, float *s, gsb_stream_t stream) {
-    const float mscale = (float)(1.0 / sqrt((double)style_dim));
-    scale_copy_kernel<<<64, 256, 0, (cudaStream_t)stream>>>(t.mod_weight, (int64_t)t.cin * style_dim, mscale, nullptr, modw);
-    GSB_CHECK_LAUNCH();
-    return sy_linear(w, modw, t.mod_bias, s, n, t.cin, style_dim, stream);
-}
-// rgbs[j] follows layer 2j of layers[0..n_following); need_mod: its modulation parameters are read
-static int check_rgbs(const gsb_styled_conv *layers, int n_following, const gsb_to_rgb *rgbs, int n_rgb, bool need_mod) {
-    GSB_CHECK_ARG(n_rgb >= 0 && n_rgb <= SY_MAX_RGB && (n_rgb == 0 || rgbs), "synthesis: bad ToRGB list");
-    for (int j = 0; j < n_rgb; ++j) {
+// ToRGB j follows layer 2j of layers[0..n_following): its cin is that layer's cout, a power of two (the epilogue's lane reduction)
+static int check_rgbs(const gsb_styled_conv *layers, int n_following, const gsb_to_rgb *rgbs) {
+    GSB_CHECK_ARG(rgbs, "synthesis: null ToRGB list");
+    for (int j = 0; j < rgbs_of(n_following); ++j) {
         const gsb_to_rgb &t = rgbs[j];
-        GSB_CHECK_ARG(2 * j < n_following, "synthesis: ToRGB %d has no layer %d to follow", j, 2 * j);
         const int c = layers[2 * j].cout;
-        GSB_CHECK_ARG(t.conv_weight && t.bias && (!need_mod || (t.mod_weight && t.mod_bias)) && t.cin == c && (c & (c - 1)) == 0,
+        GSB_CHECK_ARG(t.conv_weight && t.bias && t.mod_weight && t.mod_bias && t.cin == c && (c & (c - 1)) == 0,
                       "synthesis: ToRGB %d does not match layer %d (cin=%d, cout=%d)", j, 2 * j, t.cin, c);
     }
     return GSB_OK;
@@ -407,10 +400,11 @@ extern "C" size_t gsb_synthesis_packed_bytes(const gsb_styled_conv *layers, int 
     return gsb::synth_view(nullptr, layers, n_layers, style_dim).bytes;
 }
 
-extern "C" int gsb_synthesis_pack(const gsb_styled_conv *layers, int n_layers, int style_dim, const float *d_const_input,
-                                  void *d_packed, size_t packed_bytes, gsb_stream_t stream) {
+extern "C" int gsb_synthesis_pack(const gsb_styled_conv *layers, int n_layers, int style_dim, const gsb_to_rgb *rgbs,
+                                  const float *d_const_input, void *d_packed, size_t packed_bytes, gsb_stream_t stream) {
     using namespace gsb;
     if (int r = check_layers(layers, n_layers, style_dim)) return r;
+    if (int r = check_rgbs(layers, n_layers, rgbs)) return r;
     GSB_CHECK_ARG(d_const_input && d_packed, "synthesis_pack: null pointer");
     SynthView v = synth_view(d_packed, layers, n_layers, style_dim);
     if (packed_bytes < v.bytes) { set_error("synthesis_pack: buffer too small (%zu < %zu)", packed_bytes, v.bytes); return GSB_ERR_WORKSPACE; }
@@ -419,12 +413,12 @@ extern "C" int gsb_synthesis_pack(const gsb_styled_conv *layers, int n_layers, i
     const int c0 = layers[0].cin;
     const_nhwc_kernel<<<8, 256, 0, st>>>(d_const_input, c0, v.const_nhwc);
     GSB_CHECK_LAUNCH();
+    const float mscale = (float)(1.0 / sqrt((double)style_dim));                  // EqualLinear.scale, lr_mul = 1 (model.py:143)
     for (int l = 0; l < n_layers; ++l) {
         const gsb_styled_conv &c = layers[l];
         GSB_CHECK_ARG(c.conv_weight && c.mod_weight && c.mod_bias && c.act_bias && c.noise && c.noise_weight,
                       "synthesis_pack: layer %d has a null parameter pointer", l);
         const float scale = (float)(1.0 / sqrt((double)c.cin * 9.0));           // ModulatedConv2d.scale (model.py:219-220)
-        const float mscale = (float)(1.0 / sqrt((double)style_dim));              // EqualLinear.scale, lr_mul = 1 (model.py:143)
         if (int r = tc_split_weight(c.conv_weight, c.cout, c.cin, 9, scale, false, 9 * c.cout, v.L[l].w_hi, v.L[l].w_lo, v.L[l].scal,
                                     v.L[l].wsq, st)) return r;
         scale_copy_kernel<<<128, 256, 0, st>>>(c.mod_weight, (int64_t)c.cin * style_dim, mscale, nullptr, v.L[l].modw);
@@ -437,22 +431,33 @@ extern "C" int gsb_synthesis_pack(const gsb_styled_conv *layers, int n_layers, i
         scale_copy_kernel<<<64, 256, 0, st>>>(c.noise, (int64_t)ro * ro, 1.0f, c.noise_weight, v.L[l].noise);
         GSB_CHECK_LAUNCH();
     }
+    for (int j = 0; j < rgbs_of(n_layers); ++j) {
+        const gsb_to_rgb &t = rgbs[j];
+        scale_copy_kernel<<<64, 256, 0, st>>>(t.mod_weight, (int64_t)t.cin * style_dim, mscale, nullptr, v.R[j].modw);
+        GSB_CHECK_LAUNCH();
+        scale_copy_kernel<<<4, 256, 0, st>>>(t.mod_bias, t.cin, 1.0f, nullptr, v.R[j].modb);
+        GSB_CHECK_LAUNCH();
+        scale_copy_kernel<<<4, 256, 0, st>>>(t.conv_weight, 3 * t.cin, 1.0f, nullptr, v.R[j].convw);
+        GSB_CHECK_LAUNCH();
+        scale_copy_kernel<<<1, 32, 0, st>>>(t.bias, 3, 1.0f, nullptr, v.R[j].bias);
+        GSB_CHECK_LAUNCH();
+    }
     return GSB_OK;
 }
 
-extern "C" size_t gsb_synthesis_workspace_bytes(const gsb_styled_conv *layers, int n_run, int64_t n) {
+extern "C" size_t gsb_synthesis_workspace_bytes(const gsb_styled_conv *layers, int n_run, int n_rgb, int64_t n) {
     if (!layers || n_run < 1 || n_run > gsb::SY_MAX_LAYERS || n < 1) return 0;
-    return gsb::synth_ws(nullptr, layers, n_run, n).bytes;
+    return gsb::synth_ws(nullptr, layers, n_run, n_rgb, n, true).bytes;
 }
 
 namespace gsb {
 
 // run stage: layers[0 .. n_run) on the styles S[l] [n, cin_l]; optional fp32 activation of the last layer (d_out), optional ToRGB
-// chain: rgbs[j] follows layer 2j with style rgb_s[j] [n, cin_j].  The demodulation factors are derived from S here (model.py:239).
-static int synthesis_run(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int n_run, int style_dim,
-                         const gsb_to_rgb *rgbs, int n_rgb, const float *const *S, const float *const *rgb_s, int64_t n, float *d_out,
-                         int64_t ld_out, float *d_rgb_out, const SynthWs &w, gsb_stream_t stream) {
-    const SynthView v = synth_view(const_cast<void *>(d_packed), layers, n_layers, style_dim);
+// chain: ToRGB j < n_rgb follows layer 2j with style rgb_s[j] [n, cin_j].  The demodulation factors are derived from S here
+// (model.py:239).
+static int synthesis_run(const SynthView &v, const gsb_styled_conv *layers, int n_run, int n_rgb, const float *const *S,
+                         const float *const *rgb_s, int64_t n, float *d_out, int64_t ld_out, float *d_rgb_out, const SynthWs &w,
+                         gsb_stream_t stream) {
     cudaStream_t st = (cudaStream_t)stream;
     for (int l = 0; l < n_run; ++l) {
         const gsb_styled_conv &c = layers[l];
@@ -484,7 +489,7 @@ static int synthesis_run(const void *d_packed, const gsb_styled_conv *layers, in
         if (with_rgb) {
             rgb_cur = (j == n_rgb - 1) ? d_rgb_out : w.rgb[j & 1];
             const int64_t tot = n * hw_out;
-            sy_rgb_init_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(rgbs[j].bias, rgb_prev, n, ro, rgb_cur);
+            sy_rgb_init_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(v.R[j].bias, rgb_prev, n, ro, rgb_cur);
             GSB_CHECK_LAUNCH();
         }
         for (int64_t b0 = 0; b0 < n; b0 += spc) {
@@ -502,7 +507,7 @@ static int synthesis_run(const void *d_packed, const gsb_styled_conv *layers, in
             e.out_f32 = (hooked && d_out) ? d_out + b0 * ld_out : nullptr;
             e.ld = ld_out;
             e.overflow = v.overflow;
-            e.rgb_w = with_rgb ? rgbs[j].conv_weight : nullptr;
+            e.rgb_w = with_rgb ? v.R[j].convw : nullptr;
             e.rgb_s = with_rgb ? rgb_s[j] + b0 * c.cout : nullptr;
             e.rgb_out = with_rgb ? rgb_cur + b0 * hw_out * 3 : nullptr;
             e.rgb_scale = (float)(1.0 / sqrt((double)c.cout));
@@ -525,114 +530,88 @@ static int synthesis_run(const void *d_packed, const gsb_styled_conv *layers, in
     return GSB_OK;
 }
 
-// argument checks shared by the three chain entries; *w receives the workspace layout
-static int check_run(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int n_run, int style_dim, const gsb_to_rgb *rgbs,
-                     int n_rgb, bool need_mod, int64_t n, float *d_out, int64_t ld_out, float *d_rgb_out, void *d_workspace,
-                     size_t workspace_bytes, bool own_styles, SynthWs *w) {
+// argument checks shared by the two chain entries; *w receives the workspace layout
+static int check_run(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int n_run, int n_rgb, int style_dim, int64_t n,
+                     float *d_out, int64_t ld_out, float *d_rgb_out, void *d_workspace, size_t workspace_bytes, bool own_styles,
+                     SynthWs *w) {
     if (int r = check_layers(layers, n_layers, style_dim)) return r;
     GSB_CHECK_ARG(d_packed && d_workspace && (d_out || d_rgb_out), "synthesis: null pointer");
     GSB_CHECK_ARG(n_run >= 1 && n_run <= n_layers, "synthesis: n_run out of range");
-    if (int r = check_rgbs(layers, n_run, rgbs, n_rgb, need_mod)) return r;
-    GSB_CHECK_ARG(n_rgb == 0 || d_rgb_out, "synthesis: ToRGB list without an image output");
+    GSB_CHECK_ARG(n_rgb >= 0 && n_rgb <= rgbs_of(n_run), "synthesis: ToRGB %d has no layer %d to follow", n_rgb - 1, 2 * (n_rgb - 1));
+    GSB_CHECK_ARG(n_rgb == 0 || d_rgb_out, "synthesis: ToRGBs without an image output");
     GSB_CHECK_ARG(n >= 0, "synthesis: bad n");
     if (n == 0) return GSB_OK;
     const gsb_styled_conv &last = layers[n_run - 1];
     const int ro_last = res_out_of(last);
     GSB_CHECK_ARG(!d_out || (ld_out >= (int64_t)ro_last * ro_last * last.cout && ld_out % 4 == 0), "synthesis: bad n / ld_out");
-    *w = synth_ws(d_workspace, layers, n_run, n, n_rgb > 0, style_dim, own_styles);
+    *w = synth_ws(d_workspace, layers, n_run, n_rgb, n, own_styles);
     if (workspace_bytes < w->bytes) { set_error("synthesis: workspace too small (%zu < %zu)", workspace_bytes, w->bytes); return GSB_ERR_WORKSPACE; }
     return GSB_OK;
 }
 
-// style stage into the workspace, then the run stage (gsb_synthesis_forward / gsb_synthesis_render)
-static int synthesis_latents(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int n_run, int style_dim,
-                             const gsb_to_rgb *rgbs, int n_rgb, const float *d_w, int w_layers, int64_t n, float *d_out, int64_t ld_out,
-                             float *d_rgb_out, void *d_workspace, size_t workspace_bytes, gsb_stream_t stream) {
-    GSB_CHECK_ARG(d_w && w_layers >= 1, "synthesis: no latents");
-    SynthWs w;
-    if (int r = check_run(d_packed, layers, n_layers, n_run, style_dim, rgbs, n_rgb, true, n, d_out, ld_out, d_rgb_out, d_workspace,
-                          workspace_bytes, true, &w)) return r;
-    if (n == 0) return GSB_OK;
-    const SynthView v = synth_view(const_cast<void *>(d_packed), layers, n_layers, style_dim);
+// style stage (model.py:226,234): s = w modw^T + modb with the modulation weight scaled at pack time.  Layer l reads latent entry
+// min(l, w_layers - 1), ToRGB j entry min(2j + 1, w_layers - 1); a NULL S[l] / rgb_s[j] (or array) skips that style.
+static int style_stage(const SynthView &v, const gsb_styled_conv *layers, int n_conv, int n_rgb, int style_dim, const float *d_w,
+                       int w_layers, int64_t n, float *const *S, float *const *rgb_s, gsb_stream_t stream) {
     auto latent = [&](int idx) { return d_w + (size_t)(idx < w_layers ? idx : w_layers - 1) * n * style_dim; };
-    for (int l = 0; l < n_run; ++l)
-        if (int r = conv_style(v, layers[l], l, latent(l), n, style_dim, w.S[l], stream)) return r;
-    for (int j = 0; j < n_rgb; ++j)
-        if (int r = rgb_style(rgbs[j], latent(2 * j + 1), n, style_dim, w.rgb_modw, w.rgb_s[j], stream)) return r;
-    return synthesis_run(d_packed, layers, n_layers, n_run, style_dim, rgbs, n_rgb, w.S, w.rgb_s, n, d_out, ld_out, d_rgb_out, w, stream);
+    for (int l = 0; S && l < n_conv; ++l)
+        if (S[l])
+            if (int r = sy_linear(latent(l), v.L[l].modw, v.L[l].modb, S[l], n, layers[l].cin, style_dim, stream)) return r;
+    for (int j = 0; rgb_s && j < n_rgb; ++j)
+        if (rgb_s[j])
+            if (int r = sy_linear(latent(2 * j + 1), v.R[j].modw, v.R[j].modb, rgb_s[j], n, layers[2 * j].cout, style_dim, stream))
+                return r;
+    return GSB_OK;
 }
 
 }  // namespace gsb
 
-extern "C" int gsb_synthesis_forward(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int n_run, int style_dim,
-                                     const float *d_w, int64_t n, float *d_out, int64_t ld_out, void *d_workspace,
-                                     size_t workspace_bytes, gsb_stream_t stream) {
-    GSB_CHECK_ARG(d_out, "synthesis_forward: null output");
-    return gsb::synthesis_latents(d_packed, layers, n_layers, n_run, style_dim, nullptr, 0, d_w, 1, n, d_out, ld_out, nullptr, d_workspace,
-                                  workspace_bytes, stream);
+// Generator.forward (model.py:493-571) up to layer n_run-1 and ToRGB n_rgb-1: the style stage into the workspace, then the run stage
+extern "C" int gsb_synthesis_forward(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int n_run, int n_rgb,
+                                     int style_dim, const float *d_w, int w_layers, int64_t n, float *d_act_out, int64_t ld_act,
+                                     float *d_rgb_out, void *d_workspace, size_t workspace_bytes, gsb_stream_t stream) {
+    using namespace gsb;
+    GSB_CHECK_ARG(d_w && w_layers >= 1, "synthesis: no latents");
+    SynthWs w;
+    if (int r = check_run(d_packed, layers, n_layers, n_run, n_rgb, style_dim, n, d_act_out, ld_act, d_rgb_out, d_workspace,
+                          workspace_bytes, true, &w)) return r;
+    if (n == 0) return GSB_OK;
+    const SynthView v = synth_view(const_cast<void *>(d_packed), layers, n_layers, style_dim);
+    if (int r = style_stage(v, layers, n_run, n_rgb, style_dim, d_w, w_layers, n, w.S, w.rgb_s, stream)) return r;
+    return synthesis_run(v, layers, n_run, n_rgb, w.S, w.rgb_s, n, d_act_out, ld_act, d_rgb_out, w, stream);
 }
 
-extern "C" size_t gsb_synthesis_render_workspace_bytes(const gsb_styled_conv *layers, int n_run, int64_t n, int style_dim) {
-    if (!layers || n_run < 1 || n_run > gsb::SY_MAX_LAYERS || n < 1) return 0;
-    return gsb::synth_ws(nullptr, layers, n_run, n, true, style_dim).bytes;
-}
-
-// Render path (Generator.forward, model.py:493-571): per-layer latents + the ToRGB / skip chain.
-extern "C" int gsb_synthesis_render(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int n_run, int style_dim,
-                                    const gsb_to_rgb *rgbs, int n_rgb, const float *d_w, int w_layers, int64_t n, float *d_act_out,
-                                    int64_t ld_act, float *d_rgb_out, void *d_workspace, size_t workspace_bytes, gsb_stream_t stream) {
-    return gsb::synthesis_latents(d_packed, layers, n_layers, n_run, style_dim, rgbs, n_rgb, d_w, w_layers, n, d_act_out, ld_act,
-                                  d_rgb_out, d_workspace, workspace_bytes, stream);
-}
-
-extern "C" int gsb_synthesis_styles(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int style_dim,
-                                    const gsb_to_rgb *rgbs, int n_rgb, const float *d_w, int w_layers, int64_t n, float *const *d_S,
-                                    float *const *d_rgb_s, void *d_workspace, size_t workspace_bytes, gsb_stream_t stream) {
+extern "C" int gsb_synthesis_styles(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int style_dim, const float *d_w,
+                                    int w_layers, int64_t n, float *const *d_S, float *const *d_rgb_s, gsb_stream_t stream) {
     using namespace gsb;
     if (int r = check_layers(layers, n_layers, style_dim)) return r;
     GSB_CHECK_ARG(d_packed && d_w && w_layers >= 1 && n >= 0, "synthesis_styles: null pointer or bad n");
-    GSB_CHECK_ARG(n_rgb == 0 || d_rgb_s, "synthesis_styles: ToRGB list without outputs");
-    size_t need = 0;
-    for (int j = 0; j < n_rgb; ++j) {
-        if (!d_rgb_s[j]) continue;
-        if (int r = check_rgbs(layers, n_layers, rgbs, j + 1, true)) return r;
-        need = need > (size_t)rgbs[j].cin * style_dim * 4 ? need : (size_t)rgbs[j].cin * style_dim * 4;
-    }
-    GSB_CHECK_ARG(need == 0 || (d_workspace && workspace_bytes >= need), "synthesis_styles: workspace too small (%zu < %zu)",
-                  workspace_bytes, need);
     if (n == 0) return GSB_OK;
     const SynthView v = synth_view(const_cast<void *>(d_packed), layers, n_layers, style_dim);
-    auto latent = [&](int idx) { return d_w + (size_t)(idx < w_layers ? idx : w_layers - 1) * n * style_dim; };
-    for (int l = 0; d_S && l < n_layers; ++l)
-        if (d_S[l])
-            if (int r = conv_style(v, layers[l], l, latent(l), n, style_dim, d_S[l], stream)) return r;
-    for (int j = 0; j < n_rgb; ++j)
-        if (d_rgb_s[j])
-            if (int r = rgb_style(rgbs[j], latent(2 * j + 1), n, style_dim, (float *)d_workspace, d_rgb_s[j], stream)) return r;
-    return GSB_OK;
+    return style_stage(v, layers, n_layers, rgbs_of(n_layers), style_dim, d_w, w_layers, n, d_S, d_rgb_s, stream);
 }
 
-extern "C" size_t gsb_synthesis_render_styled_workspace_bytes(const gsb_styled_conv *layers, int n_run, int64_t n) {
+extern "C" size_t gsb_synthesis_forward_styled_workspace_bytes(const gsb_styled_conv *layers, int n_run, int n_rgb, int64_t n) {
     if (!layers || n_run < 1 || n_run > gsb::SY_MAX_LAYERS || n < 1) return 0;
-    return gsb::synth_ws(nullptr, layers, n_run, n, true, 0, false).bytes;
+    return gsb::synth_ws(nullptr, layers, n_run, n_rgb, n, false).bytes;
 }
 
-extern "C" int gsb_synthesis_render_styled(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int n_run, int style_dim,
-                                           const gsb_to_rgb *rgbs, int n_rgb, const float *const *d_S, const float *const *d_rgb_s,
-                                           int64_t n, float *d_act_out, int64_t ld_act, float *d_rgb_out, void *d_workspace,
-                                           size_t workspace_bytes, gsb_stream_t stream) {
+extern "C" int gsb_synthesis_forward_styled(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int n_run, int n_rgb,
+                                            int style_dim, const float *const *d_S, const float *const *d_rgb_s, int64_t n,
+                                            float *d_act_out, int64_t ld_act, float *d_rgb_out, void *d_workspace,
+                                            size_t workspace_bytes, gsb_stream_t stream) {
     using namespace gsb;
     SynthWs w;
-    if (int r = check_run(d_packed, layers, n_layers, n_run, style_dim, rgbs, n_rgb, false, n, d_act_out, ld_act, d_rgb_out, d_workspace,
+    if (int r = check_run(d_packed, layers, n_layers, n_run, n_rgb, style_dim, n, d_act_out, ld_act, d_rgb_out, d_workspace,
                           workspace_bytes, false, &w)) return r;
-    GSB_CHECK_ARG(d_S && (n_rgb == 0 || d_rgb_s), "synthesis_render_styled: null style list");
+    GSB_CHECK_ARG(d_S && (n_rgb == 0 || d_rgb_s), "synthesis_forward_styled: null style list");
     for (int l = 0; l < n_run; ++l)
-        GSB_CHECK_ARG(d_S[l] && aligned16(d_S[l]), "synthesis_render_styled: style of layer %d is null or not 16-byte aligned", l);
+        GSB_CHECK_ARG(d_S[l] && aligned16(d_S[l]), "synthesis_forward_styled: style of layer %d is null or not 16-byte aligned", l);
     for (int j = 0; j < n_rgb; ++j)
-        GSB_CHECK_ARG(d_rgb_s[j] && aligned16(d_rgb_s[j]), "synthesis_render_styled: style of ToRGB %d is null or not 16-byte aligned", j);
+        GSB_CHECK_ARG(d_rgb_s[j] && aligned16(d_rgb_s[j]), "synthesis_forward_styled: style of ToRGB %d is null or not 16-byte aligned", j);
     if (n == 0) return GSB_OK;
-    return synthesis_run(d_packed, layers, n_layers, n_run, style_dim, rgbs, n_rgb, d_S, d_rgb_s, n, d_act_out, ld_act, d_rgb_out, w,
-                         stream);
+    const SynthView v = synth_view(const_cast<void *>(d_packed), layers, n_layers, style_dim);
+    return synthesis_run(v, layers, n_run, n_rgb, d_S, d_rgb_s, n, d_act_out, ld_act, d_rgb_out, w, stream);
 }
 
 extern "C" int gsb_synthesis_status(const void *d_packed, const gsb_styled_conv *layers, int n_layers, int style_dim, unsigned *h_flags) {

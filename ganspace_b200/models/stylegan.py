@@ -226,12 +226,22 @@ class StyleGAN_G(nn.Sequential):
 
     def style_layers(self):
         """(name, chain layer, latent index, width 2C) of every style layer ``g_synthesis.blocks.RxR.epi{1,2}.style_mod.lin``, in
-        execution order: chain layer l is the l-th epilogue and reads latent l of an 18-latent input."""
+        execution order: chain layer l is the l-th epilogue and reads latent l of an 18-latent input.  The chain layer is also the
+        layer's position in this table, the key of its rows (``PackedStyleGAN.styles``)."""
         out = []
         for l, (_, epi, _, _) in enumerate(self.g_synthesis.layer_modules()):
             blk = self.block_names()[l // 2]
             out.append((f"{blk}.epi{l % 2 + 1}.style_mod.lin", l, l, epi.style_mod.lin.weight.shape[0]))
         return out
+
+    def hookable_layers(self):
+        return ["g_mapping"] + self.block_names() + [t[0] for t in self.style_layers()]
+
+    def unhookable_layers(self):
+        """Sub-modules that run inside the fused kernels and have no output of their own to hook: every one but
+        ``hookable_layers()``."""
+        hookable = set(self.hookable_layers())
+        return [n for n, _ in self.named_modules() if n and n not in hookable]
 
 
 def synthesis_fill(net, seed):

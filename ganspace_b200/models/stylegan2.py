@@ -187,7 +187,7 @@ class StyledConv(nn.Module):
 
 class ToRGB(nn.Module):
     """model.py:344-363.  The arithmetic (1x1 modulated conv without demodulation, bias, up-sampled skip) is fused into the
-    epilogue of the StyledConv it follows (gsb_synthesis_render); ``forward(_result=skip)`` hands the result to the hooks."""
+    epilogue of the StyledConv it follows (gsb_synthesis_forward); ``forward(_result=skip)`` hands the result to the hooks."""
 
     def __init__(self, in_channel, style_dim, upsample=True, blur_kernel=(1, 3, 3, 1)):
         super().__init__()
@@ -202,6 +202,7 @@ class ToRGB(nn.Module):
         return _result
 
     def describe(self):
+        """ToRGB descriptor for _native.PackedSynthesis, which copies the parameters at pack time."""
         c = self.conv
         return dict(conv_weight=c.weight[0, :, :, 0, 0], mod_weight=c.modulation.weight, mod_bias=c.modulation.bias,
                     bias=self.bias.reshape(3))
@@ -260,16 +261,17 @@ class Generator(nn.Module):
                 [("to_rgb1", self.to_rgb1)] + [(f"to_rgbs.{j}", m) for j, m in enumerate(self.to_rgbs)])
 
     def style_layers(self):
-        """The style space: (name, chain, index, latent entry, width) of every modulation layer, in execution order.  ``chain`` is
-        'conv' (index 0 = conv1, k + 1 = convs.k) or 'rgb' (index 0 = to_rgb1, j + 1 = to_rgbs.j); the latent entry is the
-        [N, n_latent, 512] latent's column the layer reads (model.py:546-561); width = the layer's input channels."""
+        """The style space: (name, key, latent entry, width) of every modulation layer, in execution order (conv1, to_rgb1, convs.0,
+        convs.1, to_rgbs.0, ...; ToRGB j follows StyledConv 2j).  The key is the layer's position in this table, which keys its rows
+        (``PackedSynthesis.styles``); the latent entry is the [N, n_latent, 512] latent's column the layer reads
+        (model.py:546-561); width = the layer's input channels."""
         convs, rgbs = self.chain_layers()
         out = []
         for l, (name, m) in enumerate(convs):
-            out.append((f"{name}.conv.modulation", "conv", l, l, m.conv.in_channel))
+            out.append((f"{name}.conv.modulation", len(out), l, m.conv.in_channel))
             if l % 2 == 0:
                 j = l // 2
-                out.append((f"{rgbs[j][0]}.conv.modulation", "rgb", j, 2 * j + 1, rgbs[j][1].conv.in_channel))
+                out.append((f"{rgbs[j][0]}.conv.modulation", len(out), 2 * j + 1, rgbs[j][1].conv.in_channel))
         return out
 
     def unhookable_layers(self):
@@ -309,9 +311,7 @@ class Generator(nn.Module):
             raise NotImplementedError("Generator.forward needs the wrapper's packed synthesis chain (StyleGAN2.forward); "
                                       "randomised noise is not built")
         latent = self.latent(styles, inject_index, truncation, truncation_latent, input_is_w)     # [N, n_latent, S]
-        mods = [self.conv1] + list(self.convs)
-        rgbs = [self.to_rgb1] + list(self.to_rgbs)
         w_layers = latent.permute(1, 0, 2).contiguous()
-        _, img = _synthesis.render(w_layers, len(mods), [r.describe() for r in rgbs])
+        _, img = _synthesis.forward(w_layers, len(self.convs) + 1, want_act=False, n_rgb=len(self.to_rgbs) + 1)
         image = img.permute(0, 3, 1, 2)                                            # NCHW view of the NHWC skip image
         return (image, latent) if return_latents else (image, None)

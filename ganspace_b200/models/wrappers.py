@@ -148,7 +148,19 @@ class _DeviceGenerator(BaseModel):
 
 
 class _StyledGenerator(_DeviceGenerator):
-    """A device generator with a mapping network (StyleGAN2, StyleGAN): latents are in Z, or in W after ``use_w``."""
+    """A device generator with a mapping network and a style space (StyleGAN2, StyleGAN): latents are in Z, or in W after
+    ``use_w``; ``forward`` and ``partial_forward`` share one skeleton.  Each model describes its fused chain as data:
+
+    * ``_chain_outputs()``: (name, n_run, n_rgb) of every hookable chain output in execution order, with the chain run that ends
+      at it: ``n_run`` layers and ``n_rgb`` ToRGBs.  The output is the run's last activation when ``n_rgb`` is 0, else its image;
+    * ``_style_layers()``: (name, n_run, n_rgb) of every style layer, in the order of ``model.style_layers()`` (execution order),
+      with the chain run that reaches it; style rows are keyed by their position in this table;
+    * ``_image_run()``: the (n_run, n_rgb) of the image ``forward`` returns;
+    * ``_stop(layer_name)``: the index of the chain output at which ``partial_forward`` stops (the reference's stop rule);
+    * ``_chain(n_run)``: the packed chain (``forward``, ``styles``, ``forward_styled``, ``shapes``) covering ``n_run`` layers;
+    * ``_w_layers(ws, truncate)``: the [Lw, n, 512] per-layer latents of a call ([1, n, 512] for one latent);
+    * ``_stops_before_chain(layer_name, ws)``: whether ``partial_forward`` ends before the fused chain (in the mapping network);
+    * ``model.unhookable_layers()`` and ``_unhookable_message(name)``: the sub-modules the chain gives no output of their own."""
 
     def latent_space_name(self):
         return "W" if self.w_primary else "Z"
@@ -180,6 +192,89 @@ class _StyledGenerator(_DeviceGenerator):
             raise ValueError(f"an edit on '{name}' must keep the style's shape {tuple(rows.shape)} (or [1, {rows.shape[1]}]), got "
                              f"{tuple(out.shape)}")
         return out.to(device=rows.device, dtype=torch.float32).contiguous()
+
+    def _module(self, name):
+        mods = getattr(self, "_by_name", None)
+        if mods is None:
+            mods = self._by_name = dict(self.model.named_modules())
+        return mods[name]
+
+    def _reject_sub_module_hooks(self, layer_name=None):
+        """Refuses hooks on, and ``partial_forward`` to, the sub-modules that run inside the fused chain."""
+        guarded = getattr(self, "_guarded", None)
+        if guarded is None:
+            guarded = self._guarded = {n: self._module(n) for n in self.model.unhookable_layers()}
+        for name, m in guarded.items():
+            if len(m._forward_hooks) or len(m._forward_pre_hooks):
+                raise NotImplementedError(self._unhookable_message(name))
+        if layer_name in guarded:
+            raise NotImplementedError(self._unhookable_message(layer_name))
+
+    def forward(self, x):
+        """wrappers.py: images in [0, 1] (before clamping) from one latent or a list of per-layer latents.  Hooked chain outputs
+        receive their activations (retain_layer works); an edit of one would have to be re-fed into the fused chain, which is not
+        built -- it raises instead of being silently ignored.  Hooked style layers receive their style rows once per call, and what
+        their hooks return is what every chain run of the call uses."""
+        return 0.5 * (self._synthesize(x, None).permute(0, 3, 1, 2) + 1)
+
+    def partial_forward(self, x, layer_name):
+        """Runs the network up to the chain output the reference's stop rule names for ``layer_name``; the side effect is that the
+        hooks on the way fire.  An edit is accepted on that last output alone.  With only style layers hooked, only their rows
+        are computed (no synthesis launch)."""
+        self._synthesize(x, layer_name)
+
+    def _hooked(self, name):
+        return len(self._module(name)._forward_hooks) > 0
+
+    def _synthesize(self, x, layer_name):
+        """The skeleton of ``forward`` (``layer_name`` None; returns the NHWC image) and ``partial_forward``."""
+        self._reject_sub_module_hooks(layer_name)
+        ws = x if isinstance(x, list) else [x]
+        if not self.w_primary:
+            ws = [self._mapping()(s) for s in ws]          # module calls: the mapping network's hooks fire
+        if layer_name is not None and self._stops_before_chain(layer_name, ws):
+            return None
+        w_layers = self._w_layers(ws, layer_name is None)
+        outs = self._chain_outputs()
+        outs = outs if layer_name is None else outs[:self._stop(layer_name) + 1]
+        image = self._image_run() if layer_name is None else None
+        n_run, n_rgb = image or (max(o[1] for o in outs), max(o[2] for o in outs))
+        hooked = [o for o in outs if self._hooked(o[0])]
+        # the style stage: once, with every row of the call's layers when a chain run consumes them
+        styles = [(k, t) for k, t in enumerate(self._style_layers()) if t[1] <= n_run and t[2] <= n_rgb]
+        S = None
+        if any(self._hooked(t[0]) for _, t in styles):
+            want = [(k, t) for k, t in styles if hooked or image or self._hooked(t[0])]
+            S = self._chain(n_run).styles(w_layers, [k for k, _ in want])
+            for k, t in want:
+                if self._hooked(t[0]):
+                    S[k] = self._hand_style(self._module(t[0]), S[k], t[0])
+
+        def run(n_run, n_rgb, want_act):
+            # the chains' last argument: StyleGAN2's ToRGB count, StyleGAN's want_rgb (its one torgb after the last layer)
+            chain = self._chain(n_run)
+            if S is None:
+                return (chain, *chain.forward(w_layers, n_run, None, want_act, n_rgb))
+            return (chain, *chain.forward_styled(S, n_run, None, want_act, n_rgb))
+
+        def hand(o, chain, act, img):
+            # an edit raises when the run goes on past the output: before the last output, or when the image is made
+            downstream = image is not None or o is not outs[-1]
+            if o[2]:
+                self._hand_off(self._module(o[0]), img, img.shape[1], 3, downstream, o[0])
+            else:
+                self._hand_off(self._module(o[0]), act, *chain.shapes[o[1] - 1], downstream, o[0])
+        # the image's run also serves the outputs it ends at: the last activation, and the image itself
+        served = [o for o in hooked if image and (o[1], o[2]) in (image, (image[0], 0))]
+        for o in hooked:
+            if o not in served:
+                hand(o, *run(o[1], o[2], o[2] == 0))
+        if image is None:
+            return None
+        chain, act, img = run(*image, any(o[2] == 0 for o in served))
+        for o in served:
+            hand(o, chain, act, img)
+        return img
 
     def draw_z_async(self, n_samples, seed):
         """The Z stream of ``sample_latent(n_samples, seed=seed)`` generated on a side stream; returns a callable that makes
@@ -326,119 +421,71 @@ class StyleGAN2(_StyledGenerator):
     def get_max_latents(self):
         return self.model.n_latent
 
-    def forward(self, x):
-        """wrappers.py:188-192: images in [0, 1] (before clamping) from one latent, a pair, or one latent per layer.  Hooked
-        StyledConv / ToRGB layers receive their activations (retain_layer works); an edit installed on a hooked layer would
-        have to be re-fed into the fused chain, which is not built -- it raises instead of being silently ignored.  Hooked style
-        layers ('*.conv.modulation') receive their style rows, and what their hooks return is what every chain run of the call
-        modulates with."""
-        self._reject_sub_module_hooks()
-        x = x if isinstance(x, list) else [x]
-        names = self.synthesis_layer_names()
-        target, rgb_upto = len(names) - 1, len(self.model.to_rgbs)
-        syn = self._synthesis(len(names))
-        if not self._hooked_styles(target, rgb_upto):
-            out, latent = self.model(x, noise=self.noise, truncation=self.truncation, truncation_latent=self.latent_avg,
-                                     input_is_w=self.w_primary, return_latents=True, _synthesis=syn)
-            self._fire_hooks(latent, target, rgb_upto=rgb_upto)
-            return 0.5 * (out + 1)
-        latent = self.model.latent(x, truncation=self.truncation, truncation_latent=self.latent_avg, input_is_w=self.w_primary)
-        styles = self._styles(latent.permute(1, 0, 2).contiguous(), target, rgb_upto, True)
-        _, img = syn.render_styled([styles[0][l] for l in range(len(names))], [styles[1][j] for j in range(rgb_upto + 1)], len(names),
-                                   [r.describe() for _, r in self.model.chain_layers()[1]])
-        self._fire_hooks(None, target, rgb_upto=rgb_upto, styles=styles)
-        return 0.5 * (img.permute(0, 3, 1, 2) + 1)
-
-    def _fire_hooks(self, latent, target, rgb_upto=-1, styles=None):
-        """Hand the activations of hooked StyledConv layers 0..target (and hooked ToRGB layers 0..rgb_upto) to their hooks:
-        each gets its own run of the fused chain up to that layer, on the per-layer latents ``latent`` or, when given, on the
-        style rows ``styles`` (from ``_styles``)."""
+    # ---- the fused chain conv1, to_rgb1, convs.0, convs.1, to_rgbs.0, ... (wrappers.py:188-255) ------------------------
+    def _chain_outputs(self):
+        """StyledConv l runs as (l + 1, 0); ToRGB j, which follows StyledConv 2j, as (2j + 1, j + 1)."""
         convs, rgbs = self.model.chain_layers()
-        w_layers = latent.permute(1, 0, 2).contiguous() if styles is None else None
+        out = []
+        for l, (name, _) in enumerate(convs):
+            out.append((name, l + 1, 0))
+            if l % 2 == 0:
+                out.append((rgbs[l // 2][0], l + 1, l // 2 + 1))
+        return out
 
-        def run(n_run, n_rgb, want_act):
-            syn = self._synthesis(n_run)
-            descs = [r.describe() for _, r in rgbs[:n_rgb]]
-            if styles is None:
-                return syn, syn.render(w_layers, n_run, descs, want_act=want_act)
-            return syn, syn.render_styled([styles[0][l] for l in range(n_run)], [styles[1][j] for j in range(n_rgb)], n_run, descs,
-                                          want_act=want_act)
-        for i in range(target + 1):
-            if len(convs[i][1]._forward_hooks):
-                syn, (act, _) = run(i + 1, 0, True)
-                self._hand_off(convs[i][1], act, *syn.shapes[i], True, convs[i][0])
-        for j in range(rgb_upto + 1):
-            if len(rgbs[j][1]._forward_hooks):
-                _, (_, img) = run(2 * j + 1, j + 1, False)
-                self._hand_off(rgbs[j][1], img, img.shape[1], 3, True, rgbs[j][0])
+    def _style_layers(self):
+        """The modulation layer of each chain output, in the order of ``Generator.style_layers()``."""
+        return [(f"{name}.conv.modulation", n_run, n_rgb) for name, n_run, n_rgb in self._chain_outputs()]
 
-    # ---- style space: the modulation layers '*.conv.modulation' -----------------------------------------
-    def _style_modules(self, target, rgb_upto):
-        """(name, chain, index, module) of the style layers a run to StyledConv ``target`` and ToRGB ``rgb_upto`` executes."""
-        convs, rgbs = self.model.chain_layers()
-        return [(name, chain, i, (convs if chain == "conv" else rgbs)[i][1].conv.modulation)
-                for name, chain, i, _, _ in self.model.style_layers() if i <= (target if chain == "conv" else rgb_upto)]
+    def _image_run(self):
+        return len(self.model.convs) + 1, len(self.model.to_rgbs) + 1
 
-    def _hooked_styles(self, target, rgb_upto):
-        return any(len(m._forward_hooks) for *_, m in self._style_modules(target, rgb_upto))
+    def _stops_before_chain(self, layer_name, ws):
+        if "style" in layer_name:
+            # (the reference builds the [N, n_latent, 512] repeat + StridedStyle stack before this early exit, wrappers.py:202-222 --
+            # 328 MB of traffic per 10k batch that nothing reads; skipped here)
+            return True
+        if layer_name == "input":
+            self.model.input(self.model.latents_per_layer(ws)[:, 0])
+            return True
+        return False
 
-    def _styles(self, w_layers, target, rgb_upto, all_rows):
-        """Style rows for per-layer latents ``w_layers`` [Lw, n, 512], computed once; each hooked style layer up to StyledConv
-        ``target`` / ToRGB ``rgb_upto`` fires once with its rows and what it returns replaces them.  Returns ({conv l: rows},
-        {ToRGB j: rows}) with the rows of every layer in that range when ``all_rows`` (for chain runs), else of the hooked ones."""
-        mods = self._style_modules(target, rgb_upto)
-        want = mods if all_rows else [t for t in mods if len(t[3]._forward_hooks)]
-        rgbs = self.model.chain_layers()[1]
-        rgb_idx = [i for _, chain, i, _ in want if chain == "rgb"]
-        syn = self._synthesis(max([target + 1] + [2 * j + 1 for j in rgb_idx]))
-        S, R = syn.styles(w_layers, [i for _, chain, i, _ in want if chain == "conv"], rgb_idx,
-                          [r.describe() for _, r in rgbs[:max(rgb_idx, default=-1) + 1]])
-        for name, chain, i, m in want:
-            if len(m._forward_hooks):
-                rows = S if chain == "conv" else R
-                rows[i] = self._hand_style(m, rows[i], name)
-        return S, R
-
-    def _reject_sub_module_hooks(self):
-        guarded = getattr(self, "_guarded", None)
-        if guarded is None:
-            mods = dict(self.model.named_modules())
-            guarded = self._guarded = [(n, mods[n]) for n in self.model.unhookable_layers()]
-        for name, m in guarded:
-            if len(m._forward_hooks) or len(m._forward_pre_hooks):
-                raise NotImplementedError(self._unhookable_message(name))
+    def _w_layers(self, ws, truncate):
+        """One latent, a pair (style mixing at a random index, as the reference) or one latent per layer; ``forward`` truncates."""
+        if truncate and self.truncation < 1:
+            ws = [self.latent_avg + self.truncation * (s - self.latent_avg) for s in ws]       # model.py:511-552
+        if len(ws) == 1 and ws[0].dim() < 3:
+            return ws[0].reshape(1, -1, 512)
+        return self.model.latents_per_layer(ws).permute(1, 0, 2).contiguous()
 
     def _unhookable_message(self, name):
         return (f"StyleGAN2: a hook on '{name}' is not supported: the StyledConv and ToRGB layers run as one fused chain; the "
                 "hookable synthesis layers are conv1, convs.k, to_rgb1, to_rgbs.j and their style layers '<layer>.conv.modulation'")
 
     def _stop(self, layer_name):
-        """(last StyledConv, last ToRGB) that partial_forward to ``layer_name`` runs (wrappers.py:228-255).  A style layer stops
-        at the StyledConv or ToRGB that contains it."""
+        """The StyledConv or ToRGB named, or the one that contains the style layer named (wrappers.py:228-255)."""
         base = layer_name[:-len(".conv.modulation")] if layer_name.endswith(".conv.modulation") else layer_name
-        names, rgb_names = self.synthesis_layer_names(), self._rgb_names()
-        if base in names:
-            t = names.index(base)
-            return t, (t - 1) // 2             # the reference computes every to_rgb that precedes the target as well
-        if base in rgb_names:
-            j = rgb_names.index(base)
-            return 2 * j, j
-        raise RuntimeError(f"Unknown layer '{layer_name}'")
+        names = [o[0] for o in self._chain_outputs()]
+        if base not in names:
+            raise RuntimeError(f"Unknown layer '{layer_name}'")
+        return names.index(base)
 
-    # ---- synthesis chain conv1, convs.0 .. convs.k (wrappers.py:224-255) ------------------------------------
     def synthesis_layer_names(self):
         return ["conv1"] + [f"convs.{i}" for i in range(len(self.model.convs))]
 
-    def _rgb_names(self):
-        return ["to_rgb1"] + [f"to_rgbs.{i}" for i in range(len(self.model.to_rgbs))]
+    def _chain(self, n_run):
+        return self._synthesis(n_run)
 
     def _synthesis(self, n_run):
-        """PackedSynthesis covering at least the first ``n_run`` StyledConv layers.  A pack of more layers serves as long as the
-        constant and the parameters and noise maps of these ``n_run`` layers are the ones it was packed from."""
+        """PackedSynthesis covering at least the first ``n_run`` StyledConv layers and the ToRGBs that follow them.  A pack of more
+        layers serves as long as the constant and the parameters and noise maps of these layers and ToRGBs are the ones it was
+        packed from."""
         mods = [self.model.conv1] + list(self.model.convs)
+        rgbs = [self.model.to_rgb1] + list(self.model.to_rgbs)
+        rgb_params = lambda r: [r.conv.weight, r.conv.modulation.weight, r.conv.modulation.bias, r.bias]
         keys = (_native.source_key([self.model.input.input]),) + tuple(
             _native.source_key([m.conv.weight, m.conv.modulation.weight, m.conv.modulation.bias, m.noise.weight, m.activate.bias,
-                                self.noise[i]]) for i, m in enumerate(mods[:n_run]))
+                                self.noise[i]] + (rgb_params(rgbs[i // 2]) if i % 2 == 0 else []))
+            for i, m in enumerate(mods[:n_run]))
         if self._synth_keys[:len(keys)] != keys:
             self._synth_keys = keys               # a stale or too short pack: the get() below packs n_run layers
 
@@ -447,7 +494,8 @@ class StyleGAN2(_StyledGenerator):
             for i, m in enumerate(mods[:n_run]):
                 layers.append(m.describe(self.noise[i], res))
                 res = 2 * res if m.conv.upsample else res
-            return _native.PackedSynthesis(self.model.input.input.detach()[0], layers, self.model.style_dim)
+            return _native.PackedSynthesis(self.model.input.input.detach()[0], layers,
+                                           [r.describe() for r in rgbs[:(n_run + 1) // 2]], self.model.style_dim)
         return self._synth.get([], build, self._synth_keys)
 
     def feature_layout(self, layer_name):
@@ -463,48 +511,7 @@ class StyleGAN2(_StyledGenerator):
         names = self.synthesis_layer_names()
         n_run = names.index(layer_name) + 1
         w = x if self.w_primary else self.model.style(x)
-        return self._synthesis(n_run).forward(w.reshape(-1, 512), n_run, out=out)
-
-    def partial_forward(self, x, layer_name):
-        """wrappers.py:194-259: run up to (and including) the named layer; side effect = its hooks fire.  ``x``: one latent, a
-        pair (style mixing at a random index, as the reference) or one latent per layer.  A style layer '<layer>.conv.modulation'
-        runs as far as <layer>; when no StyledConv or ToRGB on the way is hooked, only its style rows are computed."""
-        self._reject_sub_module_hooks()
-        if any(layer_name == n for n, _ in self._guarded):
-            raise NotImplementedError(self._unhookable_message(layer_name))
-        styles = x if isinstance(x, list) else [x]
-        if not self.w_primary:
-            styles = [self.model.style(s) for s in styles]
-        if "style" in layer_name:
-            # (the reference builds the [N, n_latent, 512] repeat + StridedStyle stack before this early exit, wrappers.py:202-222 --
-            # 328 MB of traffic per 10k batch that nothing reads; skipped here)
-            return
-        latent = None if (len(styles) == 1 and layer_name != "input") else self.model.latents_per_layer(styles)   # [N, n_latent, 512]
-        if layer_name == "input":
-            self.model.input(latent[:, 0])
-            return
-        names = self.synthesis_layer_names()
-        target, rgb_upto = self._stop(layer_name)
-        convs, rgbs = self.model.chain_layers()
-        if layer_name.endswith(".conv.modulation") or self._hooked_styles(target, rgb_upto):
-            chain_hooked = any(len(m._forward_hooks) for _, m in convs[:target + 1] + rgbs[:rgb_upto + 1])
-            w_layers = styles[0].reshape(1, -1, 512) if latent is None else latent.permute(1, 0, 2).contiguous()
-            st = self._styles(w_layers, target, rgb_upto, chain_hooked)
-            if chain_hooked:
-                self._fire_hooks(None, target, rgb_upto, styles=st)
-            return
-        if latent is None:
-            latent = self.model.latents_per_layer(styles)
-        rgb_hooked = any(len(m._forward_hooks) for _, m in rgbs)
-        if layer_name in names and len(styles) == 1 and not rgb_hooked:
-            # one global latent, no ToRGB hook: the decomposition's own call pattern -- the single-latent entry point
-            w = styles[0].reshape(-1, 512)
-            for i in [i for i in range(target) if len(convs[i][1]._forward_hooks)] + [target]:
-                syn = self._synthesis(target + 1)
-                # (an edit on the target layer itself has nothing downstream inside partial_forward)
-                self._hand_off(convs[i][1], syn.forward(w, i + 1), *syn.shapes[i], i < target, names[i])
-        else:
-            self._fire_hooks(latent, target, rgb_upto=rgb_upto)
+        return self._synthesis(n_run).forward(w.reshape(-1, 512), n_run, out=out)[0]
 
     def set_noise_seed(self, seed):
         # same generator stream as the reference (torch.manual_seed(seed); torch.randn per noise map),
@@ -702,112 +709,45 @@ class StyleGAN(_StyledGenerator):
         if self.model.g_synthesis.pack_cache.current() is not None:
             self.model.g_synthesis.pack_cache.current().check()
 
-    # ---- synthesis ----------------------------------------------------------------------------------------
+    # ---- the fused chain: two layers per block, torgb after the last ----------------------------------------------------------
+    def _chain_outputs(self):
+        """Block i ends the run of its two layers."""
+        return [(name, 2 * (i + 1), 0) for i, name in enumerate(self.model.block_names())]
+
+    def _style_layers(self):
+        """Style layer l is reached by the run of chain layers 0 .. l."""
+        return [(t[0], t[1] + 1, 0) for t in self.model.style_layers()]
+
+    def _image_run(self):
+        return 2 * len(self.model.g_synthesis.blocks), 1
+
+    def _chain(self, n_run):
+        return self.model.g_synthesis.packed()
+
+    def _stops_before_chain(self, layer_name, ws):
+        return "g_mapping" in layer_name or layer_name == "truncation"
+
+    def _w_layers(self, ws, truncate):
+        """[18, n, 512] per-layer dlatents (wrappers.py:382-387 / model.py:382-393) from a list of 18, else [1, n, 512]."""
+        if len(ws) == 1:
+            return ws[0].reshape(1, -1, 512).float()
+        assert len(ws) == 18, "Must provide 1 or 18 latents"
+        return torch.stack([w.reshape(-1, 512).float() for w in ws])
+
+    def _unhookable_message(self, name):
+        return (f"StyleGAN: a hook on '{name}' is not supported: g_mapping and the synthesis blocks run as fused kernels; the "
+                f"hookable layers are {', '.join(self._hookable())}")
+
     def _hookable(self):
-        return ["g_mapping"] + self.model.block_names() + [t[0] for t in self.model.style_layers()]
+        return self.model.hookable_layers()
 
-    def _reject_sub_module_hooks(self):
-        hookable = set(self._hookable())
-        for name, m in self.model.named_modules():
-            if name and name not in hookable and (len(m._forward_hooks) or len(m._forward_pre_hooks)):
-                raise NotImplementedError(f"StyleGAN: a hook on '{name}' is not supported: g_mapping and the synthesis blocks run as "
-                                          f"fused kernels; the hookable layers are {', '.join(self._hookable())}")
-
-    def _w_layers(self, x):
-        """[18, n, 512] per-layer dlatents (wrappers.py:382-387 / model.py:382-393) from one latent or a list of 18 (Z or W)."""
-        if isinstance(x, list):
-            assert len(x) == 18, "Must provide 1 or 18 latents"
-            ws = [l if self.w_primary else self.model.g_mapping(l) for l in x]
-            return torch.stack([w.reshape(-1, 512).float() for w in ws])
-        w = x if self.w_primary else self.model.g_mapping(x)
-        return w.reshape(1, -1, 512).float()
-
-    def _run(self, w_layers, target, want_rgb, styles=None):
-        """Blocks 0 .. ``target`` with the forward hooks of every hooked block on the way (a hooked earlier block gets its own run
-        of the chain); the image when ``want_rgb``.  With ``styles`` ({layer: rows}, from ``_styles``) every run takes its styles
-        from there instead of from ``w_layers``."""
-        packed = self.model.g_synthesis.packed()
-        blocks = list(self.model.g_synthesis.blocks.values())
-        names = self.model.block_names()
-        w_layers = w_layers[:2 * (target + 1)] if w_layers.shape[0] > 1 else w_layers
-
-        def run(n_run, **kw):
-            if styles is not None:
-                return packed.forward_styled(styles, n_run, **kw)
-            return packed.forward(w_layers[:n_run] if w_layers.shape[0] > 1 else w_layers, n_run, **kw)
-        hand = lambda i, act: self._hand_off(blocks[i], act, *packed.shapes[2 * i + 1], i < target or want_rgb, names[i])
-        for i in [i for i in range(target) if len(blocks[i]._forward_hooks)]:
-            hand(i, run(2 * (i + 1))[0])
-        want_act = len(blocks[target]._forward_hooks) > 0
-        act, rgb = run(2 * (target + 1), want_act=want_act or not want_rgb, want_rgb=want_rgb)
-        if want_act:
-            hand(target, act)
-        return rgb
-
-    # ---- style space: the StyleMod layers 'g_synthesis.blocks.RxR.epi{1,2}.style_mod.lin' --------------------
-    def _style_modules(self, n_run):
-        """(name, chain layer, module) of the style layers of chain layers 0 .. n_run-1."""
-        epis = self.model.g_synthesis.layer_modules()
-        return [(name, l, epis[l][1].style_mod.lin) for name, l, _, _ in self.model.style_layers() if l < n_run]
-
-    def _hooked_styles(self, n_run):
-        return any(len(m._forward_hooks) for *_, m in self._style_modules(n_run))
-
-    def _styles(self, w_layers, n_run, all_rows):
-        """Style rows for per-layer dlatents ``w_layers`` [Lw, n, 512], computed once; each hooked style layer of chain layers
-        0 .. n_run-1 fires once with its rows, and what it returns replaces them.  Returns {layer: rows} with the rows of every
-        layer in that range when ``all_rows`` (for chain runs), else of the hooked ones."""
-        mods = self._style_modules(n_run)
-        want = mods if all_rows else [t for t in mods if len(t[2]._forward_hooks)]
-        if not want:
-            return {}
-        S = self.model.g_synthesis.packed().styles(w_layers, [l for _, l, _ in want])
-        for name, l, m in want:
-            if len(m._forward_hooks):
-                S[l] = self._hand_style(m, S[l], name)
-        return S
-
-    def forward(self, x):
-        """wrappers.py:375-377: images ``0.5 (torgb + 1)`` (unclamped) from one latent or a list of 18; hooked blocks fire.  Hooked
-        style layers receive their rows once per call, and what their hooks return is what every chain run of the call uses."""
-        self._reject_sub_module_hooks()
-        w_layers = self._w_layers(x)
-        target = len(self.model.g_synthesis.blocks) - 1
-        n_layers = 2 * (target + 1)
-        styles = self._styles(w_layers, n_layers, True) if self._hooked_styles(n_layers) else None
-        rgb = self._run(w_layers, target, True, styles=styles)
-        return 0.5 * (rgb.permute(0, 3, 1, 2) + 1)
-
-    def _target_block(self, layer_name):
+    def _stop(self, layer_name):
         """The reference's stop rule (wrappers.py:394-417): the first block one of whose leaf modules' names contains ``layer_name``."""
         for i, (n, blk) in enumerate(self.model.g_synthesis.blocks.items()):
             leaves = [f"g_synthesis.blocks.{n}.{c}" for c, m in blk.named_modules(remove_duplicate=False) if c and not m._modules]
             if any(layer_name in c for c in leaves):
                 return i
         raise RuntimeError(f"Layer {layer_name} not encountered in partial_forward")
-
-    def partial_forward(self, x, layer_name):
-        """wrappers.py:379-417: the blocks up to the one the stop rule names; hooks on the way fire.  To a style layer with no block
-        on the way hooked, only the hooked style layers' rows are computed (no synthesis launch)."""
-        self._reject_sub_module_hooks()
-        if not self.w_primary:
-            x = [self.model.g_mapping(l) for l in x] if isinstance(x, list) else self.model.g_mapping(x)
-        if "g_mapping" in layer_name or layer_name == "truncation":
-            return
-        w_primary, self.w_primary = self.w_primary, True                          # x holds W from here on
-        try:
-            w_layers = self._w_layers(x)
-        finally:
-            self.w_primary = w_primary
-        target = self._target_block(layer_name)
-        n_run = 2 * (target + 1)
-        if not (layer_name.endswith(".style_mod.lin") or self._hooked_styles(n_run)):
-            self._run(w_layers, target, False)
-            return
-        blocks_hooked = any(len(b._forward_hooks) for b in list(self.model.g_synthesis.blocks.values())[:target + 1])
-        styles = self._styles(w_layers, n_run, blocks_hooked)
-        if blocks_hooked:
-            self._run(w_layers, target, False, styles=styles)
 
     def feature_layout(self, layer_name):
         names = self.model.block_names()

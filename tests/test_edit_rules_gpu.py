@@ -2,15 +2,12 @@
 fused chain cannot take that tensor back: the edit raises when the run goes on past the edited layer, and is accepted on the
 last layer of a partial run.  Each call path has its own rule:
 
-| call path                                                   | an edit raises when                              |
-|-------------------------------------------------------------|--------------------------------------------------|
-| StyleGAN2 ``partial_forward``, one latent, no ToRGB hook    | the layer comes before the target                |
-| StyleGAN2 with a ToRGB hook, per-layer latents, ``forward`` | always, the target included                      |
-| ProGAN                                                      | the layer comes before the target (the output    |
-|                                                             | block's result is the image ``forward`` returns) |
-| StyleGAN                                                    | before the target, or when the image is made     |
-| BigGAN                                                      | before the last layer run, or when the image is  |
-|                                                             | made                                             |
+| call path            | an edit raises when                                                                |
+|----------------------|------------------------------------------------------------------------------------|
+| StyleGAN2, StyleGAN  | the layer comes before the target, or when the image is made                       |
+| ProGAN               | the layer comes before the target (the output block's result is the image         |
+|                      | ``forward`` returns)                                                               |
+| BigGAN               | before the last layer run, or when the image is made                               |
 """
 from contextlib import contextmanager
 
@@ -48,12 +45,22 @@ def test_stylegan2_single_latent_partial_run():
 
 
 def test_stylegan2_per_layer_path():
+    """Per-layer latents, or a ToRGB hooked on the way: every ToRGB such a run executes comes before the target, so an edit of
+    the target is accepted; the ToRGB's own edit and that of the StyledConv a ToRGB target follows raise."""
     from ganspace_b200.models import StyleGAN2
     m = StyleGAN2(DEV, "cat", random_init=3)
     z, g = m.sample_latent(2, seed=1), m.model
-    with _hooked(g.to_rgb1, edit=False), _hooked(g.convs[0]), _raises():
+    with _hooked(g.to_rgb1, edit=False), _hooked(g.convs[0]):
         m.partial_forward(z, "convs.0")
-    with _hooked(g.convs[0]), _raises():
+    with _hooked(g.convs[0]):
+        m.partial_forward([z, z], "convs.0")
+    with _hooked(g.to_rgbs[0]):
+        m.partial_forward([z, z], "to_rgbs.0")
+    with _hooked(g.to_rgb1), _raises():
+        m.partial_forward(z, "convs.0")
+    with _hooked(g.convs[1]), _raises():
+        m.partial_forward([z, z], "to_rgbs.0")
+    with _hooked(g.conv1), _raises():
         m.partial_forward([z, z], "convs.0")
     with _hooked(g.to_rgbs[0]), _raises():
         m.forward(z)

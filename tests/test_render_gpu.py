@@ -77,7 +77,7 @@ def _per_layer_latents(seed, n):
 def test_each_styled_conv_vs_fp64(perturbed, name):
     """StyledConv ``name`` (layer l of the chain, latent l) fed the chain's own output of layer l-1 (the constant input for
     conv1) against the oracle's shared-weight form in fp64, on every element of a batch that spans two sample chunks of the
-    layer, one latent per sample and layer (gsb_synthesis_render with want_act).  Measured on an H100 80GB HBM3 (700 W): worst
+    layer, one latent per sample and layer (gsb_synthesis_forward).  Measured on an H100 80GB HBM3 (700 W): worst
     2.8e-6 (conv1), 1.7e-6 to 2.6e-6 for the 512-channel layers, under 1.4e-6 from convs.9 on."""
     m = perturbed
     l = CONV_NAMES.index(name)
@@ -92,8 +92,8 @@ def test_each_styled_conv_vs_fp64(perturbed, name):
     if l == 0:
         x = np.repeat(_np(m.model.input.input).astype(np.float64), n, axis=0)
     else:
-        x = nhwc_to_nchw(syn.render(wd, l, [], want_act=True)[0], n, *syn.shapes[l - 1])
-    got = nhwc_to_nchw(syn.render(wd, l + 1, [], want_act=True)[0], n, *syn.shapes[l])
+        x = nhwc_to_nchw(syn.forward(wd, l)[0], n, *syn.shapes[l - 1])
+    got = nhwc_to_nchw(syn.forward(wd, l + 1)[0], n, *syn.shapes[l])
     r = syn.shapes[l][0]
     L = dict(weight=_np(mod.conv.weight[0]), mod_weight=_np(mod.conv.modulation.weight), mod_bias=_np(mod.conv.modulation.bias),
              noise_weight=float(mod.noise.weight), act_bias=_np(mod.activate.bias), upsample=mod.conv.upsample)
@@ -119,12 +119,12 @@ def test_each_to_rgb_vs_fp64(perturbed, name):
     assert_spans_chunks(n, spc)
     w = _per_layer_latents(400 + j, n)
     wd = torch.from_numpy(w).to(m.device)
-    act, img = syn.render(wd, lj + 1, rgbs[:j + 1], want_act=True)
+    act, img = syn.forward(wd, lj + 1, n_rgb=j + 1)
     x = nhwc_to_nchw(act, n, *syn.shapes[lj])
     got = img.permute(0, 3, 1, 2).double().cpu().numpy()
     skip = None
     if j > 0:
-        skip = syn.render(wd, lj - 1, rgbs[:j])[1].permute(0, 3, 1, 2).double().cpu().numpy()
+        skip = syn.forward(wd, lj - 1, want_act=False, n_rgb=j)[1].permute(0, 3, 1, 2).double().cpu().numpy()
     R = {k: _np(v) for k, v in rgbs[j].items()}
     R["weight"] = R.pop("conv_weight")
     ref = oracle_go.to_rgb_forward(x, w[lj + 1], R, skip, dtype=np.float64)
@@ -204,3 +204,25 @@ def test_partial_forward_equals_forward_at_hooked_layer(model):
         model.forward(model.sample_latent(1, seed=1))
     inst.remove_edits()
     inst.close()
+
+
+def test_to_rgb_edit_in_place_repacks():
+    """The ToRGBs are packed with the chain: an in-place edit of a ToRGB's bias and modulation weight after a forward call shows in
+    the next image exactly as in a wrapper built with the edited weights."""
+    from ganspace_b200.models import StyleGAN2
+    dev = torch.device("cuda:0")
+
+    def edit(m):
+        with torch.no_grad():
+            m.model.to_rgbs[2].bias.add_(0.25)
+            m.model.to_rgbs[2].conv.modulation.weight.mul_(1.5)
+    m = StyleGAN2(dev, "cat", random_init=3)
+    z = m.sample_latent(3, seed=2)
+    before = m.forward(z)
+    edit(m)
+    after = m.forward(z)
+    fresh = StyleGAN2(dev, "cat", random_init=3)
+    edit(fresh)
+    assert torch.equal(after, fresh.forward(z))
+    assert (after - before).abs().max() > 1e-2
+    m.check_numerics()

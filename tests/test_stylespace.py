@@ -67,7 +67,8 @@ def test_oracle_edited_images_vs_reference(ka, params, mapping_weights, which):
 
 @pytest.mark.parametrize("cls", sorted(CLASSES))
 def test_style_layer_table(cls):
-    """name -> (chain layer, latent entry, width) for every modulation layer of the class's generator."""
+    """name -> (key, latent entry, width) for every modulation layer of the class's generator; the key is the position in the
+    table, in execution order."""
     from ganspace_b200.models import stylegan2
     g = stylegan2.Generator(CLASSES[cls], 512, 8)
     table = g.style_layers()
@@ -75,18 +76,19 @@ def test_style_layer_table(cls):
     assert {t[0] for t in table} == {n for n in mods if n.endswith(".conv.modulation")}
     n_conv = len(g.convs) + 1
     assert len(table) == n_conv + len(g.to_rgbs) + 1 == {1024: 26, 512: 23, 256: 20}[CLASSES[cls]]
-    for name, chain, idx, entry, width in table:
+    for pos, (name, key, entry, width) in enumerate(table):
         assert mods[name].weight.shape == (width, 512), name
+        assert key == pos, name
         if name == "conv1.conv.modulation":
-            assert (chain, idx, entry, width) == ("conv", 0, 0, 512)
+            assert (key, entry, width) == (0, 0, 512)
         elif name == "to_rgb1.conv.modulation":
-            assert (chain, idx, entry, width) == ("rgb", 0, 1, 512)
+            assert (key, entry, width) == (1, 1, 512)
         elif name.startswith("convs."):
-            k = int(name.split(".")[1])
-            assert (chain, idx, entry, width) == ("conv", k + 1, k + 1, g.convs[k].conv.in_channel), name
+            k = int(name.split(".")[1])            # chain layer l = k + 1, after the ToRGBs of layers 0, 2, .., < l
+            assert (key, entry, width) == (k + 1 + (k + 2) // 2, k + 1, g.convs[k].conv.in_channel), name
         else:
-            j = int(name.split(".")[1])
-            assert (chain, idx, entry, width) == ("rgb", j + 1, 2 * j + 3, g.convs[2 * j + 1].conv.out_channel), name
+            j = int(name.split(".")[1])            # ToRGB j + 1, after chain layer 2j + 2
+            assert (key, entry, width) == (3 * (j + 1) + 1, 2 * j + 3, g.convs[2 * j + 1].conv.out_channel), name
         assert entry < g.n_latent
     # execution order: conv1, to_rgb1, then per resolution convs.2j, convs.2j+1, to_rgbs.j
     assert [t[0].split(".conv")[0] for t in table[:5]] == ["conv1", "to_rgb1", "convs.0", "convs.1", "to_rgbs.0"]

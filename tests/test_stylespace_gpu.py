@@ -81,12 +81,15 @@ def test_style_rows_vs_fp64(model, params, n, w_layers):
     """gsb_synthesis_styles on every element of every S layer, below and above the 128-row switch of gsb_linear_forward."""
     w = torch.tensor(np.random.RandomState(n + w_layers).standard_normal((w_layers, n, 512)).astype(np.float32), device=DEV)
     syn = model._synthesis(17)
-    rgbs = [r.describe() for _, r in model.model.chain_layers()[1]]
-    S, R = syn.styles(w, range(17), range(9), rgbs)
+    table = model.model.style_layers()
+    S = syn.styles(w, range(len(table)))
+    convs, rgbs = model.model.chain_layers()
+    conv_idx = {f"{n}.conv.modulation": i for i, (n, _) in enumerate(convs)}
+    rgb_idx = {f"{n}.conv.modulation": j for j, (n, _) in enumerate(rgbs)}
     wn = w.double().cpu().numpy()
-    for name, chain, i, entry, width in model.model.style_layers():
-        got = (S if chain == "conv" else R)[i].cpu().numpy()
-        P = list(params["layers"].values())[i] if chain == "conv" else params["to_rgbs"][i]
+    for name, k, entry, width in table:
+        got = S[k].cpu().numpy()
+        P = list(params["layers"].values())[conv_idx[name]] if name in conv_idx else params["to_rgbs"][rgb_idx[name]]
         ref = so.modulation_forward(wn[min(entry, w_layers - 1)], P["mod_weight"], P["mod_bias"])
         assert got.shape == (n, width), name
         assert np.abs(got - ref).max() < MAP_TOL * max(1.0, np.abs(ref).max()), (name, np.abs(got - ref).max())
@@ -95,9 +98,8 @@ def test_style_rows_vs_fp64(model, params, n, w_layers):
 def test_partial_forward_to_style_layer_runs_no_synthesis(model):
     from ganspace_b200 import _native
     syn = model._synthesis(17)
-    rgbs = [r.describe() for _, r in model.model.chain_layers()[1]]
-    for layer, chain, i in (("convs.4.conv.modulation", "conv", 5), ("to_rgbs.2.conv.modulation", "rgb", 3),
-                            ("convs.12.conv.modulation", "conv", 13), ("conv1.conv.modulation", "conv", 0)):
+    keys = {t[0]: k for k, t in enumerate(model.model.style_layers())}
+    for layer in ("convs.4.conv.modulation", "to_rgbs.2.conv.modulation", "convs.12.conv.modulation", "conv1.conv.modulation"):
         inst = _inst(model, layer)
         z = model.sample_latent(200, seed=9)
         _native.instrument.reset()
@@ -105,8 +107,8 @@ def test_partial_forward_to_style_layer_runs_no_synthesis(model):
         assert "synthesis" not in _native.instrument.rows, layer
         got = inst.retained_features()[layer]
         w = model.model.style(z)
-        S, R = syn.styles(w[None], [i] if chain == "conv" else [], [i] if chain == "rgb" else [], rgbs)
-        assert torch.equal(got, (S if chain == "conv" else R)[i]), layer
+        k = keys[layer]
+        assert torch.equal(got, syn.styles(w[None], [k])[k]), layer
         inst.close()
 
 
@@ -127,20 +129,19 @@ def test_forward_with_style_hooks_is_bit_identical(model):
 
 
 def test_styled_run_is_the_chain_run(model):
-    """gsb_synthesis_render_styled on gsb_synthesis_styles' rows equals gsb_synthesis_render and gsb_synthesis_forward."""
+    """gsb_synthesis_forward_styled on gsb_synthesis_styles' rows equals gsb_synthesis_forward, with and without ToRGBs."""
     syn = model._synthesis(17)
-    rgbs = [r.describe() for _, r in model.model.chain_layers()[1]]
     # the whole chain at a small batch; to convs.7 (64 x 64) at a batch past the 128-row switch of the style GEMMs
     for n, Lw, n_run in ((5, 18, 17), (130, 1, 9)):
         n_rgb = (n_run - 1) // 2 + 1
         w = torch.tensor(np.random.RandomState(n).standard_normal((Lw, n, 512)).astype(np.float32), device=DEV)
-        S, R = syn.styles(w, range(n_run), range(n_rgb), rgbs)
-        act, img = syn.render(w, n_run, rgbs[:n_rgb], want_act=True)
-        act2, img2 = syn.render_styled([S[l] for l in range(n_run)], [R[j] for j in range(n_rgb)], n_run, rgbs[:n_rgb], want_act=True)
+        S = syn.styles(w, [syn.slot_of["conv", l] for l in range(n_run)] + [syn.slot_of["rgb", j] for j in range(n_rgb)])
+        act, img = syn.forward(w, n_run, n_rgb=n_rgb)
+        act2, img2 = syn.forward_styled(S, n_run, n_rgb=n_rgb)
         assert torch.equal(act, act2) and torch.equal(img, img2)
         if Lw == 1:
-            a5 = syn.forward(w[0], 6)
-            assert torch.equal(a5, syn.render_styled([S[l] for l in range(6)], [], 6, [], want_act=True)[0])
+            a5 = syn.forward(w[0], 6)[0]
+            assert torch.equal(a5, syn.forward_styled(S, 6)[0])
     model.check_numerics()
 
 
@@ -232,11 +233,11 @@ def test_notebook_activation_strip_on_style_layer(model):
     inst.close()
     # explicitly: the styles of the batch, edited, through the styled chain
     syn = model._synthesis(17)
-    rgbs = [r.describe() for _, r in model.model.chain_layers()[1]]
+    keys = {t[0]: k for k, t in enumerate(model.model.style_layers())}
     w = model.model.style(z_single.repeat_interleave(B, axis=0))[None]
-    S, R = syn.styles(w, range(17), range(9), rgbs)
-    S[4] = S[4] + (delta * act_stdev - zero)
-    _, img = syn.render_styled([S[l] for l in range(17)], [R[j] for j in range(9)], 17, rgbs)
+    S = syn.styles(w, keys.values())
+    S[keys[layer]] = S[keys[layer]] + (delta * act_stdev - zero)
+    _, img = syn.forward_styled(S, 17, want_act=False, n_rgb=9)
     ref = np.clip((0.5 * (img + 1)).cpu().numpy(), 0.0, 1.0)
     assert np.array_equal(frames, ref)
     assert np.abs(frames[0] - frames[-1]).max() > 1e-2
