@@ -101,6 +101,7 @@ SIGNATURES = {
     "gsb_fbpca_workspace_bytes": (_Z, [_I, _I, _I]),
     "gsb_fbpca_solve": (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _Z, _P]),
     "gsb_fbpca_status": (_I, [_P, _I, _P, _P]),
+    "gsb_fbpca_project_omega": (_I, [_P, _I, _I, _P, _I, _P, _P]),
 }
 
 
@@ -1299,6 +1300,19 @@ class BigIPCA:
         full = torch.empty((W * n, dl), dtype=local.dtype, device=local.device)
         dist.all_gather_into_tensor(full, local)
         return full.view(W, n, dl).permute(1, 0, 2).reshape(n, W * dl).contiguous()
+
+
+def fbpca_project_omega(Q: torch.Tensor, omega: torch.Tensor) -> torch.Tensor:
+    """Q^T Omega [r, l] fp64 for Q [d, r] fp64 and fbpca's test matrix Omega [d, l] fp32 (csrc/rsvd.cu, fp64 tensor cores)."""
+    assert Q.is_cuda and Q.dtype == torch.float64 and omega.dtype == torch.float32 and Q.dim() == omega.dim() == 2
+    assert omega.device == Q.device and omega.shape[0] == Q.shape[0]
+    Q, omega = Q.contiguous(), omega.contiguous()
+    (d, r), l = Q.shape, omega.shape[1]
+    out = torch.empty((r, l), dtype=torch.float64, device=Q.device)
+    with torch.cuda.device(Q.device), instrument.section("fbpca_project_omega"):
+        _check(load().gsb_fbpca_project_omega(_ptr(Q), d, r, _ptr(omega), l, _ptr(out), _stream()), "gsb_fbpca_project_omega")
+    instrument.count(1)
+    return out
 
 
 class FBPCARankError(NativeError):

@@ -167,6 +167,57 @@ int fb_gemm(int M, int N, int K, const double *A, int lda, const double *B, int 
 }
 
 // ---------------------------------------------------------------------------------------------
+// Omega' = Q^T Omega  [r, l]:  Q [d, r] fp64, Omega [d, l] fp32 (fbpca's test matrix as drawn), a reduction over a long d
+// (32768 at BigGAN's gen_z).  fb_gemm_kernel's warp tile, with the k-steps of d dealt round-robin to FP_SPLIT groups of
+// four warps; the groups' partial 32 x 32 tiles are then summed in shared memory in group order (deterministic).
+// ---------------------------------------------------------------------------------------------
+constexpr int FP_SPLIT = 4;
+
+__global__ void __launch_bounds__(128 * FP_SPLIT) fb_project_kernel(int r, int l, int d, const double *__restrict__ Q,
+                                                                    const float *__restrict__ Om, double *__restrict__ out) {
+    __shared__ double part[FP_SPLIT - 1][32][33];
+    const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3, grp = threadIdx.x >> 7, g = lane >> 2, t = lane & 3;
+    const int row = blockIdx.y * 32 + warp * 8 + g, n0 = blockIdx.x * 32;
+    double acc[FG_NT][2];
+#pragma unroll
+    for (int b = 0; b < FG_NT; ++b) { acc[b][0] = 0.0; acc[b][1] = 0.0; }
+#pragma unroll 4
+    for (int k0 = 4 * grp; k0 < d; k0 += 4 * FP_SPLIT) {
+        const int k = k0 + t;
+        double a = 0.0;
+        if (row < r && k < d) a = Q[(size_t)k * r + row];
+#pragma unroll
+        for (int b = 0; b < FG_NT; ++b) {
+            const int n = n0 + 8 * b + g;
+            double bv = 0.0;
+            if (n < l && k < d) bv = (double)Om[(size_t)k * l + n];
+            fb_dmma(acc[b][0], acc[b][1], a, bv);
+        }
+    }
+    const int lr = warp * 8 + g;                 // accumulator (lr, 8 b + 2 t + {0, 1}) of the CTA's tile
+    if (grp > 0) {
+#pragma unroll
+        for (int b = 0; b < FG_NT; ++b) {
+            part[grp - 1][lr][8 * b + 2 * t] = acc[b][0];
+            part[grp - 1][lr][8 * b + 2 * t + 1] = acc[b][1];
+        }
+    }
+    __syncthreads();
+    if (grp > 0 || row >= r) return;
+#pragma unroll
+    for (int b = 0; b < FG_NT; ++b) {
+        double s0 = acc[b][0], s1 = acc[b][1];
+        for (int q = 0; q < FP_SPLIT - 1; ++q) {
+            s0 += part[q][lr][8 * b + 2 * t];
+            s1 += part[q][lr][8 * b + 2 * t + 1];
+        }
+        const int col = n0 + 8 * b + 2 * t;
+        if (col < l) out[(size_t)row * l + col] = s0;
+        if (col + 1 < l) out[(size_t)row * l + col + 1] = s1;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // In-place lower Cholesky of A[n,n] (row stride lda; the upper triangle is ignored), one CTA, Crout order: column j is
 //   L_jj = sqrt(A_jj - sum_k<j L_jk^2),   L_ij = (A_ij - sum_k<j L_ik L_jk) / L_jj   (i > j, one warp per row, coalesced)
 // A pivot <= 1e-12 max_i A_ii (the matrix is not numerically positive definite: the data's rank is below l) sets bit0 of
@@ -405,6 +456,17 @@ extern "C" int gsb_fbpca_solve(void *d_state, int d, int c, int l, int flags, co
     GSB_CHECK_LAUNCH();
     if (int r = sign_rows(d_components, c, d, st)) return r;
     if (d_mean) GSB_CHECK_CUDA(cudaMemcpyAsync(d_mean, s.mean, (size_t)d * 8, cudaMemcpyDeviceToDevice, st));
+    return GSB_OK;
+}
+
+extern "C" int gsb_fbpca_project_omega(const double *d_Q, int d, int r, const float *d_omega, int l, double *d_omega_r,
+                                       gsb_stream_t stream) {
+    GSB_CHECK_ARG(d_Q && d_omega && d_omega_r, "fbpca_project_omega: null pointer");
+    GSB_CHECK_ARG(d >= 1 && r >= 1 && r <= 1024 && l >= 1 && l <= 1024,
+                  "fbpca_project_omega: needs d >= 1, 1 <= r <= 1024, 1 <= l <= 1024 (d=%d r=%d l=%d)", d, r, l);
+    dim3 grid((l + 31) / 32, (r + 31) / 32);
+    gsb::fb_project_kernel<<<grid, 128 * gsb::FP_SPLIT, 0, (cudaStream_t)stream>>>(r, l, d, d_Q, d_omega, d_omega_r);
+    GSB_CHECK_LAUNCH();
     return GSB_OK;
 }
 

@@ -303,8 +303,10 @@ def compute_arrays(config, instrumented_model, state=None):
     pooled = not transformer.batch_support
     samples_are_latents = layer_key in ["g_mapping", "style"] and inst.model.latent_space_name() == "W"
     if pooled and affine is not None:
-        raise NotImplementedError(f"--est {config.estimator} is not available for layer {layer_key} (an affine layer: the "
-                                  "test matrix would have to be projected through its isometry); use --est ipca")
+        # fbpca decomposes the stacked sample matrix, whose unfilled tail rows are zero activations, outside the affine image:
+        # in the layer's linear form act = yt Qt^T (Qt: Q and the offset's direction) they are zero coordinates, so the pool
+        # of coordinate statistics is the stacked matrix's (DESIGN.md section 5g)
+        affine = affine.linear_form()
     # conv feature maps (d up to ~10^6): the large-d IPCA engine keeps sklearn's stacked matrix in HBM and the model's
     # producer kernels write each batch into it in the device feature order (NHWC); the fixed NHWC->NCHW permutation
     # is applied once to the exported components (PCA is equivariant under it)
@@ -340,7 +342,17 @@ def compute_arrays(config, instrumented_model, state=None):
     seeds = _draw_seeds(pl.n_calls)
     # fbpca draws its test matrix from the global state when it fits, after the collection (:284) and before the W-space
     # lat_stdev seed (:327); nothing in between draws, so it is the next draw here
-    omega = transformer.draw_omega(N + NB, sample_dims) if pooled else None
+    if pooled and affine is not None and transformer.l >= affine.rank:
+        # fbpca's range covers every direction of the rank-deficient samples: its exact branch, which needs no test matrix.
+        # The reference still draws one here, but the next reader of the global state is the regression pass, which re-seeds
+        # it first (np.random.seed(SEED_LINREG), decomposition.py:81), so skipping the draw changes no later draw.
+        omega = None
+    elif pooled and affine is not None and transformer.randomized(N + NB, sample_dims) and N + NB < sample_dims:
+        raise NotImplementedError(f"--est {config.estimator} on layer {layer_key} with l = {transformer.l} < rank "
+                                  f"{affine.rank} needs N + NB >= {sample_dims} samples (with fewer, fbpca draws its test "
+                                  "matrix over the samples); use more samples, more components or --est ipca")
+    else:
+        omega = transformer.draw_omega(N + NB, sample_dims) if pooled else None
     # W-space runs end with model.sample_latent(5000) for lat_stdev (:325-329).  Without a regression pass nothing touches the
     # global NumPy state in between, so its seed is the next draw; its latent stream (one sequential MT19937 stream, ~6 ms on
     # one SM) is generated on a side stream while the run proceeds instead of at the tail of the critical path.
@@ -350,7 +362,7 @@ def compute_arrays(config, instrumented_model, state=None):
 
     # ---- Phase B: per-group statistics + merge chain (:239-265) ------------------------------------
     K = pl.K
-    d = affine.rank if affine is not None else sample_dims
+    d = affine.Q.shape[1] if affine is not None else sample_dims
     groups_per_chunk = max(1, int(LATENT_CHUNK_BYTES // max(1, NB * input_dims * 4)))
     X = None
     tr = transformer.transformer
@@ -484,7 +496,10 @@ def compute_arrays(config, instrumented_model, state=None):
             import torch.distributed as dist
             dist.all_reduce(first)                               # each row is non-zero on exactly one rank
         transformer.add_zero_rows(N + NB - K * NB)               # the unfilled tail of the sample matrix (:224)
-        transformer.fit_pooled(omega=omega)
+        if affine is not None:
+            transformer.fit_pooled_affine(omega, affine.Q, affine.rank)
+        else:
+            transformer.fit_pooled(omega=omega)
     tick("sampling + activations + IPCA chain")
     # host work that does not depend on the chain's result, done while the device still runs the last merge steps (the
     # export below is the first call that waits for them): get_random_dirs' host stream + upload, the lat_stdev latents
@@ -505,7 +520,7 @@ def compute_arrays(config, instrumented_model, state=None):
         idx = torch.argmax(lifted.abs(), dim=1)
         signs = torch.sign(lifted[torch.arange(lifted.shape[0], device=device), idx])
         Y_comp = X_comp * signs.cpu().numpy()[:, None]
-        Y_mean = tr.mean_.reshape((1, d))
+        Y_mean = (transformer.pooled_mean if pooled else tr.mean_).reshape((1, d))
         X_comp = (lifted * signs[:, None]).cpu().numpy()
         X_global_mean = (affine.lift_rows(mean_dev[None, :]) + affine.offset[None, :]).cpu().numpy()
 

@@ -307,7 +307,26 @@ class FacebookPCAEstimator:
             raise ValueError(f"n_components={c} must be in [1, min(n_samples, n_features)] = [1, {min(pool.n, d)}]")
         if omega is not None:
             omega = torch.as_tensor(np.asarray(omega, dtype=np.float64) if isinstance(omega, np.ndarray) else omega)
-        out = pool.solve(c, self.l, omega=omega, raw=raw)
+        self._finish(pool.solve(c, self.l, omega=omega, raw=raw), raw)
+
+    def fit_pooled_affine(self, omega, Q, rank):
+        """fit_pooled for samples pooled in the coordinates of a basis: activation rows x = y Q^T with Q [D, d] (fp64 device,
+        orthonormal columns, zero padding columns allowed) and y the pooled d-vectors, the stacked matrix of rank ``rank``.
+        ``omega`` [D, l]: fbpca's test matrix of the D-wide activations (None: its exact branch).  fbpca depends on Omega only
+        through range(G^2 Omega) = Q range(G_y^2 Q^T Omega) (G = Q G_y Q^T): for l < rank the randomized solve runs on the pool
+        with Q^T Omega; for l >= rank that range is all of range(G), so fbpca's result is the exact top-c PCA (DESIGN.md
+        section 5g).  Components, mean and the sign rule stay in y-coordinates (the caller lifts them); stdev and var_ratio
+        are those of the activations, Q being an isometry on the pooled rows."""
+        c, pool = self.n_components, self._pool
+        if not (1 <= c <= min(pool.n, rank)):
+            raise ValueError(f"n_components={c} must be in [1, min(n_samples, rank)] = [1, {min(pool.n, rank)}]")
+        omega_y = None
+        if omega is not None and self.l < rank:
+            omega_y = _native.fbpca_project_omega(Q, torch.as_tensor(omega).to(Q.device, torch.float32))
+        self._finish(pool.solve(c, self.l, omega=omega_y), raw=False)
+
+    def _finish(self, out, raw):
+        c, d = self.n_components, self._pool.d
         self.device_outputs = out
         flat = torch.cat([out["components"].reshape(-1), out["stdev"], out["var_ratio"], out["mean"]]).cpu().numpy()
         comp, rest = flat[:c * d].reshape(c, d), flat[c * d:]

@@ -282,17 +282,40 @@ def synthesis_fill(net, seed=0):
 class AffineLayer:
     """act = y Q^T + offset,  y = z R^T  (see module docstring).  All device tensors."""
 
-    def __init__(self, Q64, R64, offset64):
+    def __init__(self, Q64, R64, offset64, shift64=None, rank=None):
         self.Q = Q64                                   # [d, r] fp64, orthonormal columns
         self.Q32 = Q64.float().contiguous()
         self.R32 = R64.float().contiguous()           # [r, r]
         self.offset = offset64                         # [d] fp64: b + W_eff[:, r:] @ embed
-        self.rank = Q64.shape[1]
+        self.shift32 = None if shift64 is None else shift64.float().contiguous()
+        self.rank = Q64.shape[1] if rank is None else rank
         self.dim = Q64.shape[0]
 
     def coords(self, z: torch.Tensor) -> torch.Tensor:
-        """y = z R^T through the fp32 GEMM kernel."""
-        return _native.linear(z, self.R32)
+        """y = z R^T (+ shift) through the fp32 GEMM kernel."""
+        return _native.linear(z, self.R32, self.shift32)
+
+    def linear_form(self):
+        """The same map with no offset: act = yt Qt^T, Qt = [Q, q_o, 0] and yt = z Rt^T + t = [y + Q^T offset, |o_perp|, 0],
+        where o_perp = offset - Q Q^T offset and q_o = o_perp / |o_perp|.  A zero activation row is then a zero coordinate
+        row, which fbpca's zero-padded sample matrix needs (DESIGN.md section 5g).  The width is padded to a multiple of 128
+        (the GEMM kernel's output tile); ``rank`` is r + 1, or r when the offset lies in range(Q)."""
+        d, r = self.Q.shape
+        w = (r + 1 + 127) // 128 * 128
+        a = self.Q.T @ self.offset
+        perp = self.offset - self.Q @ a
+        b = torch.linalg.vector_norm(perp)
+        inside = bool(b <= 1e-12 * torch.linalg.vector_norm(self.offset))
+        Qt = torch.zeros((d, w), dtype=torch.float64, device=self.Q.device)
+        Qt[:, :r] = self.Q
+        Rt = torch.zeros((w, self.R32.shape[1]), dtype=torch.float64, device=self.Q.device)
+        Rt[:r] = self.R32.double()
+        t = torch.zeros(w, dtype=torch.float64, device=self.Q.device)
+        t[:r] = a
+        if not inside:
+            Qt[:, r] = perp / b
+            t[r] = b
+        return AffineLayer(Qt, Rt, torch.zeros_like(self.offset), shift64=t, rank=r + (0 if inside else 1))
 
     def lift_rows(self, rows64: torch.Tensor) -> torch.Tensor:
         """rows [k, r] in y-space -> [k, d] in activation space (directions: no offset); in-tree GEMM kernel, fp32 (the

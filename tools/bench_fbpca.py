@@ -6,6 +6,10 @@ eigensolve + stdevs).  Prints one JSON line and writes it to --out.
     python tools/bench_fbpca.py [--steps 5] [--n 1000000]          (GPU)
     python tools/bench_fbpca.py --reference-cpu [--ref-n 40000]     (CPU: the unmodified reference with the restated fbpca
                                                                      installed as its fbpca module, bounded N, labelled so)
+    python tools/bench_fbpca.py --config4 [--steps 5]               (GPU: config 4's layer, BigGAN-512 husky random-init
+                                                                     generator.gen_z, N = 1e6, B = 1e4: fbpca at c = 16 and
+                                                                     c = 80, each alternated with ipca at the same c, and the
+                                                                     host draw of fbpca's [32768, 32] test matrix alone)
 """
 import argparse
 import json
@@ -72,6 +76,51 @@ def run_gpu(args):
     return res
 
 
+def run_config4(args):
+    """gen_z: l = 32 < rank takes the randomized branch (host draw of Omega + projection), l = 160 the exact one."""
+    import numpy as np
+    import torch
+    from ganspace_b200 import decomposition
+    from ganspace_b200.config import Config
+    from ganspace_b200.models import get_instrumented_model
+    from ganspace_b200.models.biggan import BigGAN
+    dev = torch.device("cuda:0")
+    model = BigGAN(dev, 512, "husky", random_init=4321)
+    inst = get_instrumented_model("BigGAN-512", "husky", "generator.gen_z", dev, model=model)
+
+    def job(est, c, tmp):
+        cfg = Config(model="BigGAN-512", layer="generator.gen_z", output_class="husky", components=c, n=args.n,
+                     batch_size=args.batch, estimator=est)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        decomposition.get_or_compute(cfg, inst, submit_config=SimpleNamespace(run_dir=tmp, run_dir_root=tmp),
+                                     force_recompute=True)
+        torch.cuda.synchronize()
+        return (time.perf_counter() - t0) * 1e3
+
+    jobs = [("fbpca", 16), ("ipca", 16), ("fbpca", 80), ("ipca", 80)]
+    times = {f"{e}_c{c}": [] for e, c in jobs}
+    with tempfile.TemporaryDirectory() as tmp:
+        for _ in range(args.warmup):
+            for e, c in jobs:
+                job(e, c, tmp)
+        for _ in range(args.steps):
+            for e, c in jobs:
+                times[f"{e}_c{c}"].append(job(e, c, tmp))
+    draw = []
+    for _ in range(5):
+        t0 = time.perf_counter()
+        np.random.uniform(low=-1.0, high=1.0, size=(32768, 32)).astype(np.float32)
+        draw.append((time.perf_counter() - t0) * 1e3)
+    return {
+        "shape": f"BigGAN-512 husky random-init generator.gen_z N={args.n} B={args.batch}",
+        "gpu": _gpu_info(),
+        "ms_per_job": {k: [round(t, 1) for t in v] for k, v in times.items()},
+        "ms_per_job_median": {k: round(sorted(v)[len(v) // 2], 1) for k, v in times.items()},
+        "host_omega_draw_ms_c16": [round(t, 2) for t in draw],
+    }
+
+
 def run_profile(args):
     """Kernel table of the solve alone (torch.profiler, CUDA activities) on a synthetic pooled state of the bench's shape."""
     import numpy as np
@@ -126,11 +175,14 @@ def main():
     ap.add_argument("--reference-cpu", dest="reference_cpu", action="store_true")
     ap.add_argument("--ref-n", dest="ref_n", type=int, default=40_000)
     ap.add_argument("--profile", action="store_true")
+    ap.add_argument("--config4", action="store_true")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if args.profile:
         res = run_profile(args)
         print(res["profile_5_solves"])
+    elif args.config4:
+        res = run_config4(args)
     else:
         res = run_reference_cpu(args) if args.reference_cpu else run_gpu(args)
     line = json.dumps(res)
