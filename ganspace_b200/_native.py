@@ -81,6 +81,8 @@ SIGNATURES = {
     "gsb_stylegan_forward_styled": (_I, [_P, _P, _I, _I, _I, _P, _L, _P, _L, _P, _P, _Z, _P]),
     "gsb_biggan_conv_forward": (_I, [_P, _L, _P]),
     "gsb_biggan_bn_table": (_I, [_P, _L, _I, _P, _P, _P, _F, _I, _P, _P, _P]),
+    "gsb_biggan_bn_rows": (_I, [_P, _L, _I, _P, _I, _P]),
+    "gsb_biggan_bn_table_rows": (_I, [_P, _L, _P, _L, _L, _P, _F, _I, _P, _P, _P]),
     "gsb_biggan_attn_pool": (_I, [_P, _L, _I, _I, _P, _P, _P]),
     "gsb_biggan_softmax_rows": (_I, [_P, _L, _I, _P]),
     "gsb_biggan_rgb": (_I, [_P, _L, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
@@ -138,6 +140,12 @@ class BigGANConvDesc(C.Structure):
                 ("weight", C.c_void_p), ("w_sample_stride", C.c_int64), ("cout", C.c_int), ("bias", C.c_void_p),
                 ("alpha", C.c_float), ("res", C.c_void_p), ("ldres", C.c_int64), ("res_upsample", C.c_int), ("out", C.c_void_p),
                 ("ldo", C.c_int64)]
+
+
+class BigGANBnRowsDesc(C.Structure):
+    """``gsb_biggan_bn_rows_desc`` of include/ganspace_b200.h."""
+    _fields_ = [("w_scale", C.c_void_p), ("w_offset", C.c_void_p), ("c", C.c_int), ("scale_rows", C.c_void_p),
+                ("offset_rows", C.c_void_p)]
 
 
 class NativeError(RuntimeError):
@@ -1140,6 +1148,41 @@ def biggan_bn_table(cond, w_scale, w_offset, var, eps, scale_out, offset_out):
         _check(load().gsb_biggan_bn_table(_f32_dev(cond, "cond"), n, cdim, _f32_dev(w_scale, "w_scale"), _f32_dev(w_offset, "w_offset"),
                                           _f32_dev(var, "var"), float(eps), var.numel(), _f32_dev(scale_out, "scale"),
                                           _f32_dev(offset_out, "offset"), _stream()), "gsb_biggan_bn_table")
+    instrument.count(1)
+
+
+def biggan_bn_rows(cond, bns):
+    """One gsb_biggan_bn_rows launch: for each (w_scale [C, cdim], w_offset [C, cdim]) of ``bns`` (at most 4, the BatchNorms of one
+    block), the rows (cond w_scale^T, cond w_offset^T) [n, C] each, in the dot-product order of gsb_biggan_bn_table."""
+    n, cdim = cond.shape
+    descs = (BigGANBnRowsDesc * len(bns))()
+    out = []
+    for d, (ws, wo) in zip(descs, bns):
+        s, o = (torch.empty((n, ws.shape[0]), dtype=torch.float32, device=cond.device) for _ in range(2))
+        d.w_scale, d.w_offset = _f32_dev(ws, "w_scale").value, _f32_dev(wo, "w_offset").value
+        d.c, d.scale_rows, d.offset_rows = ws.shape[0], s.data_ptr(), o.data_ptr()
+        out.append((s, o))
+    with torch.cuda.device(cond.device):
+        _check(load().gsb_biggan_bn_rows(_f32_dev(cond, "cond"), n, cdim, C.cast(descs, C.c_void_p), len(bns), _stream()), "gsb_biggan_bn_rows")
+    instrument.count(1)
+    return out
+
+
+def _bn_rows_operand(rows, n, c, what):
+    """(tensor, row stride) of BatchNorm rows [n, c] or [1, c] (stride 0: the one row applies to every sample)."""
+    assert rows.is_cuda and rows.dtype == torch.float32 and rows.dim() == 2 and rows.shape[1] == c and rows.shape[0] in (1, n) \
+        and rows.stride(1) == 1, f"{what}: fp32 device rows [{n}, {c}] or [1, {c}] with unit column stride expected"
+    return C.c_void_p(rows.data_ptr()), (rows.stride(0) if rows.shape[0] == n and n > 1 else 0)
+
+
+def biggan_bn_table_rows(scale_rows, offset_rows, var, eps, scale_out, offset_out):
+    """gsb_biggan_bn_table_rows: the BatchNorm tables [n, C] from given rows [n, C] (row-strided) or [1, C]."""
+    n, c = scale_out.shape
+    ps, ls = _bn_rows_operand(scale_rows, n, c, "scale rows")
+    po, lo = _bn_rows_operand(offset_rows, n, c, "offset rows")
+    with torch.cuda.device(scale_out.device):
+        _check(load().gsb_biggan_bn_table_rows(ps, ls, po, lo, n, _f32_dev(var, "var"), float(eps), c, _f32_dev(scale_out, "scale"),
+                                               _f32_dev(offset_out, "offset"), _stream()), "gsb_biggan_bn_table_rows")
     instrument.count(1)
 
 

@@ -130,7 +130,21 @@ bb_conv_kernel(const gsb_biggan_conv c, int64_t n) {
     }
 }
 
-// ---- conditional BatchNorm tables -----------------------------------------------------------------------------------------
+// ---- conditional BatchNorm rows and tables --------------------------------------------------------------------------------
+// The rows s = cond_b . Ws[ch] and o = cond_b . Wo[ch] of one (sample, channel), reduced across the calling warp: lane-strided
+// fmaf over k, then warp_sum.  Every kernel that forms these rows calls this, so the fused tables and the tables built from
+// materialised rows hold the same bits.
+__device__ __forceinline__ float2 bb_cond_rows(const float *__restrict__ cond_b, const float *__restrict__ ws_ch,
+                                               const float *__restrict__ wo_ch, int cdim, int lane) {
+    float s = 0.f, o = 0.f;
+    for (int k = lane; k < cdim; k += 32) {
+        const float z = cond_b[k];
+        s = fmaf(z, ws_ch[k], s);
+        o = fmaf(z, wo_ch[k], o);
+    }
+    return make_float2(warp_sum(s), warp_sum(o));
+}
+
 // scale[b, ch] = (1 + cond_b . Ws[ch]) / sqrt(var[ch] + eps),  offset[b, ch] = cond_b . Wo[ch]   (one warp per (b, ch))
 __global__ void __launch_bounds__(256)
 bb_bn_table_kernel(const float *__restrict__ cond, int64_t n, int cdim, const float *__restrict__ ws, const float *__restrict__ wo,
@@ -140,18 +154,51 @@ bb_bn_table_kernel(const float *__restrict__ cond, int64_t n, int cdim, const fl
     if (w >= n * C) return;
     const int64_t b = w / C;
     const int ch = (int)(w % C);
-    float s = 0.f, o = 0.f;
-    for (int k = lane; k < cdim; k += 32) {
-        const float z = cond[b * cdim + k];
-        s = fmaf(z, ws[(int64_t)ch * cdim + k], s);
-        o = fmaf(z, wo[(int64_t)ch * cdim + k], o);
-    }
-    s = warp_sum(s);
-    o = warp_sum(o);
+    const float2 r = bb_cond_rows(cond + b * cdim, ws + (int64_t)ch * cdim, wo + (int64_t)ch * cdim, cdim, lane);
     if (lane == 0) {
-        scale[w] = (1.f + s) / sqrtf(var[ch] + eps);
-        offset[w] = o;
+        scale[w] = (1.f + r.x) / sqrtf(var[ch] + eps);
+        offset[w] = r.y;
     }
+}
+
+// The rows of up to GSB_BIGGAN_BN_ROWS_MAX BatchNorms of one block in one launch: one warp per (b, channel of the concatenated
+// [C_0 | C_1 | ...]), s and o written to the BatchNorm's own [n, C_j] outputs.
+struct bb_bn_rows_args {
+    gsb_biggan_bn_rows_desc d[GSB_BIGGAN_BN_ROWS_MAX];
+    int64_t start[GSB_BIGGAN_BN_ROWS_MAX + 1];     // prefix sums of the widths
+    int count;
+};
+
+__global__ void __launch_bounds__(256)
+bb_bn_rows_kernel(const float *__restrict__ cond, int64_t n, int cdim, const bb_bn_rows_args a) {
+    const int64_t w = blockIdx.x * (int64_t)(blockDim.x >> 5) + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    const int64_t total = a.start[a.count];
+    if (w >= n * total) return;
+    const int64_t b = w / total;
+    const int64_t g = w % total;
+    int j = 0;
+    while (g >= a.start[j + 1]) ++j;
+    const gsb_biggan_bn_rows_desc &d = a.d[j];
+    const int ch = (int)(g - a.start[j]);
+    const float2 r = bb_cond_rows(cond + b * cdim, d.w_scale + (int64_t)ch * cdim, d.w_offset + (int64_t)ch * cdim, cdim, lane);
+    if (lane == 0) {
+        d.scale_rows[b * d.c + ch] = r.x;
+        d.offset_rows[b * d.c + ch] = r.y;
+    }
+}
+
+// tables from given rows: scale[b, ch] = (1 + s[b, ch]) / sqrt(var[ch] + eps), offset[b, ch] = o[b, ch]; row b of s at s + b ld_s
+// (ld_s = 0: one row for every sample), likewise o.  One thread per element.
+__global__ void __launch_bounds__(256)
+bb_bn_table_rows_kernel(const float *__restrict__ s, int64_t ld_s, const float *__restrict__ o, int64_t ld_o, int64_t n,
+                        const float *__restrict__ var, float eps, int C, float *__restrict__ scale, float *__restrict__ offset) {
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i >= n * C) return;
+    const int64_t b = i / C;
+    const int ch = (int)(i % C);
+    scale[i] = (1.f + s[b * ld_s + ch]) / sqrtf(var[ch] + eps);
+    offset[i] = o[b * ld_o + ch];
 }
 
 // ---- SelfAttn: 2x2 max-pool of phi (written K-major for the score product) and g -------------------------------------------
@@ -263,6 +310,42 @@ extern "C" int gsb_biggan_bn_table(const float *d_cond, int64_t n, int cdim, con
     const int64_t warps = n * c;
     bb_bn_table_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, (cudaStream_t)stream>>>(d_cond, n, cdim, d_w_scale, d_w_offset, d_var,
                                                                                      eps, c, d_scale, d_offset);
+    GSB_CHECK_LAUNCH();
+    return GSB_OK;
+}
+
+extern "C" int gsb_biggan_bn_rows(const float *d_cond, int64_t n, int cdim, const gsb_biggan_bn_rows_desc *descs, int count,
+                                  gsb_stream_t stream) {
+    using namespace gsb;
+    GSB_CHECK_ARG(d_cond && descs && n >= 0 && cdim > 0 && count >= 1 && count <= GSB_BIGGAN_BN_ROWS_MAX,
+                  "biggan_bn_rows: bad argument (count=%d, at most %d)", count, GSB_BIGGAN_BN_ROWS_MAX);
+    bb_bn_rows_args a;
+    a.count = count;
+    a.start[0] = 0;
+    for (int j = 0; j < count; ++j) {
+        const gsb_biggan_bn_rows_desc &d = descs[j];
+        GSB_CHECK_ARG(d.w_scale && d.w_offset && d.scale_rows && d.offset_rows && d.c > 0, "biggan_bn_rows: bad descriptor %d", j);
+        a.d[j] = d;
+        a.start[j + 1] = a.start[j] + d.c;
+    }
+    if (n == 0) return GSB_OK;
+    const int64_t warps = n * a.start[count];
+    bb_bn_rows_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, (cudaStream_t)stream>>>(d_cond, n, cdim, a);
+    GSB_CHECK_LAUNCH();
+    return GSB_OK;
+}
+
+extern "C" int gsb_biggan_bn_table_rows(const float *d_scale_rows, int64_t ld_scale_rows, const float *d_offset_rows,
+                                        int64_t ld_offset_rows, int64_t n, const float *d_var, float eps, int c, float *d_scale,
+                                        float *d_offset, gsb_stream_t stream) {
+    using namespace gsb;
+    GSB_CHECK_ARG(d_scale_rows && d_offset_rows && d_var && d_scale && d_offset && n >= 0 && c > 0 &&
+                      (ld_scale_rows == 0 || ld_scale_rows >= c) && (ld_offset_rows == 0 || ld_offset_rows >= c),
+                  "biggan_bn_table_rows: bad argument (c=%d, ld=%lld, %lld)", c, (long long)ld_scale_rows, (long long)ld_offset_rows);
+    if (n == 0) return GSB_OK;
+    const int64_t total = n * c;
+    bb_bn_table_rows_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+        d_scale_rows, ld_scale_rows, d_offset_rows, ld_offset_rows, n, d_var, eps, c, d_scale, d_offset);
     GSB_CHECK_LAUNCH();
     return GSB_OK;
 }

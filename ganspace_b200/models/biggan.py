@@ -19,7 +19,8 @@ and reuses the small-d engine.  ``partial_forward`` still produces the full acti
 
 Synthesis (``forward``, ``partial_forward`` to ``generator.layers.k``): the reference's module tree (GenBlock, SelfAttn,
 BigGANBatchNorm, generator.bn, conv_to_rgb; same names, shapes and creation order) holds the parameters, and ``_Chain`` runs
-them on the kernels of csrc/biggan.cu (DESIGN.md section 5i).  Decomposing a layer other than gen_z is not built and raises.
+them on the kernels of csrc/biggan.cu (DESIGN.md section 5i).  The conditional-BatchNorm row layers generator.layers.k.bn_j.scale /
+.offset are affine in z as well (``affine_layer``, ``style_layers``); decomposing any other generator layer raises.
 """
 from __future__ import annotations
 
@@ -50,6 +51,15 @@ _LAYERS = {
           (True, 8, 4), (False, 4, 4), (True, 4, 2), (False, 2, 2), (True, 2, 1), (False, 1, 1), (True, 1, 1)],
 }
 _CHANNEL_WIDTH = 128
+
+
+_ROW_LAYER = re.compile(r"^generator\.layers\.([0-9]+)\.bn_([0-3])\.(scale|offset)$")
+
+
+def _row_layer(name):
+    """(k, j, 'scale' | 'offset') of a row-layer name generator.layers.k.bn_j.scale / .offset, else None."""
+    m = _ROW_LAYER.match(name)
+    return None if m is None else (int(m[1]), int(m[2]), m[3])
 
 
 class _Config:
@@ -92,7 +102,11 @@ class _SNParams(nn.Module):
 class SNLinear(_SNParams):
     """``spectral_norm(nn.Linear)`` in eval mode: y = x (W_orig / sigma)^T + b."""
 
-    def forward(self, x):
+    def forward(self, x=None, _result=None):
+        # the conditional-BatchNorm linears (generator.layers.k.bn_j.scale / .offset) run in the BigGAN chain, which hands their
+        # rows to the hooks with forward(_result=rows), the convention of _FusedModule
+        if _result is not None:
+            return _result
         # latents are truncated normals in [-2, 2] * truncation and the class embedding is a fixed vector: inside fp16's range,
         # so batches of >= 128 rows run on the tensor cores (fp32-grade hi/lo split)
         return _native.linear(x, self.effective_weight(), self.bias.detach(), bounded=bool(x.abs().max() < 6e4) if x.shape[0] >= 128 else False)
@@ -218,6 +232,21 @@ class _BigGANNet(nn.Module):
         self.generator = _Generator(_sn_linear(2 * self.config.z_dim, 4 * 4 * 16 * self.config.channel_width, self.config.eps),
                                     self.config)
         self.n_latents = len(self.config.layers) + 1
+
+    def style_layers(self):
+        """(name, width) of every conditional-BatchNorm row layer ``generator.layers.k.bn_j.scale`` / ``.offset``, in execution order
+        (per GenBlock k: bn_0 .. bn_3, scale before offset, as BigGANBatchNorm.forward calls them)."""
+        return [(f"generator.layers.{k}.bn_{j}.{kind}", getattr(layer, f"bn_{j}").num_features)
+                for k, layer in enumerate(self.generator.layers) if isinstance(layer, GenBlock)
+                for j in range(4) for kind in ("scale", "offset")]
+
+    def unhookable_layers(self, n_modules=None, tail=True):
+        """The sub-modules the chain gives no output of their own, in generator.layers[:n_modules] (all by default) and, with
+        ``tail``, generator.bn and generator.conv_to_rgb: every module inside a block except the row layers."""
+        rows = {name for name, _ in self.style_layers()}
+        out = [name for i, layer in enumerate(list(self.generator.layers)[:n_modules])
+               for name, m in layer.named_modules(prefix=f"generator.layers.{i}") if m is not layer and name not in rows]
+        return out + (["generator.bn", "generator.conv_to_rgb"] if tail else [])
 
 
 @torch.no_grad()
@@ -356,15 +385,36 @@ class _Chain:
     def _empty(self, *shape):
         return torch.empty(shape, dtype=torch.float32, device=self.device)
 
-    def block(self, i, x, cond):
-        """GenBlock i on NHWC x [n, R, R, cin] with condition vectors cond [n, 256] -> [n, R', R', cout]."""
+    def rows(self, i, cond, js):
+        """The rows (cond W_scale^T, cond W_offset^T) [n, C_j] of BatchNorms ``js`` of GenBlock i, in one launch: what the hooks of
+        generator.layers.i.bn_j.scale / .offset receive."""
+        bns = self.steps[i]["bns"]
+        with _native.instrument.section("biggan rows"):
+            return _native.biggan_bn_rows(cond, [(bns[j]["ws"], bns[j]["wo"]) for j in js])
+
+    def table(self, i, j, n, scale_rows, offset_rows):
+        """The (scale, offset) tables [n, C] of BatchNorm j of GenBlock i from given rows ([n, C], row-strided, or [1, C])."""
+        bn = self.steps[i]["bns"][j]
+        c = bn["mean"].numel()
+        scale, offset = self._empty(n, c), self._empty(n, c)
+        with _native.instrument.section("biggan rows"):
+            _native.biggan_bn_table_rows(scale_rows, offset_rows, bn["var"], bn["eps"], scale, offset)
+        return scale, offset
+
+    def block(self, i, x, cond, tables=None):
+        """GenBlock i on NHWC x [n, R, R, cin] with condition vectors cond [n, 256] -> [n, R', R', cout].  ``tables``: {j: (scale,
+        offset)} caller-built tables [n, C_j] for BatchNorm j (``table``); the others are folded from cond here."""
         p = self.steps[i]
         n, R = x.shape[0], x.shape[1]
         R2 = 2 * R if p["up"] else R
         mid, cin, cout = p["mid"], p["cin"], p["cout"]
+        tables = tables or {}
         with _native.instrument.section(f"biggan layers.{i}"):
             tabs = []
-            for bn in p["bns"]:
+            for j, bn in enumerate(p["bns"]):
+                if j in tables:
+                    tabs.append((bn["mean"], *tables[j]))
+                    continue
                 c = bn["mean"].numel()
                 scale, offset = self._empty(n, c), self._empty(n, c)
                 _native.biggan_bn_table(cond, bn["ws"], bn["wo"], bn["var"], bn["eps"], scale, offset)
@@ -516,30 +566,85 @@ class BigGAN(_DeviceGenerator):
     def _synthesize(self, x, n_modules, want_image):
         """gen_z, then generator.layers[:n_modules] (and the tail when ``want_image``), firing the hooks of every layer on the
         way.  A hook's result on gen_z is what the chain continues from; an edit on a later layer would have to be re-fed into the
-        chain, which is not built -- it raises instead of being silently ignored (except on the last layer of a partial run)."""
+        chain, which is not built -- it raises instead of being silently ignored (except on the last layer of a partial run).
+        The row layers generator.layers.k.bn_j.scale / .offset are the exception: a hooked block's rows are computed from its own
+        condition vectors and handed to the hooks, and its BatchNorm tables are built from what they return, so an edit there
+        reaches block k and everything after it.  A partial run (no image) with no generator.layers.k hooked computes only the
+        hooked rows and launches no conv."""
         g = self.model.generator
         layers = list(g.layers)[:n_modules]
-        inner = [(name, m) for i, l in enumerate(layers) for name, m in l.named_modules(prefix=f"generator.layers.{i}") if m is not l]
-        if want_image:
-            inner += [("generator.bn", g.bn), ("generator.conv_to_rgb", g.conv_to_rgb)]
-        for name, m in inner:
-            if len(m._forward_hooks):
+        mods = self._modules_by_name()
+        for name in self.model.unhookable_layers(n_modules, tail=want_image):
+            if len(mods[name]._forward_hooks):
                 raise NotImplementedError(f"a hook on '{name}': the BigGAN chain materialises the outputs of gen_z and of "
                                           "generator.layers.k only")
+        hooked_rows = {}                                # block index -> [(j, kind, name)] of its hooked row layers
+        for name, _ in self.model.style_layers():
+            k, j, kind = _row_layer(name)
+            if k < len(layers) and len(mods[name]._forward_hooks):
+                hooked_rows.setdefault(k, []).append((j, kind, name))
         conds = self._conds(x)
-        h = g.gen_z(conds[0])
         chain = self._chain()
+        if hooked_rows and not want_image and not any(len(m._forward_hooks) for m in layers):
+            if len(g.gen_z._forward_hooks):
+                g.gen_z(conds[0])
+            for k in sorted(hooked_rows):
+                self._block_tables(chain, k, self._block_cond(conds, k), hooked_rows[k], build=False)
+            return None
+        h = g.gen_z(conds[0])
         act = h.contiguous().view(h.shape[0], 4, 4, -1)                 # gen_z's output is NHWC [4, 4, 16 ch] already
         ci = 1
         for i, mod in enumerate(layers):
             if isinstance(mod, GenBlock):
-                act = chain.block(i, act, conds[ci])
+                tables = self._block_tables(chain, i, conds[ci], hooked_rows[i]) if i in hooked_rows else None
+                act = chain.block(i, act, conds[ci], tables)
                 ci += 1
             else:
                 act = chain.attn(i, act)
             if len(mod._forward_hooks):
                 self._hand_off(mod, act, act.shape[1], act.shape[3], want_image or i < len(layers) - 1, f"generator.layers.{i}")
         return chain.rgb(act).permute(0, 3, 1, 2) if want_image else None
+
+    def _modules_by_name(self):
+        mods = getattr(self, "_by_name", None)
+        if mods is None:
+            mods = self._by_name = dict(self.model.named_modules())
+        return mods
+
+    def _block_cond(self, conds, k):
+        """The condition vectors of the GenBlock at generator.layers[k] (one per GenBlock, after gen_z's)."""
+        return conds[1 + sum(isinstance(m, GenBlock) for m in list(self.model.generator.layers)[:k])]
+
+    def _block_tables(self, chain, k, cond, hooked, build=True):
+        """The rows of the BatchNorms of GenBlock k that have a hooked row layer (one launch), handed to the hooks; returns {j:
+        (scale, offset)} tables built from what the hooks return (``build``; a rows-only run builds none)."""
+        mods = self._modules_by_name()
+        js = sorted({j for j, _, _ in hooked})
+        rows = dict(zip(js, chain.rows(k, cond, js)))
+        tables = {}
+        for j in js:
+            s, o = rows[j]
+            for jj, kind, name in hooked:
+                if jj == j and kind == "scale":
+                    s = self._hand_rows(mods[name], s, name)
+                elif jj == j:
+                    o = self._hand_rows(mods[name], o, name)
+            if build:
+                tables[j] = chain.table(k, j, cond.shape[0], s, o)
+        return tables
+
+    @staticmethod
+    def _hand_rows(module, rows, name):
+        """Hands a row layer's rows [n, C] to its hooks and returns what the tables are built from: the rows, or the hooks' edit
+        (a [1, C] edit applies to every sample, as nethook broadcasts it)."""
+        out = module(_result=rows)
+        if out is rows:
+            return rows
+        if not (out.dim() == 2 and out.shape[1] == rows.shape[1] and out.shape[0] in (1, rows.shape[0])):
+            raise ValueError(f"an edit on '{name}' must keep the rows' shape {tuple(rows.shape)} (or [1, {rows.shape[1]}]), got "
+                             f"{tuple(out.shape)}")
+        out = out.to(device=rows.device, dtype=torch.float32)
+        return out if out.stride(1) == 1 else out.contiguous()
 
     def forward(self, x):
         """wrappers.py:599-607: images 0.5 (G(z) + 1) in [0, 1], [n, 3, R, R] (an NCHW view of NHWC storage), from one latent or
@@ -565,20 +670,34 @@ class BigGAN(_DeviceGenerator):
         self._synthesize(x, n_layers, False)
         return None
 
-    # ---- low-rank structure of gen_z ----------------------------------------------------------------
+    # ---- low-rank structure of gen_z and of the row layers ------------------------------------------------
     def affine_layer(self, layer_name):
-        # GANSPACE_B200_BIGGAN_AFFINE=0: no low-rank shortcut -- the activations are materialised and go through the general
-        # large-d engine (csrc/bigd.cu), a cross-check of the shortcut
-        if layer_name.startswith("generator.") and layer_name != "generator.gen_z":
+        """The exact factorisation act = (z R^T) Q^T + offset of a layer that is affine in z, or None when the decomposition
+        driver is to materialise the layer's activations.  gen_z: A = W_eff[:, :128], offset = b + W_eff[:, 128:] embed.  A row
+        layer generator.layers.k.bn_j.scale / .offset of width C: rows = z A^T + W_eff[:, 128:] embed (no bias), rank min(C, 128);
+        C <= 128 gives no saving, so its rows are materialised (gsb_biggan_bn_rows) and go to the small-d engine.
+        GANSPACE_B200_BIGGAN_AFFINE=0: no low-rank shortcut -- gen_z's activations are materialised and go through the general
+        large-d engine (csrc/bigd.cu), and so are the rows of every row layer with C <= 1024 (the small-d engine), a cross-check
+        of the shortcut."""
+        widths = dict(self.model.style_layers())
+        if layer_name.startswith("generator.") and layer_name != "generator.gen_z" and layer_name not in widths:
             raise NotImplementedError(f"BigGAN: decomposing '{layer_name}' is not built; of the generator's layers only "
-                                      "generator.gen_z can be decomposed")
-        if layer_name != "generator.gen_z" or os.environ.get("GANSPACE_B200_BIGGAN_AFFINE", "1") == "0":
+                                      "generator.gen_z and the conditional-BatchNorm row layers generator.layers.k.bn_j.scale / "
+                                      ".offset can be decomposed")
+        if layer_name != "generator.gen_z" and layer_name not in widths:
+            return None
+        no_shortcut = os.environ.get("GANSPACE_B200_BIGGAN_AFFINE", "1") == "0"
+        if layer_name == "generator.gen_z" and no_shortcut:
+            return None
+        r = self.model.config.z_dim
+        if layer_name in widths and (widths[layer_name] <= r or (no_shortcut and widths[layer_name] <= 1024)):
             return None
         if layer_name not in self._affine:
-            g = self.model.generator.gen_z
-            w = g.effective_weight().double()                                # [d, 256]
-            r = self.model.config.z_dim
+            g = self._modules_by_name()[layer_name]
+            w = g.effective_weight().to(self.device).double()                # [d, 256] (the row layers' weights stay on the host)
             Q, R = torch.linalg.qr(w[:, :r].contiguous(), mode="reduced")   # one-time setup (like weight packing)
-            offset = g.bias.detach().double() + w[:, r:] @ self._embed().double()
+            offset = w[:, r:] @ self._embed().double()
+            if g.bias is not None:
+                offset = g.bias.detach().double() + offset
             self._affine[layer_name] = AffineLayer(Q.contiguous(), R.contiguous(), offset.contiguous())
         return self._affine[layer_name]
