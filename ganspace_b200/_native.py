@@ -40,6 +40,8 @@ SIGNATURES = {
     "gsb_batch_stats": (_I, [_P, _L, _I, _L, _P, _P, _P, _Z, _P]),
     "gsb_batch_stats_multi_workspace_bytes": (_Z, [_I, _L, _I]),
     "gsb_batch_stats_multi": (_I, [_P, _I, _L, _I, _L, _P, _P, _P, _Z, _P]),
+    "gsb_batch_stats_grouped_workspace_bytes": (_Z, [_P, _I]),
+    "gsb_batch_stats_grouped": (_I, [_P, _I, _P, _Z, _P]),
     "gsb_ipca_state_bytes": (_Z, [_I, _I]),
     "gsb_ipca_workspace_bytes": (_Z, [_I, _I]),
     "gsb_ipca_reset": (_I, [_P, _I, _I, _P]),
@@ -105,6 +107,12 @@ SIGNATURES = {
     "gsb_fbpca_status": (_I, [_P, _I, _P, _P]),
     "gsb_fbpca_project_omega": (_I, [_P, _I, _I, _P, _I, _P, _P]),
 }
+
+
+class StatsDesc(C.Structure):
+    """``gsb_stats_desc`` of include/ganspace_b200.h."""
+    _fields_ = [("x", C.c_void_p), ("ld", C.c_int64), ("d", C.c_int), ("n_groups", C.c_int), ("rows_per_group", C.c_int64),
+                ("mean_out", C.c_void_p), ("gram_out", C.c_void_p)]
 
 
 class StyledConvDesc(C.Structure):
@@ -555,6 +563,42 @@ def batch_stats_multi(x: torch.Tensor, n_groups: int, rows_per_group: int, mean_
                                          _ptr(ws), ws.numel(), _stream()), "gsb_batch_stats_multi")
     instrument.count(4 if (d % 128 == 0 and d <= 1024) else 3 * n_groups)
     return mean, gram
+
+
+def stats_grouped_width(d: int) -> bool:
+    """Whether ``batch_stats_multi`` takes the tensor-core path at width d, i.e. whether ``batch_stats_grouped`` gives its bits
+    (GANSPACE_B200_STATS=simt moves every width to the fp32 FMA kernels, which the grouped entry does not run)."""
+    return d % 128 == 0 and 128 <= d <= 1024 and os.environ.get("GANSPACE_B200_STATS") != "simt"
+
+
+def batch_stats_grouped(items):
+    """``batch_stats_multi`` of several inputs at once: ``items`` is a list of (x [>= G*rows, d] fp32 with unit column stride,
+    n_groups G, rows_per_group, mean_out [G, d] fp64 or None, gram_out [G, d, d] fp64 or None); returns [(mean, gram), ...] in
+    the same order, bit-identical to calling ``batch_stats_multi`` on each.  Every width must be a multiple of 128 up to 1024
+    (NativeError otherwise, before anything runs)."""
+    lib = load()
+    if not items:
+        return []
+    descs = (StatsDesc * len(items))()
+    outs = []
+    dev = items[0][0].device
+    for i, (x, n_groups, rows, mean, gram) in enumerate(items):
+        assert x.is_cuda and x.device == dev and x.dtype == torch.float32 and x.dim() == 2 and x.stride(1) == 1
+        assert x.shape[0] >= n_groups * rows
+        d = x.shape[1]
+        mean = mean if mean is not None else torch.empty((n_groups, d), dtype=torch.float64, device=dev)
+        gram = gram if gram is not None else torch.empty((n_groups, d, d), dtype=torch.float64, device=dev)
+        assert mean.shape == (n_groups, d) and gram.shape == (n_groups, d, d) and mean.dtype == gram.dtype == torch.float64
+        descs[i] = StatsDesc(x.data_ptr(), x.stride(0), d, int(n_groups), int(rows), _ptr(mean).value, _ptr(gram).value)
+        outs.append((mean, gram))
+    ws_bytes = lib.gsb_batch_stats_grouped_workspace_bytes(descs, len(items))
+    if ws_bytes == 0:
+        _check(lib.gsb_batch_stats_grouped(descs, len(items), C.c_void_p(0), 0, _stream()), "gsb_batch_stats_grouped")
+    ws = scratch.get("stats", ws_bytes, dev)
+    with torch.cuda.device(dev), instrument.section("stats"):
+        _check(lib.gsb_batch_stats_grouped(descs, len(items), _ptr(ws), ws.numel(), _stream()), "gsb_batch_stats_grouped")
+    instrument.count(5 * (-(-len(items) // 32)))
+    return outs
 
 
 class IPCAChain:

@@ -28,6 +28,7 @@
 // (35 MB as hi+lo) out of the 50 MB L2.
 #include "tc_common.cuh"
 #include <math.h>
+#include <string.h>
 
 namespace gsb {
 namespace gtc {
@@ -49,24 +50,76 @@ struct Params {
     int total_kb, chunk_kb; // K-blocks per group, per work item
 };
 
+// gram_tc_grouped_launch: up to GRAM_GROUPED_MAX operand sets of different widths in one persistent grid (Store epilogue)
+struct GroupedGramDesc {
+    double *out;            // [n_groups][d][d]
+    const int *exps;        // [n_groups]
+    int d, nt, npairs, total_kb;
+    int item0;              // first work item of the descriptor
+};
+struct GroupedGramParams {
+    CUtensorMap tm[GRAM_GROUPED_MAX][2];      // hi, lo operand maps of each descriptor
+    GroupedGramDesc desc[GRAM_GROUPED_MAX];
+    int n_desc, num_items;
+};
+
 struct Item { int g, m0, n0, kb0, kb1; };
 
-__device__ __forceinline__ Item decode_item(int item, const Params &p) {
-    const int outer = item / p.npairs;
-    int pair = item % p.npairs, ti = 0;
-    while (pair >= p.nt - ti) { pair -= p.nt - ti; ++ti; }
+// work item -> (group, chunk of K, tile pair), tile pair fastest
+__device__ __forceinline__ Item decode_tile(int item, int nt, int npairs, int n_chunks, int chunk_kb, int total_kb) {
+    const int outer = item / npairs;
+    int pair = item % npairs, ti = 0;
+    while (pair >= nt - ti) { pair -= nt - ti; ++ti; }
     Item w;
-    w.g = outer / p.n_chunks;
-    w.kb0 = (outer % p.n_chunks) * p.chunk_kb;
-    w.kb1 = (w.kb0 + p.chunk_kb < p.total_kb) ? w.kb0 + p.chunk_kb : p.total_kb;
+    w.g = outer / n_chunks;
+    w.kb0 = (outer % n_chunks) * chunk_kb;
+    w.kb1 = (w.kb0 + chunk_kb < total_kb) ? w.kb0 + chunk_kb : total_kb;
     w.m0 = ti * BM;
     w.n0 = (ti + pair) * BN;
     return w;
 }
 
-template <GramEpilogue EPI>
-__global__ void __launch_bounds__(tc::THREADS, 1)
-gram_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, const Params p) {
+// What a work item reads and writes: its operand maps and its output Gram(s)
+struct Target {
+    const CUtensorMap *hi, *lo;
+    double *out;
+    const int *exps;
+    int ld, n_rows;
+};
+
+// the work items of one gram_tc_launch: one pair of operand maps, one output
+struct PlainItems {
+    const CUtensorMap *hi, *lo;
+    const Params *p;
+    __device__ __forceinline__ int count() const { return p->n_groups * p->n_chunks * p->npairs; }
+    __device__ __forceinline__ void prefetch(int lane) const { if (lane == 0) { tc::tma_prefetch_desc(hi); tc::tma_prefetch_desc(lo); } }
+    __device__ __forceinline__ Item decode(int item, Target &t) const {
+        t.hi = hi; t.lo = lo; t.out = p->out; t.exps = p->exps; t.ld = p->ld; t.n_rows = p->n_rows;
+        return decode_tile(item, p->nt, p->npairs, p->n_chunks, p->chunk_kb, p->total_kb);
+    }
+};
+
+// the work items of gram_tc_grouped_launch: (descriptor, group, tile pair), descriptor-major, each descriptor with its own maps,
+// width and Store output
+struct GroupedItems {
+    const GroupedGramParams *p;
+    __device__ __forceinline__ int count() const { return p->num_items; }
+    __device__ __forceinline__ void prefetch(int lane) const {
+        if (lane < p->n_desc) { tc::tma_prefetch_desc(&p->tm[lane][0]); tc::tma_prefetch_desc(&p->tm[lane][1]); }
+    }
+    __device__ __forceinline__ Item decode(int item, Target &t) const {
+        int i = 0;
+        while (i + 1 < p->n_desc && item >= p->desc[i + 1].item0) ++i;
+        const GroupedGramDesc &g = p->desc[i];
+        t.hi = &p->tm[i][0]; t.lo = &p->tm[i][1]; t.out = g.out; t.exps = g.exps; t.ld = g.d; t.n_rows = g.d;
+        return decode_tile(item - g.item0, g.nt, g.npairs, 1, g.total_kb, g.total_kb);
+    }
+};
+
+// The persistent kernel body, shared by both work-item maps: the producer and the MMA / promotion / epilogue code are the same
+// instructions whichever map decodes the items, so a Gram computed through either map has the same bits.
+template <GramEpilogue EPI, class Items>
+__device__ __forceinline__ void gram_tc_body(const Items &items) {
     using namespace tc;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -75,13 +128,13 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
     uint64_t *empty_bar = bars + STAGES;           // [STAGES]: one arrival per consumer warp
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int num_items = p.n_groups * p.n_chunks * p.npairs;
+    const int num_items = items.count();
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CONSUMER_THREADS / 32); }
         mbar_fence_init();
     }
-    if (warp == PRODUCER_WARP && lane == 0) { tma_prefetch_desc(&tm_hi); tma_prefetch_desc(&tm_lo); }
+    if (warp == PRODUCER_WARP) items.prefetch(lane);
     __syncthreads();
 
     if (warp == PRODUCER_WARP) {
@@ -89,15 +142,16 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
         if (lane == 0) {
             int stage = 0; uint32_t phase = 0;
             for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-                const Item w = decode_item(item, p);
+                Target t;
+                const Item w = items.decode(item, t);
                 for (int kb = w.kb0; kb < w.kb1; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1);
                     uint8_t *st = smem + stage * STAGE_BYTES;
                     mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES);
-                    tma_load_3d(&tm_hi, &full_bar[stage], st, kb * BK, w.m0, w.g);
-                    tma_load_3d(&tm_lo, &full_bar[stage], st + TILE_BYTES, kb * BK, w.m0, w.g);
-                    tma_load_3d(&tm_hi, &full_bar[stage], st + 2 * TILE_BYTES, kb * BK, w.n0, w.g);
-                    tma_load_3d(&tm_lo, &full_bar[stage], st + 3 * TILE_BYTES, kb * BK, w.n0, w.g);
+                    tma_load_3d(t.hi, &full_bar[stage], st, kb * BK, w.m0, w.g);
+                    tma_load_3d(t.lo, &full_bar[stage], st + TILE_BYTES, kb * BK, w.m0, w.g);
+                    tma_load_3d(t.hi, &full_bar[stage], st + 2 * TILE_BYTES, kb * BK, w.n0, w.g);
+                    tma_load_3d(t.lo, &full_bar[stage], st + 3 * TILE_BYTES, kb * BK, w.n0, w.g);
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
@@ -111,7 +165,8 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
 #pragma unroll
         for (int j = 0; j < 64; ++j) { acc[j] = 0.f; r[j] = 0.f; }
         for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-            const Item w = decode_item(item, p);
+            Target t;
+            const Item w = items.decode(item, t);
             const int nkb = w.kb1 - w.kb0;
             for (int g0 = 0; g0 < nkb; g0 += FLUSH_KB) {
                 const int g1 = (g0 + FLUSH_KB < nkb) ? g0 + FLUSH_KB : nkb;
@@ -131,36 +186,36 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
                 for (int j = 0; j < 64; ++j) r[j] = __fadd_rn(r[j], acc[j]);
             }
             if constexpr (EPI == GramEpilogue::Store) {
-                const double unscale = ldexp(1.0, -2 * __ldg(p.exps + w.g));
-                double *G = p.out + (size_t)w.g * p.ld * p.ld;
+                const double unscale = ldexp(1.0, -2 * __ldg(t.exps + w.g));
+                double *G = t.out + (size_t)w.g * t.ld * t.ld;
                 const bool diag = (w.m0 == w.n0);
 #pragma unroll
                 for (int j = 0; j < 64; j += 2) {
                     const int gm = w.m0 + row_frag + 8 * ((j >> 1) & 1), gn = w.n0 + 8 * (j >> 2) + col_frag;
                     const double v0 = (double)r[j] * unscale, v1 = (double)r[j + 1] * unscale;
                     if (!diag) {
-                        *reinterpret_cast<double2 *>(G + (size_t)gm * p.ld + gn) = make_double2(v0, v1);
-                        G[(size_t)gn * p.ld + gm] = v0;
-                        G[(size_t)(gn + 1) * p.ld + gm] = v1;
+                        *reinterpret_cast<double2 *>(G + (size_t)gm * t.ld + gn) = make_double2(v0, v1);
+                        G[(size_t)gn * t.ld + gm] = v0;
+                        G[(size_t)(gn + 1) * t.ld + gm] = v1;
                     } else {
                         // diagonal tile: (i,j) and (j,i) come out of differently ordered MMA sums; keep the upper triangle
                         // and mirror it, so the chain reads an exactly symmetric matrix
-                        if (gn >= gm) { G[(size_t)gm * p.ld + gn] = v0; G[(size_t)gn * p.ld + gm] = v0; }
-                        if (gn + 1 >= gm) { G[(size_t)gm * p.ld + gn + 1] = v1; G[(size_t)(gn + 1) * p.ld + gm] = v1; }
+                        if (gn >= gm) { G[(size_t)gm * t.ld + gn] = v0; G[(size_t)gn * t.ld + gm] = v0; }
+                        if (gn + 1 >= gm) { G[(size_t)gm * t.ld + gn + 1] = v1; G[(size_t)(gn + 1) * t.ld + gm] = v1; }
                     }
                 }
             } else {
                 const int gm0 = w.m0 + row_frag, gm1 = gm0 + 8;
-                const int em0 = gm0 < p.n_rows ? __ldg(&p.exps[gm0]) : 0, em1 = gm1 < p.n_rows ? __ldg(&p.exps[gm1]) : 0;
+                const int em0 = gm0 < t.n_rows ? __ldg(&t.exps[gm0]) : 0, em1 = gm1 < t.n_rows ? __ldg(&t.exps[gm1]) : 0;
 #pragma unroll
                 for (int j = 0; j < 64; ++j) {
                     const int gm = ((j >> 1) & 1) ? gm1 : gm0, gn = w.n0 + 8 * (j >> 2) + col_frag + (j & 1);
-                    if (gm < p.n_rows && gn < p.n_rows && gn >= gm) {
+                    if (gm < t.n_rows && gn < t.n_rows && gn >= gm) {
                         // 2^-(e_i + e_j) as an fp64 bit pattern: exact, |e_i + e_j| stays far inside the normal range
-                        const int e = ((j >> 1) & 1 ? em1 : em0) + __ldg(&p.exps[gn]);
+                        const int e = ((j >> 1) & 1 ? em1 : em0) + __ldg(&t.exps[gn]);
                         const double val = (double)r[j] * __hiloint2double((1023 - e) << 20, 0);
-                        atomicAdd(&p.out[(size_t)gm * p.ld + gn], val);
-                        if (gn > gm) atomicAdd(&p.out[(size_t)gn * p.ld + gm], val);
+                        atomicAdd(&t.out[(size_t)gm * t.ld + gn], val);
+                        if (gn > gm) atomicAdd(&t.out[(size_t)gn * t.ld + gm], val);
                     }
                 }
             }
@@ -168,6 +223,17 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
             for (int j = 0; j < 64; ++j) r[j] = 0.f;
         }
     }
+}
+
+template <GramEpilogue EPI>
+__global__ void __launch_bounds__(tc::THREADS, 1)
+gram_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, const __grid_constant__ Params p) {
+    gram_tc_body<EPI>(PlainItems{&tm_hi, &tm_lo, &p});
+}
+
+__global__ void __launch_bounds__(tc::THREADS, 1)
+gram_tc_grouped_kernel(const __grid_constant__ GroupedGramParams p) {
+    gram_tc_body<GramEpilogue::Store>(GroupedItems{&p});
 }
 
 // ---- operand preparation ----------------------------------------------------------------------------------
@@ -241,6 +307,37 @@ int gram_tc_launch(GramEpilogue epi, const __half *hi, const __half *lo, int64_t
         gram_tc_kernel<GramEpilogue::Store><<<grid, tc::THREADS, SMEM_BYTES, st>>>(tm_hi, tm_lo, p);
     else
         gram_tc_kernel<GramEpilogue::Accumulate><<<grid, tc::THREADS, SMEM_BYTES, st>>>(tm_hi, tm_lo, p);
+    GSB_CHECK_LAUNCH();
+    return GSB_OK;
+}
+
+// Store Grams of several operand sets (stats_tc_grouped): work items (descriptor, group, tile pair) flattened into one grid
+int gram_tc_grouped_launch(const GramGroupedOperand *ops, int n, cudaStream_t st) {
+    using namespace gtc;
+    GSB_CHECK_ARG(n > 0 && n <= GRAM_GROUPED_MAX, "gram_tc_grouped_launch: 0 < n <= %d descriptors (n=%d)", GRAM_GROUPED_MAX, n);
+    if (int r = raise_dyn_smem(gram_tc_grouped_kernel, SMEM_BYTES)) return r;
+    GroupedGramParams p;
+    memset(&p, 0, sizeof(p));
+    int items = 0;
+    for (int i = 0; i < n; ++i) {
+        const GramGroupedOperand &o = ops[i];
+        const uint64_t dims[3] = {(uint64_t)o.nb, (uint64_t)o.d, (uint64_t)o.n_groups};
+        const uint64_t strides[2] = {(uint64_t)o.nbp * 2, (uint64_t)o.d * o.nbp * 2};
+        const uint32_t box[3] = {(uint32_t)BK, (uint32_t)BM, 1};
+        if (int r = tc_make_tmap(&p.tm[i][0], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, o.hi, 3, dims, strides, box)) return r;
+        if (int r = tc_make_tmap(&p.tm[i][1], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, o.lo, 3, dims, strides, box)) return r;
+        GroupedGramDesc &g = p.desc[i];
+        g.out = o.out; g.exps = o.exps; g.d = o.d;
+        g.nt = (o.d + BM - 1) / BM;
+        g.npairs = g.nt * (g.nt + 1) / 2;
+        g.total_kb = (int)((o.nb + BK - 1) / BK);
+        g.item0 = items;
+        items += o.n_groups * g.npairs;
+    }
+    p.n_desc = n;
+    p.num_items = items;
+    const int grid = items < num_sms() ? items : num_sms();
+    gram_tc_grouped_kernel<<<grid, tc::THREADS, SMEM_BYTES, st>>>(p);
     GSB_CHECK_LAUNCH();
     return GSB_OK;
 }

@@ -152,6 +152,38 @@ extern "C" int gsb_batch_stats_multi(const float *d_x, int n_groups, int64_t row
     return GSB_OK;
 }
 
+static int check_grouped(const gsb_stats_desc *descs, int n_desc) {
+    GSB_CHECK_ARG(descs && n_desc > 0, "batch_stats_grouped: need a non-empty descriptor array (n_desc=%d)", n_desc);
+    for (int i = 0; i < n_desc; ++i) {
+        const gsb_stats_desc &s = descs[i];
+        GSB_CHECK_ARG(s.x && s.mean_out && s.gram_out, "batch_stats_grouped: null pointer in descriptor %d", i);
+        GSB_CHECK_ARG(gsb::stats_tc_grouped_width(s.d),
+                      "batch_stats_grouped: descriptor %d has d=%d; the grouped statistics take d %% 128 == 0, 128 <= d <= 1024 "
+                      "(other widths: gsb_batch_stats_multi)", i, s.d);
+        GSB_CHECK_ARG(s.n_groups > 0 && s.n_groups <= 65535 && s.rows_per_group > 0 && s.ld >= s.d && s.ld % 4 == 0,
+                      "batch_stats_grouped: descriptor %d needs 0<groups<=65535, rows>0, ld>=d, ld%%4==0 (groups=%d rows=%lld "
+                      "ld=%lld)", i, s.n_groups, (long long)s.rows_per_group, (long long)s.ld);
+    }
+    return GSB_OK;
+}
+
+extern "C" size_t gsb_batch_stats_grouped_workspace_bytes(const gsb_stats_desc *descs, int n_desc) {
+    if (check_grouped(descs, n_desc)) return 0;
+    return gsb::stats_tc_grouped_workspace_bytes(descs, n_desc);
+}
+
+// Statistics of several inputs in one set of launches per 32 descriptors; every descriptor is checked before anything runs.
+extern "C" int gsb_batch_stats_grouped(const gsb_stats_desc *descs, int n_desc, void *d_workspace, size_t workspace_bytes,
+                                       gsb_stream_t stream) {
+    if (int r = check_grouped(descs, n_desc)) return r;
+    GSB_CHECK_ARG(d_workspace, "batch_stats_grouped: null workspace");
+    if (workspace_bytes < gsb::stats_tc_grouped_workspace_bytes(descs, n_desc)) {
+        gsb::set_error("batch_stats_grouped: workspace too small");
+        return GSB_ERR_WORKSPACE;
+    }
+    return gsb::stats_tc_grouped(descs, n_desc, d_workspace, (cudaStream_t)stream);
+}
+
 extern "C" int gsb_batch_stats(const float *d_x, int64_t n, int d, int64_t ld, double *d_mean,
                                double *d_gram, void *d_workspace, size_t workspace_bytes,
                                gsb_stream_t stream) {

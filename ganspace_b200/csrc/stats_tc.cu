@@ -29,11 +29,12 @@ namespace stc {
 // ---- column sums per group ----------------------------------------------------------------------------------------
 constexpr int SUM_ROWS = 256;               // rows per column-sum slice
 
-__global__ void colsum_groups_kernel(const float *__restrict__ x, int64_t nb, int d, int64_t ld, int rows_per_cta,
-                                     double *__restrict__ part /* [G][ny][d] */, float *__restrict__ absmax /* [G], zeroed */) {
-    const int col = blockIdx.x * blockDim.x + threadIdx.x;
-    const int g = blockIdx.z;
-    const int64_t r0 = (int64_t)blockIdx.y * rows_per_cta;
+// one (column block, row slice, group) block of column sums; part: [G][ny][d]
+__device__ __forceinline__ void colsum_groups_body(const float *__restrict__ x, int64_t nb, int d, int64_t ld, int rows_per_cta,
+                                                   double *__restrict__ part, float *__restrict__ absmax, int bx, int by, int ny,
+                                                   int g) {
+    const int col = bx * blockDim.x + threadIdx.x;
+    const int64_t r0 = (int64_t)by * rows_per_cta;
     const int64_t r1 = r0 + rows_per_cta < nb ? r0 + rows_per_cta : nb;
     const float *xg = x + (size_t)g * nb * ld;
     double a0 = 0.0, a1 = 0.0;              // fp64 sum of the fp32 samples, as sklearn's _safe_accumulator_op does
@@ -46,16 +47,21 @@ __global__ void colsum_groups_kernel(const float *__restrict__ x, int64_t nb, in
             mx = fmaxf(mx, fmaxf(fabsf(v0), fabsf(v1)));
         }
         if (r < r1) { const float v0 = xg[r * ld + col]; a0 += (double)v0; mx = fmaxf(mx, fabsf(v0)); }
-        part[((size_t)g * gridDim.y + blockIdx.y) * d + col] = a0 + a1;
+        part[((size_t)g * ny + by) * d + col] = a0 + a1;
     }
     for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
     if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<int *>(absmax + g), __float_as_int(mx));   // mx >= 0: int order == float order
 }
 
+__global__ void colsum_groups_kernel(const float *__restrict__ x, int64_t nb, int d, int64_t ld, int rows_per_cta,
+                                     double *__restrict__ part /* [G][ny][d] */, float *__restrict__ absmax /* [G], zeroed */) {
+    colsum_groups_body(x, nb, d, ld, rows_per_cta, part, absmax, blockIdx.x, blockIdx.y, gridDim.y, blockIdx.z);
+}
+
 // mean per (group, feature); scale exponent per group: |x - mean| <= 2 max|x|, and 2 max|x| 2^e lands in [8192, 32768)
-__global__ void mean_groups_kernel(const double *__restrict__ part, int ny, int n_groups, int d, double nd, double *__restrict__ mean,
-                                   float *__restrict__ mean32, const float *__restrict__ absmax, int *__restrict__ exps) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void mean_groups_body(const double *__restrict__ part, int ny, int n_groups, int d, double nd,
+                                                 double *__restrict__ mean, float *__restrict__ mean32, const float *__restrict__ absmax,
+                                                 int *__restrict__ exps, int i) {
     if (i < n_groups * d) {
         const int g = i / d, c = i % d;
         double t = 0.0;
@@ -72,15 +78,19 @@ __global__ void mean_groups_kernel(const double *__restrict__ part, int ny, int 
     }
 }
 
+__global__ void mean_groups_kernel(const double *__restrict__ part, int ny, int n_groups, int d, double nd, double *__restrict__ mean,
+                                   float *__restrict__ mean32, const float *__restrict__ absmax, int *__restrict__ exps) {
+    mean_groups_body(part, ny, n_groups, d, nd, mean, mean32, absmax, exps, blockIdx.x * blockDim.x + threadIdx.x);
+}
+
 // ---- centre, scale, split, transpose ---------------------------------------------------------------------------------
 // tile: 64 samples x 64 features; 256 threads.  xt_hi / xt_lo: [G][d][nbp] fp16 (nbp = nb rounded up to 64).
-__global__ void __launch_bounds__(256)
-center_split_t_kernel(const float *__restrict__ x, int64_t nb, int d, int64_t ld, int64_t nbp, const float *__restrict__ mean32,
-                      const int *__restrict__ exps, __half *__restrict__ xt_hi, __half *__restrict__ xt_lo) {
+__device__ __forceinline__ void center_split_t_body(const float *__restrict__ x, int64_t nb, int d, int64_t ld, int64_t nbp,
+                                                    const float *__restrict__ mean32, const int *__restrict__ exps,
+                                                    __half *__restrict__ xt_hi, __half *__restrict__ xt_lo, int bx, int by, int g) {
     __shared__ float tile[64][65];
-    const int g = blockIdx.z;
-    const int64_t r0 = (int64_t)blockIdx.x * 64;
-    const int c0 = blockIdx.y * 64;
+    const int64_t r0 = (int64_t)bx * 64;
+    const int c0 = by * 64;
     const int tid = threadIdx.x;
     const float *xg = x + (size_t)g * nb * ld;
     const float *mg = mean32 + (size_t)g * d;
@@ -114,6 +124,12 @@ center_split_t_kernel(const float *__restrict__ x, int64_t nb, int d, int64_t ld
     }
 }
 
+__global__ void __launch_bounds__(256)
+center_split_t_kernel(const float *__restrict__ x, int64_t nb, int d, int64_t ld, int64_t nbp, const float *__restrict__ mean32,
+                      const int *__restrict__ exps, __half *__restrict__ xt_hi, __half *__restrict__ xt_lo) {
+    center_split_t_body(x, nb, d, ld, nbp, mean32, exps, xt_hi, xt_lo, blockIdx.x, blockIdx.y, blockIdx.z);
+}
+
 struct WsView {
     double *sum;
     float *mean32;
@@ -137,6 +153,75 @@ static WsView carve(void *base, int n_groups, int64_t nb, int d) {
     w.xt_lo = (__half *)take((size_t)n_groups * d * nbp * 2);
     w.bytes = off;
     return w;
+}
+
+// ---- grouped: the three preparation kernels for several inputs per launch -------------------------------------------
+// Each kernel's blocks are the concatenation of what the plain launches of the descriptors would run, in descriptor order;
+// a block finds its descriptor by its first block index and runs the plain kernel's body on the decoded coordinates.
+struct PrepDesc {
+    const float *x;
+    int64_t nb, ld, nbp;
+    int d, n_groups, ny;
+    double *mean, *sum;
+    float *mean32, *absmax;
+    int *exps;
+    __half *xt_hi, *xt_lo;
+    int blk_colsum, blk_mean, blk_center;       // first block of the descriptor in each launch
+};
+struct PrepParams {
+    PrepDesc desc[GRAM_GROUPED_MAX];
+    int n_desc;
+};
+
+template <int PrepDesc::*FIRST>
+__device__ __forceinline__ const PrepDesc &find_desc(const PrepParams &p, int b) {
+    int i = 0;
+    while (i + 1 < p.n_desc && b >= p.desc[i + 1].*FIRST) ++i;
+    return p.desc[i];
+}
+
+__global__ void colsum_grouped_kernel(const __grid_constant__ PrepParams p) {
+    const PrepDesc &q = find_desc<&PrepDesc::blk_colsum>(p, blockIdx.x);
+    const int local = blockIdx.x - q.blk_colsum, gx = (q.d + 127) / 128;
+    colsum_groups_body(q.x, q.nb, q.d, q.ld, SUM_ROWS, q.sum, q.absmax, local % gx, (local / gx) % q.ny, q.ny, local / (gx * q.ny));
+}
+
+__global__ void mean_grouped_kernel(const __grid_constant__ PrepParams p) {
+    const PrepDesc &q = find_desc<&PrepDesc::blk_mean>(p, blockIdx.x);
+    const int local = blockIdx.x - q.blk_mean;
+    mean_groups_body(q.sum, q.ny, q.n_groups, q.d, (double)q.nb, q.mean, q.mean32, q.absmax, q.exps, local * blockDim.x + threadIdx.x);
+}
+
+__global__ void __launch_bounds__(256) center_split_t_grouped_kernel(const __grid_constant__ PrepParams p) {
+    const PrepDesc &q = find_desc<&PrepDesc::blk_center>(p, blockIdx.x);
+    const int local = blockIdx.x - q.blk_center, gx = (int)(q.nbp / 64), gy = q.d / 64;
+    center_split_t_body(q.x, q.nb, q.d, q.ld, q.nbp, q.mean32, q.exps, q.xt_hi, q.xt_lo, local % gx, (local / gx) % gy,
+                        local / (gx * gy));
+}
+
+// Workspace of one set of grouped launches: the scale maxima of every group first (one memset zeroes them all), then each
+// descriptor's column-sum slices, fp32 means and split operands (carve's layout)
+static size_t carve_grouped(void *base, const gsb_stats_desc *descs, int n, PrepDesc *out) {
+    char *p = reinterpret_cast<char *>(base);
+    int total_groups = 0;
+    for (int i = 0; i < n; ++i) total_groups += descs[i].n_groups;
+    size_t off = align_up((size_t)total_groups * sizeof(float), 1024);
+    int g0 = 0;
+    for (int i = 0; i < n; ++i) {
+        const gsb_stats_desc &s = descs[i];
+        WsView w = carve(p ? p + off : nullptr, s.n_groups, s.rows_per_group, s.d);
+        if (out) {
+            PrepDesc &q = out[i];
+            q.x = s.x; q.nb = s.rows_per_group; q.ld = s.ld; q.nbp = (s.rows_per_group + 63) / 64 * 64;
+            q.d = s.d; q.n_groups = s.n_groups; q.ny = (int)((s.rows_per_group + SUM_ROWS - 1) / SUM_ROWS);
+            q.mean = s.mean_out; q.sum = w.sum; q.mean32 = w.mean32; q.exps = w.exps;
+            q.absmax = reinterpret_cast<float *>(p) + g0;
+            q.xt_hi = w.xt_hi; q.xt_lo = w.xt_lo;
+        }
+        g0 += s.n_groups;
+        off += w.bytes;
+    }
+    return off;
 }
 
 }  // namespace stc
@@ -172,6 +257,50 @@ int stats_tc(const float *x, int n_groups, int64_t nb, int d, int64_t ld, double
         GSB_CHECK_LAUNCH();
     }
     return gram_tc_launch(GramEpilogue::Store, w.xt_hi, w.xt_lo, nb, nbp, n_groups, d, d, w.exps, gram, st);
+}
+
+bool stats_tc_grouped_width(int d) { return d % 128 == 0 && d >= 128 && d <= 1024; }
+
+size_t stats_tc_grouped_workspace_bytes(const gsb_stats_desc *descs, int n_desc) {
+    size_t bytes = 0;
+    for (int i0 = 0; i0 < n_desc; i0 += GRAM_GROUPED_MAX) {
+        const int n = n_desc - i0 < GRAM_GROUPED_MAX ? n_desc - i0 : GRAM_GROUPED_MAX;
+        const size_t b = stc::carve_grouped(nullptr, descs + i0, n, nullptr);
+        bytes = b > bytes ? b : bytes;
+    }
+    return bytes;
+}
+
+// descriptors already checked: one set of four launches (+ one memset) per GRAM_GROUPED_MAX descriptors, sharing ws
+int stats_tc_grouped(const gsb_stats_desc *descs, int n_desc, void *ws, cudaStream_t st) {
+    using namespace stc;
+    for (int i0 = 0; i0 < n_desc; i0 += GRAM_GROUPED_MAX) {
+        const int n = n_desc - i0 < GRAM_GROUPED_MAX ? n_desc - i0 : GRAM_GROUPED_MAX;
+        PrepParams p;
+        memset(&p, 0, sizeof(p));
+        p.n_desc = n;
+        carve_grouped(ws, descs + i0, n, p.desc);
+        int total_groups = 0, b_col = 0, b_mean = 0, b_ctr = 0;
+        GramGroupedOperand ops[GRAM_GROUPED_MAX];
+        for (int i = 0; i < n; ++i) {
+            PrepDesc &q = p.desc[i];
+            q.blk_colsum = b_col; q.blk_mean = b_mean; q.blk_center = b_ctr;
+            b_col += ((q.d + 127) / 128) * q.ny * q.n_groups;
+            b_mean += (q.n_groups * q.d + 255) / 256;
+            b_ctr += (int)(q.nbp / 64) * (q.d / 64) * q.n_groups;
+            total_groups += q.n_groups;
+            ops[i] = GramGroupedOperand{q.xt_hi, q.xt_lo, q.nb, q.nbp, q.d, q.n_groups, q.exps, descs[i0 + i].gram_out};
+        }
+        GSB_CHECK_CUDA(cudaMemsetAsync(ws, 0, (size_t)total_groups * sizeof(float), st));
+        colsum_grouped_kernel<<<b_col, 128, 0, st>>>(p);
+        GSB_CHECK_LAUNCH();
+        mean_grouped_kernel<<<b_mean, 256, 0, st>>>(p);
+        GSB_CHECK_LAUNCH();
+        center_split_t_grouped_kernel<<<b_ctr, 256, 0, st>>>(p);
+        GSB_CHECK_LAUNCH();
+        if (int r = gram_tc_grouped_launch(ops, n, st)) return r;
+    }
+    return GSB_OK;
 }
 
 }  // namespace gsb

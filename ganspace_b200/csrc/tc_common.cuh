@@ -168,6 +168,18 @@ int tc_make_tmap(CUtensorMap *map, CUtensorMapDataType type, const void *base, i
 enum class GramEpilogue { Store, Accumulate };
 int gram_tc_launch(GramEpilogue epi, const __half *hi, const __half *lo, int64_t k, int64_t k_pitch, int n_groups, int n_pad,
                    int n_rows, const int *exps, double *out, cudaStream_t st);
+// Store Grams of up to GRAM_GROUPED_MAX operand sets of different widths in one launch (gram_tc.cu): for each set, out[g] as
+// gram_tc_launch(Store, hi, lo, nb, nbp, n_groups, d, d, exps, out) computes it, with the same bits; work items are
+// (set, group, tile pair), set-major
+constexpr int GRAM_GROUPED_MAX = 32;
+struct GramGroupedOperand {
+    const __half *hi, *lo;      // [n_groups][d][nbp]
+    int64_t nb, nbp;
+    int d, n_groups;            // d % 128 == 0
+    const int *exps;            // [n_groups]
+    double *out;                // [n_groups][d][d]
+};
+int gram_tc_grouped_launch(const GramGroupedOperand *ops, int n, cudaStream_t st);
 // large-d small side T = M M^T (gram_tc.cu)
 size_t gram_tc_workspace_bytes(int n_pad, int64_t d);
 bool gram_tc_supported(int64_t d);
@@ -177,6 +189,10 @@ int gram_tc(const float *M, int n_rows, int n_pad, int64_t d, void *ws, double *
 bool stats_tc_supported(int64_t nb, int d);
 size_t stats_tc_workspace_bytes(int n_groups, int64_t nb, int d);
 int stats_tc(const float *x, int n_groups, int64_t nb, int d, int64_t ld, double *mean, double *gram, void *ws, cudaStream_t st);
+// the same for several inputs (gsb_batch_stats_grouped; widths d % 128 == 0, d <= 1024), each with stats_tc's bits
+bool stats_tc_grouped_width(int d);
+size_t stats_tc_grouped_workspace_bytes(const gsb_stats_desc *descs, int n_desc);
+int stats_tc_grouped(const gsb_stats_desc *descs, int n_desc, void *ws, cudaStream_t st);
 
 // mapping network, dense layers and the conv tap GEMM on the persistent layer kernel (mapping_tc.cu)
 size_t mapping_tc_packed_bytes(int n_layers, int dim);

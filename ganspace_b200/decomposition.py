@@ -21,6 +21,7 @@ is already being computed -- the result does not depend on the world size (SURVE
 """
 from __future__ import annotations
 
+import copy
 import datetime
 import inspect
 import os
@@ -34,7 +35,7 @@ import torch
 from . import _native
 from . import plan as _plan
 from .config import Config  # noqa: F401  (re-exported like the reference module does)
-from .estimators import get_estimator
+from .estimators import DeviceIncrementalPCA, get_estimator
 from .models import get_instrumented_model
 from .netdissect.nethook import InstrumentedModel
 
@@ -190,12 +191,16 @@ def linreg_lstsq(comp_np, mean_np, stdev_np, inst, config, affine=None, native=F
     return M_t.cpu().numpy()[:n_comp, :], Z_mean.cpu().numpy().reshape(1, -1)
 
 
-def regression(comp, mean, stdev, inst, config, affine=None, native=False):
+def _warn_if_not_orthonormal(comp):
     M = np.dot(comp, comp.T)
     # fp32 components (large-d engine) are orthonormal to ~1e-6, the reference's float64 ones to 1e-15
     if not np.allclose(M, np.identity(M.shape[0]), atol=1e-8 if comp.dtype == np.float64 else 5e-6):
         det = np.linalg.det(M)
         print(f"WARNING: Computed basis is not orthonormal (determinant={det})")
+
+
+def regression(comp, mean, stdev, inst, config, affine=None, native=False):
+    _warn_if_not_orthonormal(comp)
     return linreg_lstsq(comp, mean, stdev, inst, config, affine=affine, native=native)
 
 
@@ -222,18 +227,22 @@ def compute(config, dump_name, instrumented_model):
         print(f'Saving current state to "{dump_name.name}" before exiting')
     rank, world, live = _dist()
     if rank == 0:
-        os.makedirs(dump_name.parent, exist_ok=True)
-        # same 8-array .npz container, read by np.load exactly like the reference's; stored WITHOUT deflate: the arrays are
-        # float32 noise (7 % smaller compressed) and single-core zlib costs 8-18 ms for config 2 -- a fifth of the whole
-        # device run -- and minutes for conv feature maps (act_comp = 168 MB at convs.4).  GANSPACE_B200_NPZ_COMPRESS=1 restores
-        # np.savez_compressed (decomposition.py:331-341).
-        compress = os.environ.get("GANSPACE_B200_NPZ_COMPRESS") == "1" and sum(a.nbytes for a in arrays.values()) <= (64 << 20)
-        (np.savez_compressed if compress else np.savez)(dump_name, **arrays)
+        _write_npz(dump_name, arrays)
     if live:
         import torch.distributed as dist
         dist.barrier()
     if state.get("canceled_at") is not None:
         sys.exit(1)
+
+
+def _write_npz(dump_name, arrays):
+    os.makedirs(dump_name.parent, exist_ok=True)
+    # same 8-array .npz container, read by np.load exactly like the reference's; stored WITHOUT deflate: the arrays are
+    # float32 noise (7 % smaller compressed) and single-core zlib costs 8-18 ms for config 2 -- a fifth of the whole
+    # device run -- and minutes for conv feature maps (act_comp = 168 MB at convs.4).  GANSPACE_B200_NPZ_COMPRESS=1 restores
+    # np.savez_compressed (decomposition.py:331-341).
+    compress = os.environ.get("GANSPACE_B200_NPZ_COMPRESS") == "1" and sum(a.nbytes for a in arrays.values()) <= (64 << 20)
+    (np.savez_compressed if compress else np.savez)(dump_name, **arrays)
 
 
 def _phase_timer():
@@ -249,6 +258,58 @@ def _phase_timer():
         print(f"[timing] {label}: {now - state['t']:.3f} s", flush=True)
         state["t"] = now
     return tick
+
+
+def _export_components(transformer, affine, pooled, sample_dims, device):
+    """The fitted estimator's result in the layer's coordinates: (X_comp, X_stdev, X_var_ratio, device mean, X_global_mean) for
+    the file, and (Y_comp, Y_mean) for the regression (an affine layer's r-dimensional coordinates)."""
+    tr = transformer.transformer
+    X_comp, X_stdev, X_var_ratio = transformer.get_components()
+    X_comp = np.array(X_comp, copy=True)
+    mean_dev = transformer.device_outputs["mean"] if pooled else tr.device_attributes()["mean"]
+    if affine is None:
+        X_global_mean = (transformer.pooled_mean if pooled else tr.mean_).reshape((1, sample_dims))
+        Y_comp, Y_mean = X_comp, X_global_mean              # device feature order (== the reference's unless `layout`)
+    else:
+        # lift through the isometry: components = components_y Q^T (svd_flip's sign rule is applied on the lifted
+        # rows, as sklearn would on the full activations), mean = mean_y Q^T + offset
+        lifted = affine.lift_rows(torch.from_numpy(X_comp).to(device))
+        idx = torch.argmax(lifted.abs(), dim=1)
+        signs = torch.sign(lifted[torch.arange(lifted.shape[0], device=device), idx])
+        Y_comp = X_comp * signs.cpu().numpy()[:, None]
+        Y_mean = (transformer.pooled_mean if pooled else tr.mean_).reshape((1, affine.Q.shape[1]))
+        X_comp = (lifted * signs[:, None]).cpu().numpy()
+        X_global_mean = (affine.lift_rows(mean_dev[None, :]) + affine.offset[None, :]).cpu().numpy()
+    return X_comp, X_stdev, X_var_ratio, mean_dev, X_global_mean, Y_comp, Y_mean
+
+
+def _final_arrays(config, X_comp, X_global_mean, X_stdev, X_var_ratio, Z_comp, Z_global_mean, rand_std_dev, lat_samples,
+                  sample_shape, input_shape, input_dims, to_nchw):
+    """The 8 arrays of the file from the exported result: the reference's shapes, and lat_stdev (W space: the spread of 5000
+    latents, ``lat_samples()``, along the latent components) read back together with random_stdevs."""
+    X_comp = to_nchw(X_comp).reshape(-1, *sample_shape)
+    X_global_mean = to_nchw(X_global_mean).reshape(sample_shape)
+    Z_comp = Z_comp.reshape(-1, *input_shape)
+    Z_global_mean = Z_global_mean.reshape(input_shape)
+
+    lat_stdev = np.ones_like(X_stdev)
+    if config.use_w:
+        samples = lat_samples()
+        zc = torch.from_numpy(Z_comp.reshape(-1, input_dims).astype(np.float32))
+        both = torch.cat([rand_std_dev.reshape(-1), _native.project_std(samples.contiguous(), zc).reshape(-1)]).cpu().numpy()
+        X_stdev_random, lat_stdev = both[:rand_std_dev.numel()], both[rand_std_dev.numel():]
+    else:
+        X_stdev_random = rand_std_dev.cpu().numpy()
+    return {
+        "act_comp": X_comp.astype(np.float32),
+        "act_mean": X_global_mean.astype(np.float32),
+        "act_stdev": X_stdev.astype(np.float32),
+        "lat_comp": Z_comp.astype(np.float32),
+        "lat_mean": Z_global_mean.astype(np.float32),
+        "lat_stdev": lat_stdev.astype(np.float32),
+        "var_ratio": X_var_ratio.astype(np.float32),
+        "random_stdevs": X_stdev_random.astype(np.float32),
+    }
 
 
 def compute_arrays(config, instrumented_model, state=None):
@@ -507,22 +568,8 @@ def compute_arrays(config, instrumented_model, state=None):
     pre_dirs = None if device_dirs else \
         torch.from_numpy(to_native(get_random_dirs(config.components, int(np.prod(sample_shape))))).to(device, non_blocking=True)
     pre_lat = model.z_to_latent(lat_stdev_z()).reshape(5000, input_dims) if (config.use_w and lat_stdev_z is not None) else None
-    X_comp, X_stdev, X_var_ratio = transformer.get_components()
-    X_comp = np.array(X_comp, copy=True)
-    mean_dev = transformer.device_outputs["mean"] if pooled else tr.device_attributes()["mean"]
-    if affine is None:
-        X_global_mean = (transformer.pooled_mean if pooled else tr.mean_).reshape((1, sample_dims))
-        Y_comp, Y_mean = X_comp, X_global_mean              # device feature order (== the reference's unless `layout`)
-    else:
-        # lift through the isometry: components = components_y Q^T (svd_flip's sign rule is applied on the lifted
-        # rows, as sklearn would on the full activations), mean = mean_y Q^T + offset
-        lifted = affine.lift_rows(torch.from_numpy(X_comp).to(device))
-        idx = torch.argmax(lifted.abs(), dim=1)
-        signs = torch.sign(lifted[torch.arange(lifted.shape[0], device=device), idx])
-        Y_comp = X_comp * signs.cpu().numpy()[:, None]
-        Y_mean = (transformer.pooled_mean if pooled else tr.mean_).reshape((1, d))
-        X_comp = (lifted * signs[:, None]).cpu().numpy()
-        X_global_mean = (affine.lift_rows(mean_dev[None, :]) + affine.offset[None, :]).cpu().numpy()
+    X_comp, X_stdev, X_var_ratio, mean_dev, X_global_mean, Y_comp, Y_mean = \
+        _export_components(transformer, affine, pooled, sample_dims, device)
 
     assert X_comp.shape[1] == sample_dims and X_comp.shape[0] == config.components \
         and X_global_mean.shape[1] == sample_dims and X_stdev.shape[0] == config.components, "Invalid shape"
@@ -555,36 +602,12 @@ def compute_arrays(config, instrumented_model, state=None):
         X = tr.last_batch_rows(n_rand_samples)              # (feature shards gathered when distributed)
     rand_std_dev = _native.project_std(X[:n_rand_samples], dirs_dev, sub=sub)       # read back below, with lat_stdev
 
-    X_comp = to_nchw(X_comp).reshape(-1, *sample_shape)
-    X_global_mean = to_nchw(X_global_mean).reshape(sample_shape)
-    Z_comp = Z_comp.reshape(-1, *input_shape)
-    Z_global_mean = Z_global_mean.reshape(input_shape)
-
-    lat_stdev = np.ones_like(X_stdev)
-    if config.use_w:
-        if pre_lat is not None:
-            samples = pre_lat
-        else:
-            samples = model.sample_latent(5000).reshape(5000, input_dims)
-        zc = torch.from_numpy(Z_comp.reshape(-1, input_dims).astype(np.float32))
-        both = torch.cat([rand_std_dev.reshape(-1), _native.project_std(samples.contiguous(), zc).reshape(-1)]).cpu().numpy()
-        X_stdev_random, lat_stdev = both[:rand_std_dev.numel()], both[rand_std_dev.numel():]
-    else:
-        X_stdev_random = rand_std_dev.cpu().numpy()
-
+    arrays = _final_arrays(config, X_comp, X_global_mean, X_stdev, X_var_ratio, Z_comp, Z_global_mean, rand_std_dev,
+                           lambda: pre_lat if pre_lat is not None else model.sample_latent(5000).reshape(5000, input_dims),
+                           sample_shape, input_shape, input_dims, to_nchw)
     if hasattr(model, "check_numerics"):
         model.check_numerics()
     tick("random directions + layout")
-    arrays = {
-        "act_comp": X_comp.astype(np.float32),
-        "act_mean": X_global_mean.astype(np.float32),
-        "act_stdev": X_stdev.astype(np.float32),
-        "lat_comp": Z_comp.astype(np.float32),
-        "lat_mean": Z_global_mean.astype(np.float32),
-        "lat_stdev": lat_stdev.astype(np.float32),
-        "var_ratio": X_var_ratio.astype(np.float32),
-        "random_stdevs": X_stdev_random.astype(np.float32),
-    }
     if instrumented_model is None:
         inst.close()
         del inst
@@ -609,6 +632,19 @@ def _compute(submit_config, config, model=None, force_recompute=False):
     if config.use_w and "StyleGAN" not in config.model:
         raise RuntimeError(f"Cannot change latent space of non-StyleGAN model {config.model}")
 
+    dump_path = _dump_path(basedir, config)
+
+    if not dump_path.is_file() or force_recompute:
+        print("Not cached")
+        t_start = datetime.datetime.now()
+        compute(config, dump_path, model)
+        print("Total time:", datetime.datetime.now() - t_start)
+    return dump_path
+
+
+def _dump_path(basedir, config):
+    """The cache file of a decomposition: ``<run_dir>/cache/components/<model>-<class>_<layer>_<estimator>_n<n>[_w][_seed].npz``,
+    named from the requested number of components."""
     transformer = get_estimator(config.estimator, config.components, config.sparsity)
     dump_name = "{}-{}_{}_{}_n{}{}{}.npz".format(
         config.model.lower(),
@@ -619,11 +655,304 @@ def _compute(submit_config, config, model=None, force_recompute=False):
         "_w" if config.use_w else "",
         f"_seed{config.seed}" if config.seed else "",
     )
-    dump_path = basedir / "cache" / "components" / dump_name
+    return Path(basedir) / "cache" / "components" / dump_name
 
-    if not dump_path.is_file() or force_recompute:
-        print("Not cached")
+
+# ---- several layers in one pass -------------------------------------------------------------------------------------------
+# bytes of activation rows (all layers together) whose statistics one set of launches computes in a multi-layer pass; a round
+# of groups that holds more is split, which leaves every group's statistics unchanged
+MULTI_ROWS_BYTES = 2 << 30
+
+
+def get_or_compute_layers(config, layers, model=None, submit_config=None, force_recompute=False):
+    """``get_or_compute`` for several layers of one model at once: returns ``{layer: path}``, each path the file that
+    ``get_or_compute`` with ``config.layer = layer`` returns, with the same arrays.  Layers already in the cache are skipped
+    unless ``force_recompute``.
+
+    The layers share one draw of the latents, one activation run per microbatch (a ``partial_forward`` to the deepest of them
+    with every layer retained), one grouped statistics launch per round and one regression pass; each layer keeps its own
+    merge chain.  Every per-layer random stream is the one ``get_or_compute`` would draw, so the files are the per-layer files.
+
+    Takes the layers a per-layer run decomposes with the small-d engine (d <= 1024) or through an exact affine factorisation
+    (BigGAN ``generator.gen_z`` and its BatchNorm row layers), with ``--est ipca`` and a fixed ``batch_size``, in a single
+    process.  ``config`` is not modified."""
+    layers = list(layers)
+    if len(set(layers)) != len(layers):
+        raise ValueError(f"get_or_compute_layers: repeated layer names in {layers}")
+    if config.n is None:
+        raise RuntimeError("Must specify number of samples with -n=XXX")
+    if model and not isinstance(model, InstrumentedModel):
+        raise RuntimeError('Passed model has to be wrapped in "InstrumentedModel"')
+    if config.use_w and "StyleGAN" not in config.model:
+        raise RuntimeError(f"Cannot change latent space of non-StyleGAN model {config.model}")
+    if config.estimator != "ipca":
+        raise NotImplementedError(f"get_or_compute_layers: --est {config.estimator} is not available for several layers at once "
+                                  "(only ipca); use get_or_compute per layer")
+    if config.batch_size is None:
+        raise ValueError("get_or_compute_layers needs a batch_size: the per-layer memory probe could pick a different B per layer")
+    latents = [l for l in layers if l in ("g_mapping", "style") and config.use_w]
+    if latents:
+        raise ValueError(f"get_or_compute_layers: {latents} are the W latents themselves; they have no activation pass to "
+                         "share: use get_or_compute")
+    if _dist()[2]:
+        raise NotImplementedError("get_or_compute_layers runs in a single process; use get_or_compute in a distributed job")
+    if submit_config is None:
+        wrkdir = str(Path(__file__).parent.resolve())
+        submit_config = SimpleNamespace(run_dir_root=wrkdir, run_dir=wrkdir)
+    configs = {}
+    for layer in layers:
+        configs[layer] = copy.copy(config)
+        configs[layer].layer = layer
+    paths = {layer: _dump_path(submit_config.run_dir, configs[layer]) for layer in layers}
+    todo = [layer for layer in layers if force_recompute or not paths[layer].is_file()]
+    if todo:
+        print("Not cached:", ", ".join(todo))
         t_start = datetime.datetime.now()
-        compute(config, dump_path, model)
+        _compute_layers(config, todo, {layer: configs[layer] for layer in todo}, paths, model)
         print("Total time:", datetime.datetime.now() - t_start)
-    return dump_path
+    return paths
+
+
+def _compute_layers(config, layers, configs, paths, instrumented_model):
+    """Runs the joint pass and writes every layer's file once all of them are computed (an interrupted or failed pass writes
+    nothing)."""
+    timestamp = lambda: datetime.datetime.now().strftime("%d.%m %H:%M")
+    print(f"[{timestamp()}] Computing {len(layers)} layers in one pass")
+    try:
+        arrays = _layers_arrays(config, layers, instrumented_model)
+    except _native.ChainNotConverged as err:
+        # the status word is library-global: which layer's chain found no gap is not known.  Every layer runs again on its own,
+        # each with compute()'s own retry through the direct chain step.
+        print(f"{err}\nRe-running each layer on its own", flush=True)
+        for layer in layers:
+            compute(copy.copy(configs[layer]), paths[layer], instrumented_model)
+        return
+    for layer in layers:
+        _write_npz(paths[layer], arrays[layer])
+
+
+def _layers_arrays(config, layers, instrumented_model):
+    """The 8 arrays of every layer, as ``compute_arrays`` computes them one layer at a time."""
+    global B
+    tick = _phase_timer()
+    torch.manual_seed(0)
+    np.random.seed(0)
+
+    device = _native.require_cuda("cuda")
+    if instrumented_model is None:
+        inst = get_instrumented_model(config.model, config.output_class, list(layers),
+                                      torch.device("cuda", torch.cuda.current_device()))
+        model = inst.model
+    else:
+        print("Reusing InstrumentedModel instance")
+        inst = instrumented_model
+        model = inst.model
+        inst.remove_edits()
+        model.set_output_class(config.output_class)
+    device = model.device
+    if config.use_w:
+        print("Using W latent space")
+        model.use_w()
+
+    # ---- the layers: exact affine factorisation or activations read from the hooks ----------------------------------------
+    spec = {}
+    for layer in layers:
+        affine = model.affine_layer(layer) if hasattr(model, "affine_layer") else None
+        spec[layer] = SimpleNamespace(affine=affine)
+    act_layers = [l for l in layers if spec[l].affine is None]
+
+    # ---- shape pass: one latent (the draw the per-layer run makes), every layer retained ----------------------------------
+    inst.retain_layers(layers)
+    z1 = model.sample_latent(1)
+
+    def run_to(target):
+        for l in layers:
+            inst.retained_layer(l, clear=True)
+        model.partial_forward(z1, target)
+        return {l: v for l, v in inst.retained_features().items() if l in spec and v is not None}
+
+    # the activation pass of every microbatch is one partial_forward to a layer whose run fills every activation layer
+    deepest = None
+    for target in reversed(act_layers):
+        got = run_to(target)
+        if all(l in got for l in act_layers):
+            deepest = target
+            break
+    if act_layers and deepest is None:
+        raise NotImplementedError(f"get_or_compute_layers: no partial_forward of {model.__class__.__name__} reaches all of "
+                                  f"{act_layers}; use get_or_compute")
+    shapes = {l: tuple(got[l].shape) for l in act_layers}
+    for l in layers:
+        if l not in shapes:
+            shapes[l] = tuple(run_to(l)[l].shape)
+    input_shape = inst.model.get_latent_shape()
+    input_dims = int(inst.model.get_latent_dims())
+    B = config.batch_size
+    small_d_max = DeviceIncrementalPCA.SMALL_D_MAX
+    for l in layers:
+        s = spec[l]
+        s.shape = shapes[l]
+        s.dims = int(np.prod(s.shape))
+        s.c = min(config.components, s.dims)
+        print(f"{l}: feature shape {s.shape}")
+        if s.affine is None and s.dims > small_d_max:
+            raise NotImplementedError(f"get_or_compute_layers: {l} is a conv feature map (d = {s.dims} > {small_d_max}, the "
+                                      "large-d engine); use get_or_compute")
+        if s.affine is not None and s.c > s.affine.rank:
+            raise NotImplementedError(f"components={s.c} exceeds the rank {s.affine.rank} of layer {l}")
+        s.d = s.affine.Q.shape[1] if s.affine is not None else s.dims
+        s.plan = _plan.make_plan(config.n, B, s.c)
+        s.transformer = get_estimator(config.estimator, s.c, config.sparsity, device=device)
+    print("B={}, N={}, layers={}".format(B, spec[layers[0]].plan.N, len(layers)), flush=True)
+
+    # ---- Phase A: the seeds; each layer's are a prefix of the longest list (one global stream) ----------------------------
+    torch.manual_seed(config.seed or SEED_SAMPLING)
+    np.random.seed(config.seed or SEED_SAMPLING)
+    seeds = _draw_seeds(max(spec[l].plan.n_calls for l in layers))
+
+    # ---- Phase B: statistics + one merge chain per layer; layers whose plans agree (the same NB) share the pass -----------
+    by_plan = {}
+    for l in layers:
+        by_plan.setdefault(spec[l].plan, []).append(l)
+    for pl, members in by_plan.items():
+        _fit_layers(model, inst, pl, members, spec, seeds, deepest, input_shape, input_dims, device)
+    tick("sampling + activations + IPCA chains")
+
+    # ---- per layer: export, affine lift and sign rule ---------------------------------------------------------------------
+    for l in layers:
+        s = spec[l]
+        s.X_comp, s.X_stdev, s.X_var_ratio, s.mean_dev, s.X_global_mean, s.Y_comp, s.Y_mean = \
+            _export_components(s.transformer, s.affine, False, s.dims, device)
+        assert s.X_comp.shape[1] == s.dims and s.X_comp.shape[0] == s.c and s.X_global_mean.shape[1] == s.dims \
+            and s.X_stdev.shape[0] == s.c, "Invalid shape"
+
+    # ---- one regression pass for every layer ------------------------------------------------------------------------------
+    Z = _linreg_layers(model, inst, config, layers, spec, deepest)
+    tick("export + regression")
+
+    # ---- per layer: random directions, lat_stdev, the arrays ---------------------------------------------------------------
+    shared = {}
+
+    def lat_samples():
+        # the per-layer run draws these 5000 latents right after its regression pass: the same seed for every layer
+        if "lat" not in shared:
+            shared["lat"] = model.sample_latent(5000).reshape(5000, input_dims)
+        return shared["lat"]
+
+    out = {}
+    for l in layers:
+        s = spec[l]
+        Z_comp, Z_global_mean = Z[l]
+        Z_comp /= np.linalg.norm(Z_comp, axis=-1, keepdims=True)
+        dirs = torch.from_numpy(get_random_dirs(s.c, s.dims)).to(device, non_blocking=True)
+        if s.affine is not None:                            # dirs . (x - mean) == (dirs Q) . (y - ybar)
+            dirs = _native.linear(dirs, s.affine.Q.T.float().contiguous())
+        X = s.last_rows
+        rand_std_dev = _native.project_std(X[:min(5000, X.shape[0])], dirs, sub=s.mean_dev)
+        out[l] = _final_arrays(config, s.X_comp, s.X_global_mean, s.X_stdev, s.X_var_ratio, Z_comp, Z_global_mean, rand_std_dev,
+                               lat_samples, s.shape, input_shape, input_dims, lambda A: A)
+    if hasattr(model, "check_numerics"):
+        model.check_numerics()
+    tick("random directions")
+    if instrumented_model is None:
+        inst.close()
+    return out
+
+
+def _fit_layers(model, inst, pl, layers, spec, seeds, deepest, input_shape, input_dims, device):
+    """Phase B of ``compute_arrays`` for several layers with one plan: the same chunks, rounds and groups; each microbatch's
+    activations come from one partial_forward, each round's statistics from one grouped launch (tensor-core widths) plus
+    batch_stats_multi (other widths), and each layer's chain steps through the groups in order on its own stream."""
+    K, NB = pl.K, pl.NB
+    groups_per_chunk = max(1, int(LATENT_CHUNK_BYTES // max(1, NB * input_dims * 4)))
+    acts = [l for l in layers if spec[l].affine is None]
+    grouped = [l for l in layers if _native.stats_grouped_width(spec[l].d)]
+    per_group_bytes = NB * 4 * sum(spec[l].d for l in layers)
+    span_max = max(1, MULTI_ROWS_BYTES // per_group_bytes)
+    stopped = set()
+
+    def layer_rows(rows):
+        """{layer: [n, d] rows} for latent rows ``rows`` (n a multiple of NB), with compute_arrays' microbatches."""
+        out = {l: spec[l].affine.coords(rows) for l in layers if spec[l].affine is not None}
+        if acts:
+            bufs = {l: torch.empty((rows.shape[0], spec[l].d), dtype=torch.float32, device=device) for l in acts}
+            for g0 in range(0, rows.shape[0], NB):
+                for mb in range(0, NB, B):
+                    z = rows[g0 + mb:g0 + mb + B].reshape(-1, *input_shape[1:])
+                    with torch.no_grad():
+                        model.partial_forward(z, deepest)
+                    feats = inst.retained_features()
+                    space_left = min(B, NB - mb)
+                    for l in acts:
+                        bufs[l][g0 + mb:g0 + mb + space_left] = feats[l].reshape((z.shape[0], -1))[:space_left]
+            out.update(bufs)
+        return out
+
+    for c0 in range(0, K, groups_per_chunk):
+        c1 = min(c0 + groups_per_chunk, K)
+        runs = _plan.contiguous_runs(_plan.groups_to_process(pl, 0, 1, c0, c1))
+        needed, offsets = _plan.batch_slots(pl, runs)
+        lat, ensure_rows = _sample_batches_lazy(model, B, [seeds[b] for b in needed])
+        lat = lat.reshape(lat.shape[0], -1)
+        where = {kk: off + (kk - run[0]) * NB for run, off in zip(runs, offsets) for kk in run}
+        for rnd in _plan.rounds(c0, c1, 1, STATS_FIRST_BLOCK if c0 == 0 else STATS_BLOCK, STATS_BLOCK):
+            for s0 in range(0, len(rnd), span_max):
+                span = list(rnd)[s0:s0 + span_max]
+                r0 = where[span[0]]
+                assert all(where[kk] == r0 + i * NB for i, kk in enumerate(span))
+                ensure_rows(r0 + len(span) * NB)
+                X = layer_rows(lat[r0:r0 + len(span) * NB])
+                stats = dict(zip(grouped, _native.batch_stats_grouped([(X[l], len(span), NB, None, None) for l in grouped])))
+                for l in layers:
+                    if l not in stats:
+                        stats[l] = _native.batch_stats_multi(X[l], len(span), NB)
+                    spec[l].last_rows = X[l][(len(span) - 1) * NB:]
+                for i in range(len(span)):
+                    for l in layers:
+                        if l not in stopped and not spec[l].transformer.fit_partial_stats(NB, stats[l][0][i], stats[l][1][i]):
+                            stopped.add(l)      # the per-layer loop leaves its fit here (n_components > first batch)
+        ensure_rows(lat.shape[0])
+        del lat
+
+
+def _linreg_layers(model, inst, config, layers, spec, deepest):
+    """``linreg_lstsq`` for every layer from one pass over the SEED_LINREG latents: {layer: (Z_comp, Z_mean)}."""
+    for l in layers:
+        _warn_if_not_orthonormal(spec[l].Y_comp)
+    print("Performing least squares regression", flush=True)
+    torch.manual_seed(SEED_LINREG)
+    np.random.seed(SEED_LINREG)
+    dev = model.device
+    ops = {}
+    for l in layers:
+        s = spec[l]
+        ops[l] = (torch.from_numpy(s.Y_comp).float().to(dev).contiguous(),
+                  torch.from_numpy(s.Y_mean).float().to(dev).reshape(-1).contiguous(),
+                  torch.from_numpy(s.X_stdev).float().to(dev).contiguous())
+    n_samp = max(10_000, config.n) // B * B
+    latent_dims = int(model.get_latent_dims())      # consumes one global draw, as in the reference (:88)
+    accs = {l: _native.LinregAccumulator(ops[l][0].shape[0], latent_dims, dev) for l in layers}
+    acts = [l for l in layers if spec[l].affine is None]
+    seeds = _draw_seeds(n_samp // B)
+    group = max(1, min(len(seeds), (256 << 20) // max(1, B * latent_dims * 4)))
+    for start in range(0, len(seeds), group):
+        idx = list(range(start, min(start + group, len(seeds))))
+        z_all = _sample_batches(model, B, [seeds[i] for i in idx])
+        for j in range(len(idx)):
+            z = z_all[j * B:(j + 1) * B]
+            if acts:
+                with torch.no_grad():
+                    model.partial_forward(z, deepest)
+                feats = inst.retained_features()
+            for l in layers:
+                if spec[l].affine is not None:
+                    act = spec[l].affine.coords(z.reshape(B, -1))
+                else:
+                    act = feats[l].reshape(B, -1)
+                accs[l].accumulate(act.contiguous(), *ops[l], z.reshape(B, -1).contiguous())
+    out = {}
+    for l in layers:
+        accs[l].n_total = n_samp
+        M_t, Z_mean = accs[l].solve()
+        out[l] = (M_t.cpu().numpy()[:ops[l][0].shape[0], :], Z_mean.cpu().numpy().reshape(1, -1))
+    return out
