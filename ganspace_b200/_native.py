@@ -53,7 +53,8 @@ SIGNATURES = {
     "gsb_project_std": (_I, [_P, _L, _I, _L, _P, _I, _P, _P, _P, _Z, _P]),
     "gsb_linreg_state_bytes": (_Z, [_I, _I]),
     "gsb_linreg_reset": (_I, [_P, _I, _I, _P]),
-    "gsb_linreg_workspace_bytes": (_Z, [_L, _I]),
+    "gsb_linreg_feature_splits": (_I, [_L, _I, _I]),
+    "gsb_linreg_workspace_bytes": (_Z, [_L, _I, _I]),
     "gsb_linreg_accumulate": (_I, [_P, _I, _I, _P, _L, _I, _P, _P, _P, _P, _P, _Z, _P]),
     "gsb_linreg_solve": (_I, [_P, _I, _I, _L, _P, _P, _P]),
     "gsb_linreg_solve_status": (_I, [_P, _I, _I, _P, _P]),
@@ -759,12 +760,12 @@ class LinregAccumulator:
         n, d = act.shape
         act, comp32, mean32, stdev32, z = (t.contiguous() for t in (act, comp32, mean32, stdev32, z))
         assert z.shape == (n, self.L) and comp32.shape == (self.c, d)
-        ws = scratch.get("linreg", lib.gsb_linreg_workspace_bytes(n, self.c), self.dev)
+        ws = scratch.get("linreg", lib.gsb_linreg_workspace_bytes(n, self.c, d), self.dev)
         with torch.cuda.device(self.dev):
             _check(lib.gsb_linreg_accumulate(_ptr(self.state), self.c, self.L, _ptr(act), n, d, _ptr(comp32),
                                              _ptr(mean32), _ptr(stdev32), _ptr(z), _ptr(ws), ws.numel(), _stream()),
                    "gsb_linreg_accumulate")
-        instrument.count(2)
+        instrument.count(2 if lib.gsb_linreg_feature_splits(n, self.c, d) == 1 else 3)     # + the split sum
         self.n_total += n
 
     RCOND = 1e-6        # eigenvalues of A^T A below RCOND * largest count as zero in the minimum-norm fallback

@@ -85,28 +85,46 @@ __global__ void moments_to_std_kernel(const double *__restrict__ mom, int c, dou
 }
 
 // A[r,k] = ((act[r,:] - mean) . comp[k,:]) / stdev[k]      decomposition.py:119-123
+// gridDim.z > 1 (conv feature maps, d ~ 10^5..10^6): the feature axis is split into gridDim.z slabs of a multiple of PJ_K
+// features; CTA z stores its partial coordinates, undivided, in part[z][row][k] -- every (z, row < n, k < c) slot, an
+// empty slab's zeros included -- and linreg_split_sum_kernel adds them in z order.  No atomics: the result does not depend
+// on the order the CTAs run in.
 __global__ void __launch_bounds__(256)
 linreg_coords_kernel(const float *__restrict__ act, int64_t n, int d, const float *__restrict__ comp, int c,
-                     const float *__restrict__ mean, const float *__restrict__ stdev, float *__restrict__ A) {
+                     const float *__restrict__ mean, const float *__restrict__ stdev, float *__restrict__ A,
+                     float *__restrict__ part) {
     __shared__ float Xs[PJ_ROWS][PJ_K + 1], Cs[PJ_COMPS][PJ_K + 1];
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
     const int k0 = blockIdx.y * PJ_COMPS;
     const int64_t r0 = (int64_t)blockIdx.x * PJ_ROWS;
     float acc[8];
-    // gridDim.z > 1 (conv feature maps, d ~ 10^5..10^6): the feature axis is split over CTAs, partial coordinates are
-    // added with fp32 atomics into the zeroed A (the division by stdev distributes over the partial sums)
     const int slab = (int)(((int64_t)d + gridDim.z - 1) / gridDim.z + PJ_K - 1) / PJ_K * PJ_K;
     const int i_begin = blockIdx.z * slab;
     project_tile<2>(act, n, d, d, comp, c, nullptr, mean, r0, k0, acc, Xs, Cs, i_begin, i_begin + slab);
     const int k = k0 + tx;
     if (k >= c) return;
     const float sd = stdev[k];
+    float *slot = part + (size_t)blockIdx.z * n * c;
 #pragma unroll
     for (int r = 0; r < 8; ++r) {
         int64_t row = r0 + ty + 8 * r;
         if (row >= n) continue;
         if (gridDim.z == 1) A[row * c + k] = acc[r] / sd;
-        else atomicAdd(&A[row * c + k], acc[r] / sd);
+        else slot[row * c + k] = acc[r];
+    }
+}
+
+// A[row,k] = (sum_{z < splits} part[z][row][k]) / stdev[k], the sum in z order; one division, after the sum.  A separate
+// kernel rather than a pass folded into linreg_normal_eq_kernel's loader: that loader reads each A element once per
+// 32-column output tile, so folding would re-read all the partials (c + L) / 32 times.
+__global__ void __launch_bounds__(256)
+linreg_split_sum_kernel(const float *__restrict__ part, int splits, int64_t n, int c, const float *__restrict__ stdev,
+                        float *__restrict__ A) {
+    const int64_t nc = n * c;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nc; e += (int64_t)gridDim.x * blockDim.x) {
+        float s = 0.f;
+        for (int z = 0; z < splits; ++z) s += part[z * nc + e];
+        A[e] = s / stdev[e % c];
     }
 }
 
@@ -282,7 +300,21 @@ extern "C" int gsb_linreg_reset(void *d_state, int c, int latent_dim, gsb_stream
     return GSB_OK;
 }
 
-extern "C" size_t gsb_linreg_workspace_bytes(int64_t n, int c) { return gsb::align_up((size_t)n * c * sizeof(float), 256); }
+// Few row tiles and a long feature axis: split d over 2..64 CTAs.  The doubling stops once tiles * splits reaches
+// 8 * SMs, so splits * n * c stays under 2 * 8 * SMs * PJ_ROWS * PJ_COMPS floats for any n.
+extern "C" int gsb_linreg_feature_splits(int64_t n, int c, int d) {
+    if (n <= 0 || c <= 0 || d <= 0) return 1;
+    const int64_t tiles = ((n + gsb::PJ_ROWS - 1) / gsb::PJ_ROWS) * ((c + gsb::PJ_COMPS - 1) / gsb::PJ_COMPS);
+    int splits = 1;
+    while (splits < 64 && tiles * splits < 8 * gsb::num_sms() && d / (2 * splits) >= 4096) splits *= 2;
+    return splits;
+}
+
+extern "C" size_t gsb_linreg_workspace_bytes(int64_t n, int c, int d) {
+    const int splits = gsb_linreg_feature_splits(n, c, d);
+    const size_t a = gsb::align_up((size_t)n * c * sizeof(float), 256);
+    return splits > 1 ? a + gsb::align_up((size_t)splits * n * c * sizeof(float), 256) : a;
+}
 
 extern "C" int gsb_linreg_accumulate(void *d_state, int c, int latent_dim, const float *d_act, int64_t n, int d,
                                      const float *d_comp, const float *d_mean, const float *d_stdev,
@@ -290,22 +322,25 @@ extern "C" int gsb_linreg_accumulate(void *d_state, int c, int latent_dim, const
                                      gsb_stream_t stream) {
     GSB_CHECK_ARG(d_state && d_act && d_comp && d_mean && d_stdev && d_z && d_workspace, "linreg_accumulate: null pointer");
     GSB_CHECK_ARG(n > 0 && c > 0 && c <= 512 && d > 0 && latent_dim > 0, "linreg_accumulate: bad sizes");
-    if (workspace_bytes < gsb_linreg_workspace_bytes(n, c)) {
+    if (workspace_bytes < gsb_linreg_workspace_bytes(n, c, d)) {
         gsb::set_error("linreg_accumulate: workspace too small");
         return GSB_ERR_WORKSPACE;
     }
     cudaStream_t st = (cudaStream_t)stream;
     gsb::LinregView v = gsb::linreg_view(d_state, c, latent_dim);
     float *A = reinterpret_cast<float *>(d_workspace);
-    int splits = 1;                                           // few row tiles and a long feature axis: split d
-    {
-        const int64_t tiles = ((n + gsb::PJ_ROWS - 1) / gsb::PJ_ROWS) * ((c + gsb::PJ_COMPS - 1) / gsb::PJ_COMPS);
-        while (splits < 64 && tiles * splits < 8 * gsb::num_sms() && d / (2 * splits) >= 4096) splits *= 2;
-    }
-    if (splits > 1) GSB_CHECK_CUDA(cudaMemsetAsync(A, 0, (size_t)n * c * sizeof(float), st));
+    float *part = reinterpret_cast<float *>(reinterpret_cast<char *>(d_workspace) +
+                                            gsb::align_up((size_t)n * c * sizeof(float), 256));
+    const int splits = gsb_linreg_feature_splits(n, c, d);
     dim3 g1((unsigned)((n + gsb::PJ_ROWS - 1) / gsb::PJ_ROWS), (c + gsb::PJ_COMPS - 1) / gsb::PJ_COMPS, splits);
-    gsb::linreg_coords_kernel<<<g1, 256, 0, st>>>(d_act, n, d, d_comp, c, d_mean, d_stdev, A);
+    gsb::linreg_coords_kernel<<<g1, 256, 0, st>>>(d_act, n, d, d_comp, c, d_mean, d_stdev, A, part);
     GSB_CHECK_LAUNCH();
+    if (splits > 1) {
+        const int64_t nc = n * c;
+        const int64_t want = (nc + 255) / 256, cap = 8 * gsb::num_sms();
+        gsb::linreg_split_sum_kernel<<<(unsigned)(want < cap ? want : cap), 256, 0, st>>>(part, splits, n, c, d_stdev, A);
+        GSB_CHECK_LAUNCH();
+    }
     dim3 g2((c + latent_dim + gsb::NE_T - 1) / gsb::NE_T, (c + gsb::NE_T - 1) / gsb::NE_T,
             (unsigned)((n + gsb::NE_ROWS - 1) / gsb::NE_ROWS));
     gsb::linreg_normal_eq_kernel<<<g2, 256, 0, st>>>(A, d_z, n, c, latent_dim, v.AtA, v.AtZ, v.sumZ);
