@@ -99,6 +99,7 @@ SIGNATURES = {
     "gsb_bigd_step_gram": (_I, [_P, _P, _L, _I, _I, _L, _I, _I, _P, _P, _Z, _P]),
     "gsb_bigd_step_solve": (_I, [_P, _P, _L, _I, _I, _L, _I, _I, _P, _P, _Z, _P]),
     "gsb_bigd_step_commit": (_I, [_P, _P, _L, _I, _I, _L, _I, _I, _P, _P, _Z, _P]),
+    "gsb_nhwc_to_nchw_rows": (_I, [_P, _L, _P, _L, _L, _I, _I, _I, _P]),
     "gsb_fbpca_state_bytes": (_Z, [_I]),
     "gsb_fbpca_reset": (_I, [_P, _I, _P]),
     "gsb_fbpca_accumulate": (_I, [_P, _I, _I, _L, _P, _P, _P]),
@@ -922,6 +923,18 @@ class PackedSynthesis(_PackedTapGenerator):
     def _rgb_after(self, n_rgb: int) -> int:
         return 2 * (n_rgb - 1)
 
+    def workspace_bytes(self, n_run: int, n: int) -> int:
+        """Workspace of ``forward`` to layer n_run - 1 for n rows, without ToRGBs."""
+        return int(load().gsb_synthesis_workspace_bytes(self.desc, n_run, 0, int(n)))
+
+    def rows_within(self, n_run: int, n: int, budget: int) -> int:
+        """The most rows (n, or a power of two below it) whose ``forward`` to layer n_run - 1 needs at most ``budget`` bytes of
+        workspace; at least 1."""
+        rows = int(n)
+        while rows > 1 and self.workspace_bytes(n_run, rows) > budget:
+            rows = 1 << ((rows - 1).bit_length() - 1)
+        return rows
+
     def style_width(self, k: int) -> int:
         """Width of style layer ``k``'s rows: the input channels of its StyledConv or ToRGB."""
         chain, i = self.slots[k]
@@ -1273,6 +1286,38 @@ def exchange_rows(stage: torch.Tensor, out: torch.Tensor, world: int, group=None
     return out
 
 
+class DeviceMemoryError(NativeError, MemoryError):
+    """A planned allocation does not fit the device's free memory (raised before anything is allocated or launched)."""
+
+
+def check_device_memory(nbytes: int, device, what: str):
+    """Raises DeviceMemoryError if ``nbytes`` exceed the free memory of ``device`` (blocks cached by torch's allocator count
+    as free)."""
+    dev = require_cuda(device)
+    free, total = torch.cuda.mem_get_info(dev)
+    free += torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+    if int(nbytes) > free:
+        raise DeviceMemoryError(f"{what} needs {int(nbytes):,} bytes of device memory, but {dev} has {free:,} of {total:,} "
+                                "bytes free; use fewer components or a smaller batch size")
+
+
+def nhwc_to_nchw_rows(x: torch.Tensor, hw: int, c: int, out: torch.Tensor = None) -> torch.Tensor:
+    """Rows [n, hw*c] in NHWC feature order (the producers' order) permuted to NCHW ([n, c*hw], the reference's flattening) on
+    the device (gsb_nhwc_to_nchw_rows); bit-exact.  fp32 or fp64; ``x`` and ``out`` may be row-strided and must not overlap."""
+    assert x.is_cuda and x.dtype in (torch.float32, torch.float64) and x.dim() == 2 and x.shape[1] == hw * c and x.stride(1) == 1
+    n = int(x.shape[0])
+    out = torch.empty((n, hw * c), dtype=x.dtype, device=x.device) if out is None else out
+    assert out.dtype == x.dtype and out.shape == x.shape and out.stride(1) == 1
+    with torch.cuda.device(x.device):
+        for r0 in range(0, n, 65535):
+            r1 = min(n, r0 + 65535)
+            _check(load().gsb_nhwc_to_nchw_rows(C.c_void_p(x[r0:r1].data_ptr()), x.stride(0), C.c_void_p(out[r0:r1].data_ptr()),
+                                                out.stride(0), r1 - r0, int(hw),
+                                                int(c), x.element_size(), _stream()), "gsb_nhwc_to_nchw_rows")
+    instrument.count(-(-n // 65535))
+    return out
+
+
 class BigIPCA:
     """Large-d IncrementalPCA engine (csrc/bigd.cu): the stacked matrix M = [S*Vt; batch; correction] lives in HBM,
     producers write the batch rows in place (``batch_rows``), ``step`` runs one partial_fit.
@@ -1280,7 +1325,9 @@ class BigIPCA:
     ``shard=(rank, world)``: feature-sharded over a torch.distributed job -- this object holds the column block
     d/world of M; ``step`` all-reduces the small-side Gram (fp64, (c+nb+1)^2) and agrees on the svd_flip signs."""
 
-    def __init__(self, d: int, c: int, nb_max: int, device, shard=None, gram: str = None):
+    def __init__(self, d: int, c: int, nb_max: int, device, shard=None, gram: str = None, reserve: int = 0):
+        """``reserve``: bytes that must stay free next to the engine (e.g. the synthesis workspace of its producer); the
+        constructor raises DeviceMemoryError before it allocates or launches anything if the device cannot hold both."""
         lib = load()
         self.dev = require_cuda(device)
         # small-side Gram kernel: "tc" = tensor cores (wgmma) with a promoted accumulator (gram_tc.cu; default -- measured error vs fp64
@@ -1297,10 +1344,11 @@ class BigIPCA:
                 raise NativeError(f"feature sharding needs d % (16*world) == 0 (d={d}, world={self.shard[1]})")
             d = d // self.shard[1]
         self.d, self.c, self.nb_max = int(d), int(c), int(nb_max)
+        need = BigIPCA.device_bytes(self.d, self.c, self.nb_max, self.flags)
         ws_bytes = lib.gsb_bigd_workspace_bytes(self.d, self.c, self.nb_max, self.flags)
-        if ws_bytes == 0:
-            raise NativeError(f"gsb_bigd_workspace_bytes: {lib.gsb_last_error().decode()}")
         self.rows = lib.gsb_bigd_rows(self.c, self.nb_max)
+        check_device_memory(need + int(reserve), self.dev, f"the large-d IPCA engine (d = {self.d}, {self.c} components, "
+                            f"batches of {self.nb_max} rows: {need / 1e9:.2f} GB, plus {int(reserve) / 1e9:.2f} GB for its producer)")
         self.M = torch.empty((self.rows, self.d), dtype=torch.float32, device=self.dev)
         self.state = torch.empty(lib.gsb_bigd_state_bytes(self.d, self.c), dtype=torch.uint8, device=self.dev)
         self.ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.dev)
@@ -1313,6 +1361,15 @@ class BigIPCA:
         off = int(t_ptr) - self.ws.data_ptr()
         self._T = self.ws[off:off + self.rows * self.rows * 8].view(torch.float64)      # small-side Gram [rows, rows]
         self._rowmax = torch.empty((self.c, 2), dtype=torch.float32, device=self.dev)
+
+    @staticmethod
+    def device_bytes(d: int, c: int, nb_max: int, flags: int = 1) -> int:
+        """Device memory the engine allocates: the stacked matrix M (gsb_bigd_rows x d fp32), state, workspace, batch mean."""
+        lib = load()
+        ws = lib.gsb_bigd_workspace_bytes(int(d), int(c), int(nb_max), int(flags))
+        if ws == 0:
+            raise NativeError(f"gsb_bigd_workspace_bytes: {lib.gsb_last_error().decode()}")
+        return int(lib.gsb_bigd_rows(int(c), int(nb_max))) * int(d) * 4 + int(lib.gsb_bigd_state_bytes(int(d), int(c))) + ws + 8 * int(d)
 
     def batch_rows(self, nb: int) -> torch.Tensor:
         assert 1 <= nb <= self.nb_max

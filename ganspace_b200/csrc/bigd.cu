@@ -313,6 +313,30 @@ bigd_export_small_kernel(const double *__restrict__ unnorm, const double *__rest
     }
 }
 
+// NHWC -> NCHW of whole rows: dst[r][ch * hw + p] = src[r][p * c + ch].  Each row is an [hw, c] matrix transposed through a
+// 32 x 33 shared-memory tile (the extra column keeps the column reads free of bank conflicts): one CTA per (channel tile,
+// pixel tile, row), 32-lane reads along the channels of a pixel and 32-lane writes along the pixels of a channel, both
+// coalesced.  A pure copy: the output holds the input's bits.
+constexpr int TP_TILE = 32, TP_ROWS = 8;
+template <typename T>
+__global__ void __launch_bounds__(TP_TILE * TP_ROWS)
+nhwc_to_nchw_kernel(const T *__restrict__ src, int64_t ld_src, T *__restrict__ dst, int64_t ld_dst, int hw, int c) {
+    __shared__ T tile[TP_TILE][TP_TILE + 1];
+    const int64_t r = blockIdx.z;
+    const int ch0 = blockIdx.x * TP_TILE, p0 = blockIdx.y * TP_TILE;
+    const T *s = src + r * ld_src;
+    T *o = dst + r * ld_dst;
+    for (int i = threadIdx.y; i < TP_TILE; i += TP_ROWS) {
+        const int p = p0 + i, ch = ch0 + threadIdx.x;
+        if (p < hw && ch < c) tile[i][threadIdx.x] = s[(int64_t)p * c + ch];
+    }
+    __syncthreads();
+    for (int i = threadIdx.y; i < TP_TILE; i += TP_ROWS) {
+        const int ch = ch0 + i, p = p0 + threadIdx.x;
+        if (p < hw && ch < c) o[(int64_t)ch * hw + p] = tile[threadIdx.x][i];
+    }
+}
+
 static int bigd_check(int64_t d, int c, int nb_max) {
     GSB_CHECK_ARG(d >= 1024 && d % 16 == 0 && d < (1ll << 31), "bigd: need d >= 1024, d %% 16 == 0 (d=%lld)", (long long)d);
     GSB_CHECK_ARG(c >= 1 && c <= PJ_CMAX, "bigd: need 1 <= c <= %d (c=%d)", PJ_CMAX, c);
@@ -434,6 +458,27 @@ extern "C" int gsb_bigd_export(const void *d_state, const float *d_M, int64_t d,
     }
     bigd_export_small_kernel<<<1, 1024, 0, st>>>(s.unnorm, s.S, d, c, (double)n_seen, d_singular_values, d_explained_variance,
                                                   d_explained_variance_ratio);
+    GSB_CHECK_LAUNCH();
+    return GSB_OK;
+}
+
+extern "C" int gsb_nhwc_to_nchw_rows(const void *d_src, int64_t ld_src, void *d_dst, int64_t ld_dst, int64_t rows, int hw, int c,
+                                     int elem_bytes, gsb_stream_t stream) {
+    using namespace gsb;
+    GSB_CHECK_ARG(d_src && d_dst && d_src != d_dst, "nhwc_to_nchw_rows: null or aliased pointer");
+    GSB_CHECK_ARG(elem_bytes == 4 || elem_bytes == 8, "nhwc_to_nchw_rows: elements of 4 (fp32) or 8 (fp64) bytes (got %d)", elem_bytes);
+    GSB_CHECK_ARG(rows >= 0 && rows <= 65535 && hw >= 1 && c >= 1, "nhwc_to_nchw_rows: bad shape (rows=%lld, hw=%d, c=%d)",
+                  (long long)rows, hw, c);
+    GSB_CHECK_ARG(ld_src >= (int64_t)hw * c && ld_dst >= (int64_t)hw * c, "nhwc_to_nchw_rows: row pitch below hw * c");
+    if (rows == 0) return GSB_OK;
+    dim3 grid((unsigned)((c + TP_TILE - 1) / TP_TILE), (unsigned)((hw + TP_TILE - 1) / TP_TILE), (unsigned)rows);
+    GSB_CHECK_ARG(grid.y <= 65535, "nhwc_to_nchw_rows: hw = %d has too many pixel tiles", hw);
+    if (elem_bytes == 4)
+        nhwc_to_nchw_kernel<float><<<grid, dim3(TP_TILE, TP_ROWS), 0, (cudaStream_t)stream>>>(
+            static_cast<const float *>(d_src), ld_src, static_cast<float *>(d_dst), ld_dst, hw, c);
+    else
+        nhwc_to_nchw_kernel<double><<<grid, dim3(TP_TILE, TP_ROWS), 0, (cudaStream_t)stream>>>(
+            static_cast<const double *>(d_src), ld_src, static_cast<double *>(d_dst), ld_dst, hw, c);
     GSB_CHECK_LAUNCH();
     return GSB_OK;
 }

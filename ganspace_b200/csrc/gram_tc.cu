@@ -263,20 +263,21 @@ row_exponent_kernel(const float *__restrict__ M, int64_t d, int n_rows, int *__r
         }
     }
 }
+// columns [k0, k0 + w) of every row of M (row pitch ld) -> fp16 hi / lo rows of pitch w
 __global__ void __launch_bounds__(256)
-row_split_kernel(const float *__restrict__ M, int64_t d, int n_rows, const int *__restrict__ rexp, __half *__restrict__ hi,
-                 __half *__restrict__ lo) {
+row_split_kernel(const float *__restrict__ M, int64_t ld, int64_t k0, int64_t w, int n_rows, const int *__restrict__ rexp,
+                 __half *__restrict__ hi, __half *__restrict__ lo) {
     const int r = blockIdx.y;
-    const int64_t q = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;           // float4 index within the row
-    if (q >= d / 4) return;
+    const int64_t q = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;           // float4 index within the slab of the row
+    if (q >= w / 4) return;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (r < n_rows) v = reinterpret_cast<const float4 *>(M + (size_t)r * d)[q];
+    if (r < n_rows) v = reinterpret_cast<const float4 *>(M + (size_t)r * ld + k0)[q];
     const float sc = ldexpf(1.f, rexp[r]);
     const float f[4] = {v.x * sc, v.y * sc, v.z * sc, v.w * sc};              // power-of-two scale: exact
     uint2 ph, pl;
     tc::split4(f, ph, pl);
-    reinterpret_cast<uint2 *>(hi + (size_t)r * d)[q] = ph;
-    reinterpret_cast<uint2 *>(lo + (size_t)r * d)[q] = pl;
+    reinterpret_cast<uint2 *>(hi + (size_t)r * w)[q] = ph;
+    reinterpret_cast<uint2 *>(lo + (size_t)r * w)[q] = pl;
 }
 
 }  // namespace gtc
@@ -342,25 +343,38 @@ int gram_tc_grouped_launch(const GramGroupedOperand *ops, int n, cudaStream_t st
     return GSB_OK;
 }
 
+// The fp16 operands cover at most GRAM_TC_SLAB columns of d at a time: wider rows (StyleGAN2 convs.6 .. convs.9, d = 2 M / 4 M)
+// are converted and multiplied slab by slab into the same T, so the operand copy stays 4.4 GB at n_pad = 2112 instead of
+// growing with d (35 GB at d = 4,194,304).  Widths up to one slab (config 5's d = 524,288) run as one launch, as before.
+constexpr int64_t GRAM_TC_SLAB = 524288;
+static int64_t gram_tc_slab(int64_t d) { return d < GRAM_TC_SLAB ? d : GRAM_TC_SLAB; }
+
 size_t gram_tc_workspace_bytes(int n_pad, int64_t d) {
-    return 2 * align_up((size_t)n_pad * d * 2, 256) + align_up((size_t)n_pad * sizeof(int), 256);
+    return 2 * align_up((size_t)n_pad * gram_tc_slab(d) * 2, 256) + align_up((size_t)n_pad * sizeof(int), 256);
 }
 bool gram_tc_supported(int64_t d) { return d % 64 == 0; }
 
 // T[n_pad, n_pad] (fp64, zeroed by the caller) += M[0:n_rows] M[0:n_rows]^T.  ws: gram_tc_workspace_bytes(n_pad, d).
+// The per-row exponents come from the whole row, so every slab is split with the same scale and the slabs' partial sums add up
+// exactly as the chunks of one launch do (fp64 atomics into T).
 int gram_tc(const float *M, int n_rows, int n_pad, int64_t d, void *ws, double *T, cudaStream_t st) {
     using namespace gtc;
     GSB_CHECK_ARG(gram_tc_supported(d) && n_rows <= n_pad, "gram_tc: d %% 64 != 0");
-    const size_t hb = align_up((size_t)n_pad * d * 2, 256);
+    const int64_t slab = gram_tc_slab(d);
+    const size_t hb = align_up((size_t)n_pad * slab * 2, 256);
     __half *hi = reinterpret_cast<__half *>(ws);
     __half *lo = reinterpret_cast<__half *>(reinterpret_cast<char *>(ws) + hb);
     int *rexp = reinterpret_cast<int *>(reinterpret_cast<char *>(ws) + 2 * hb);
     row_exponent_kernel<<<n_pad, 1024, 0, st>>>(M, d, n_rows, rexp);
     GSB_CHECK_LAUNCH();
-    dim3 sg((unsigned)((d / 4 + 255) / 256), (unsigned)n_pad);
-    row_split_kernel<<<sg, 256, 0, st>>>(M, d, n_rows, rexp, hi, lo);
-    GSB_CHECK_LAUNCH();
-    return gram_tc_launch(GramEpilogue::Accumulate, hi, lo, d, d, 1, n_pad, n_rows, rexp, T, st);
+    for (int64_t k0 = 0; k0 < d; k0 += slab) {
+        const int64_t w = (d - k0 < slab) ? d - k0 : slab;                      // a multiple of 64, as d and slab are
+        dim3 sg((unsigned)((w / 4 + 255) / 256), (unsigned)n_pad);
+        row_split_kernel<<<sg, 256, 0, st>>>(M, d, k0, w, n_rows, rexp, hi, lo);
+        GSB_CHECK_LAUNCH();
+        if (int r = gram_tc_launch(GramEpilogue::Accumulate, hi, lo, w, w, 1, n_pad, n_rows, rexp, T, st)) return r;
+    }
+    return GSB_OK;
 }
 
 }  // namespace gsb

@@ -143,18 +143,22 @@ def _sample_batches_lazy(model, Bsz, seeds):
 
 
 # Solve for directions in latent space that match PCs in activation space (reference :77-139)
-def linreg_lstsq(comp_np, mean_np, stdev_np, inst, config, affine=None, native=False):
+def linreg_lstsq(comp_np, mean_np, stdev_np, inst, config, affine=None, native=False, act_buf=None):
     """``affine``: when the hooked layer is affine in the latent (models/biggan.py AffineLayer), comp/mean are
     given in its r-dimensional coordinates and the projections run there: (act-mean).comp^T == (y-ybar).comp_y^T.
     ``native``: comp/mean are given in the model's device feature order (``feature_layout``) and the activations
-    come from ``model.activations_into`` in that same order (no hook read-back, no permutation)."""
+    come from ``model.activations_into`` in that same order (no hook read-back, no permutation); comp/mean may then be
+    device tensors.  ``act_buf``: [>= B, d] rows the native producer may overwrite (the large-d engine's batch rows, once
+    nothing reads them), instead of a new [B, d] buffer."""
     print("Performing least squares regression", flush=True)
     torch.manual_seed(SEED_LINREG)
     np.random.seed(SEED_LINREG)
     model = inst.model
     dev = model.device
-    comp = torch.from_numpy(comp_np).float().to(dev).contiguous()
-    mean = torch.from_numpy(mean_np).float().to(dev).reshape(-1).contiguous()
+    # comp / mean may be device tensors already (conv layers: the engine's export in the device feature order)
+    as_dev = lambda a: (a if torch.is_tensor(a) else torch.from_numpy(a)).float().to(dev)
+    comp = as_dev(comp_np).contiguous()
+    mean = as_dev(mean_np).reshape(-1).contiguous()
     stdev = torch.from_numpy(stdev_np).float().to(dev).contiguous()
 
     n_samp = max(10_000, config.n) // B * B
@@ -163,7 +167,10 @@ def linreg_lstsq(comp_np, mean_np, stdev_np, inst, config, affine=None, native=F
     rank, world, live = _dist()
 
     acc = _native.LinregAccumulator(n_comp, latent_dims, dev)
-    act_buf = torch.empty((B, comp.shape[1]), dtype=torch.float32, device=dev) if native else None
+    if native and act_buf is None:
+        act_buf = torch.empty((B, comp.shape[1]), dtype=torch.float32, device=dev)
+    elif native:
+        act_buf = act_buf[:B]
     seeds = _draw_seeds(n_samp // B)
     group = max(1, min(len(seeds), (256 << 20) // max(1, B * latent_dims * 4)))
     for start in range(0, len(seeds), group):
@@ -199,9 +206,10 @@ def _warn_if_not_orthonormal(comp):
         print(f"WARNING: Computed basis is not orthonormal (determinant={det})")
 
 
-def regression(comp, mean, stdev, inst, config, affine=None, native=False):
-    _warn_if_not_orthonormal(comp)
-    return linreg_lstsq(comp, mean, stdev, inst, config, affine=affine, native=native)
+def regression(comp, mean, stdev, inst, config, affine=None, native=False, act_buf=None, host_comp=None):
+    """``host_comp``: a host copy of ``comp`` (any feature order) for the orthonormality check when ``comp`` is a device tensor."""
+    _warn_if_not_orthonormal(comp if host_comp is None else host_comp)
+    return linreg_lstsq(comp, mean, stdev, inst, config, affine=affine, native=native, act_buf=act_buf)
 
 
 def compute(config, dump_name, instrumented_model):
@@ -359,6 +367,7 @@ def compute_arrays(config, instrumented_model, state=None):
     if affine is not None and config.components > affine.rank:
         raise NotImplementedError(f"components={config.components} exceeds the rank {affine.rank} of layer {layer_key}")
     transformer = get_estimator(config.estimator, config.components, config.sparsity, device=device)
+    tr = transformer.transformer
     # fbpca (the one non-batched estimator on the device path) pools the per-group statistics instead of merging them into a
     # chain, and solves once at the end (estimators.FacebookPCAEstimator, csrc/rsvd.cu)
     pooled = not transformer.batch_support
@@ -395,6 +404,18 @@ def compute_arrays(config, instrumented_model, state=None):
     pl = _plan.make_plan(config.n, B, config.components)
     N, NB = pl.N, pl.NB
     print("B={}, N={}, dims={}, N/dims={:.1f}".format(B, N, sample_dims, N / sample_dims), flush=True)
+    # conv feature maps whose components are large enough to matter (c d >= 4 M) are read back already permuted to NCHW: one
+    # device transpose and one copy, instead of a host copy in NHWC plus a permuted host copy
+    device_layout = layout is not None and config.components * sample_dims >= (1 << 22)
+    if large_d and layout is not None and hasattr(model, "activations_workspace_bytes"):
+        # the engine's stacked matrix and its producer's scratch have to fit the device together: check before anything runs
+        reserve = model.activations_workspace_bytes(layer_key, B)
+        need = _native.BigIPCA.device_bytes(sample_dims // world if live else sample_dims, config.components, NB)
+        _native.check_device_memory(need + reserve, device, f"{model.model_name} {layer_key} (d = {sample_dims}, "
+                                    f"{config.components} components, batches of {NB}): the large-d IPCA engine "
+                                    f"({need:,} bytes) and the synthesis workspace ({reserve:,} bytes)")
+    if device_layout:
+        tr.host_layout = (layout[1][0] * layout[1][1], layout[1][2])
 
     torch.manual_seed(config.seed or SEED_SAMPLING)
     np.random.seed(config.seed or SEED_SAMPLING)
@@ -426,7 +447,6 @@ def compute_arrays(config, instrumented_model, state=None):
     d = affine.Q.shape[1] if affine is not None else sample_dims
     groups_per_chunk = max(1, int(LATENT_CHUNK_BYTES // max(1, NB * input_dims * 4)))
     X = None
-    tr = transformer.transformer
     state["N"] = N
     k = 0
     stop = False                 # fit_partial returned False (e.g. n_components > first batch): the reference leaves the loop (:262-263)
@@ -564,47 +584,62 @@ def compute_arrays(config, instrumented_model, state=None):
     tick("sampling + activations + IPCA chain")
     # host work that does not depend on the chain's result, done while the device still runs the last merge steps (the
     # export below is the first call that waits for them): get_random_dirs' host stream + upload, the lat_stdev latents
-    device_dirs = layout is not None and config.components * sample_dims >= (1 << 22)
+    device_dirs = device_layout
     pre_dirs = None if device_dirs else \
         torch.from_numpy(to_native(get_random_dirs(config.components, int(np.prod(sample_shape))))).to(device, non_blocking=True)
     pre_lat = model.z_to_latent(lat_stdev_z()).reshape(5000, input_dims) if (config.use_w and lat_stdev_z is not None) else None
     X_comp, X_stdev, X_var_ratio, mean_dev, X_global_mean, Y_comp, Y_mean = \
         _export_components(transformer, affine, pooled, sample_dims, device)
+    host_comp = None
+    if device_layout:
+        # X_comp / X_global_mean came back in NCHW order; the regression runs in the device order, on the engine's own export
+        host_comp, Y_comp, Y_mean = X_comp, tr.device_attributes()["components"], mean_dev.reshape(1, -1)
 
     assert X_comp.shape[1] == sample_dims and X_comp.shape[0] == config.components \
         and X_global_mean.shape[1] == sample_dims and X_stdev.shape[0] == config.components, "Invalid shape"
 
+    def random_projections():
+        """random projections of the last group's buffer, centred on the global mean (:289-291,312-316)"""
+        X_last = first if pooled else X
+        n_rand_samples = min(5000, NB if large_d else X_last.shape[0])
+        if device_dirs:
+            # get_random_dirs' stream (RandomState(2).normal) drawn by the device generator: 42M normals at convs.4
+            g = _native.legacy_normal([SEED_RANDOM_DIRS], config.components * sample_dims, device).view(config.components, -1)
+            g = g / torch.linalg.vector_norm(g.double(), dim=1, keepdim=True).float()
+            dirs_dev = g.view(config.components, lc, lh, lw).permute(0, 2, 3, 1).reshape(config.components, -1).contiguous()
+        else:
+            dirs_dev = pre_dirs
+        if affine is not None:                                  # dirs . (x - mean) == (dirs Q) . (y - ybar)
+            dirs_dev = _native.linear(dirs_dev, affine.Q.T.float().contiguous())
+        sub = mean_dev
+        if large_d:                                             # the engine centred the last group in place by its batch mean
+            sub = mean_dev - tr.last_batch_mean()
+            X_last = tr.last_batch_rows(n_rand_samples)         # (feature shards gathered when distributed)
+        return _native.project_std(X_last[:n_rand_samples], dirs_dev, sub=sub)      # read back below, with lat_stdev
+
+    # conv feature maps: the projections of the last batch come first, so that the regression's activations can then be written
+    # over the engine's batch rows instead of into a [B, d] buffer of their own (33.5 GB at convs.8 and B = 2000).  Neither step
+    # draws from a random state the other one reads, so the order changes no result.
+    act_buf = None
+    if large_d:
+        rand_std_dev = random_projections()
+        if layout is not None and not live and B <= tr._chain.nb_max:
+            act_buf = tr._chain.batch_rows(B)
     if samples_are_latents:
         Z_comp = X_comp
         Z_global_mean = X_global_mean
     else:
-        Z_comp, Z_global_mean = regression(Y_comp, Y_mean, X_stdev, inst, config, affine=affine, native=layout is not None)
+        Z_comp, Z_global_mean = regression(Y_comp, Y_mean, X_stdev, inst, config, affine=affine, native=layout is not None,
+                                           act_buf=act_buf, host_comp=host_comp)
 
     tick("export + regression")
     Z_comp /= np.linalg.norm(Z_comp, axis=-1, keepdims=True)
-
-    # random projections of the last group's buffer, centred on the global mean (:289-291,312-316)
-    if pooled:
-        X = first
-    n_rand_samples = min(5000, NB if large_d else X.shape[0])
-    if device_dirs:
-        # get_random_dirs' stream (RandomState(2).normal) drawn by the device generator: 42M normals at convs.4
-        g = _native.legacy_normal([SEED_RANDOM_DIRS], config.components * sample_dims, device).view(config.components, -1)
-        g = g / torch.linalg.vector_norm(g.double(), dim=1, keepdim=True).float()
-        dirs_dev = g.view(config.components, lc, lh, lw).permute(0, 2, 3, 1).reshape(config.components, -1).contiguous()
-    else:
-        dirs_dev = pre_dirs
-    if affine is not None:                                  # dirs . (x - mean) == (dirs Q) . (y - ybar)
-        dirs_dev = _native.linear(dirs_dev, affine.Q.T.float().contiguous())
-    sub = mean_dev
-    if large_d:                                             # the engine centred the last group in place by its batch mean
-        sub = mean_dev - tr.last_batch_mean()
-        X = tr.last_batch_rows(n_rand_samples)              # (feature shards gathered when distributed)
-    rand_std_dev = _native.project_std(X[:n_rand_samples], dirs_dev, sub=sub)       # read back below, with lat_stdev
+    if not large_d:
+        rand_std_dev = random_projections()
 
     arrays = _final_arrays(config, X_comp, X_global_mean, X_stdev, X_var_ratio, Z_comp, Z_global_mean, rand_std_dev,
                            lambda: pre_lat if pre_lat is not None else model.sample_latent(5000).reshape(5000, input_dims),
-                           sample_shape, input_shape, input_dims, to_nchw)
+                           sample_shape, input_shape, input_dims, (lambda A: A) if device_layout else to_nchw)
     if hasattr(model, "check_numerics"):
         model.check_numerics()
     tick("random directions + layout")

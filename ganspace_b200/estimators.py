@@ -40,6 +40,7 @@ class DeviceIncrementalPCA:
         self._dev = None             # ... and its device tensors
         self._shard = None           # (rank, world): feature-sharded large-d engine (SURVEY.md section 8e)
         self._stage = None
+        self.host_layout = None      # large-d engine: (hw, c) of NHWC rows -- components_ / mean_ are read back in NCHW order
         self.n_samples_seen_ = np.int64(0)
 
     def enable_feature_sharding(self, rank, world):
@@ -171,6 +172,16 @@ class DeviceIncrementalPCA:
                     host[k] = flat[off:off + n].reshape(tuple(dev[k].shape)).astype(
                         np.float32 if dev[k].dtype == torch.float32 else np.float64)
                     off += n
+            elif self.host_layout is not None:
+                # conv feature maps in the producers' NHWC order: components and mean are permuted to the reference's NCHW
+                # order on the device (gsb_nhwc_to_nchw_rows), then copied once; the device tensors keep the NHWC order
+                hw, ch = self.host_layout
+                host = {}
+                for k, v in dev.items():
+                    if k in ("components", "mean", "var"):
+                        host[k] = _native.nhwc_to_nchw_rows(v.reshape(-1, hw * ch), hw, ch).cpu().numpy().reshape(v.shape)
+                    else:
+                        host[k] = v.cpu().numpy()
             else:                                        # conv feature maps: 168 MB of components, copied as they are
                 host = {k: v.cpu().numpy() for k, v in dev.items()}
             self._dev = dev

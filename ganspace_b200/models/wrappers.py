@@ -299,6 +299,12 @@ class _StyledGenerator(_DeviceGenerator):
 class StyleGAN2(_StyledGenerator):
     CONFIGS = {"ffhq": 1024, "car": 512, "cat": 256, "church": 256, "horse": 256,
                "bedrooms": 256, "kitchen": 256, "places": 256}
+    # deepest feature maps get_or_compute decomposes: convs.8 / convs.9, 128 x 128 x 256.  At c = 80 and a 2000-row batch the large-d
+    # engine's stacked matrix is 2112 x d fp32 -- 35.4 GB there -- and convs.10 (d = 8,388,608) would need 71 GB for it alone
+    MAX_DECOMPOSITION_DIMS = 4_194_304
+    # largest synthesis workspace one activations_into call allocates: bigger batches run in slices of rows (the chain's workspace
+    # holds four fp16 planes of the widest input map, 8.4 GB per 1000 samples into convs.8)
+    SYNTH_WORKSPACE_BUDGET = 4 << 30
 
     def __init__(self, device, class_name, truncation=1.0, use_w=False, random_init=None):
         super().__init__("StyleGAN2", class_name or "ffhq")
@@ -510,8 +516,23 @@ class StyleGAN2(_StyledGenerator):
         ``out`` [n, H*W*C] (may be row-strided): the decomposition driver's producer for conv layers."""
         names = self.synthesis_layer_names()
         n_run = names.index(layer_name) + 1
-        w = x if self.w_primary else self.model.style(x)
-        return self._synthesis(n_run).forward(w.reshape(-1, 512), n_run, out=out)[0]
+        w = (x if self.w_primary else self.model.style(x)).reshape(-1, 512)
+        synth = self._synthesis(n_run)
+        step = synth.rows_within(n_run, w.shape[0], self.SYNTH_WORKSPACE_BUDGET)
+        if step >= w.shape[0]:
+            return synth.forward(w, n_run, out=out)[0]
+        # every kernel of the chain treats each sample on its own, so slices of rows give the bits of one call
+        if out is None:
+            out = torch.empty((w.shape[0], synth.out_dims(n_run)), dtype=torch.float32, device=self.device)
+        for r0 in range(0, w.shape[0], step):
+            synth.forward(w[r0:r0 + step], n_run, out=out[r0:r0 + step])
+        return out
+
+    def activations_workspace_bytes(self, layer_name, n):
+        """Device scratch that ``activations_into`` of ``n`` rows to ``layer_name`` allocates (at most SYNTH_WORKSPACE_BUDGET)."""
+        n_run = self.synthesis_layer_names().index(layer_name) + 1
+        synth = self._synthesis(n_run)
+        return synth.workspace_bytes(n_run, synth.rows_within(n_run, n, self.SYNTH_WORKSPACE_BUDGET))
 
     def set_noise_seed(self, seed):
         # same generator stream as the reference (torch.manual_seed(seed); torch.randn per noise map),
