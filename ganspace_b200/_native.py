@@ -20,6 +20,7 @@ _P, _I, _L, _Z, _D, _F = C.c_void_p, C.c_int, C.c_int64, C.c_size_t, C.c_double,
 SIGNATURES = {
     "gsb_abi_version": (_I, []),
     "gsb_last_error": (C.c_char_p, []),
+    "gsb_state_layout_version": (_I, [_I]),
     "gsb_legacy_normal_f32": (_I, [_P, _I, _L, _P, _L, _P]),
     "gsb_legacy_truncnorm_f32": (_I, [_P, _I, _L, _D, _D, _F, _P, _L, _P]),
     "gsb_mt19937_raw_u32": (_I, [_P, _I, _L, _P, _L, _P]),
@@ -182,6 +183,27 @@ def load():
             raise NativeError("ABI version mismatch between ganspace_b200/_native.py and the library")
         _lib = lib
     return _lib
+
+
+STATE_KINDS = {"ipca": 0, "bigd": 1, "fbpca": 2}        # GSB_STATE_* of include/ganspace_b200.h
+
+
+def state_layout_version(kind: str) -> int:
+    """The layout version the library reports for an engine's state blob ('ipca', 'bigd' or 'fbpca')."""
+    return int(load().gsb_state_layout_version(STATE_KINDS[kind]))
+
+
+def _to_host(t: torch.Tensor):
+    """One device -> host copy of a saved blob, as a NumPy array."""
+    return t.detach().cpu().numpy()
+
+
+def _load_blob(dst: torch.Tensor, src, what: str):
+    """Copy a saved host blob into the device tensor ``dst``; its size must be the tensor's."""
+    src = torch.as_tensor(src)
+    if src.numel() != dst.numel() or src.dtype != dst.dtype:
+        raise ValueError(f"{what}: saved blob of {src.numel()} x {src.dtype} does not fit {dst.numel()} x {dst.dtype}")
+    dst.copy_(src.reshape(dst.shape))
 
 
 def require_cuda(device=None) -> torch.device:
@@ -651,6 +673,22 @@ class IPCAChain:
         if self.stream is not None:
             with torch.cuda.device(self.dev):
                 torch.cuda.current_stream().wait_stream(self.stream)
+
+    def state_dict(self):
+        """The chain after the steps enqueued so far: the fp64 state blob (with the iterated chain's (H, Q)) and n_seen."""
+        self.join()
+        with torch.cuda.device(self.dev):
+            return {"state": _to_host(self.state), "n_seen": self.n_seen}
+
+    def load_state_dict(self, sd):
+        """Continue from a ``state_dict`` of a chain of the same (d, c) and chain mode; later steps see what they would have
+        seen after the saved steps."""
+        self.join()
+        with torch.cuda.device(self.dev):
+            _load_blob(self.state, sd["state"], "IPCAChain.load_state_dict")
+            if self.stream is not None:
+                self.stream.wait_stream(torch.cuda.current_stream())
+        self.n_seen = int(sd["n_seen"])
 
     def export(self):
         lib = load()
@@ -1375,6 +1413,21 @@ class BigIPCA:
         assert 1 <= nb <= self.nb_max
         return self.M[self.c:self.c + nb]
 
+    def state_dict(self):
+        """What the next step reads: S*Vt (rows [0, c) of M), the fp64 state blob (mean, unnormalised variance, S), n_seen,
+        and the last batch's mean and size (for its centred rows)."""
+        with torch.cuda.device(self.dev):
+            return {"M": _to_host(self.M[:self.c]), "state": _to_host(self.state), "batch_mean": _to_host(self.batch_mean),
+                    "n_seen": self.n_seen, "last_nb": self.last_nb}
+
+    def load_state_dict(self, sd):
+        """Continue from a ``state_dict`` of an engine of the same (d, c); this engine's nb_max may be larger."""
+        with torch.cuda.device(self.dev):
+            _load_blob(self.M[:self.c], sd["M"], "BigIPCA.load_state_dict")
+            _load_blob(self.state, sd["state"], "BigIPCA.load_state_dict")
+            _load_blob(self.batch_mean, sd["batch_mean"], "BigIPCA.load_state_dict")
+        self.n_seen, self.last_nb = int(sd["n_seen"]), int(sd["last_nb"])
+
     def _args(self, nb):
         return (_ptr(self.state), _ptr(self.M), self.d, self.c, self.nb_max, self.n_seen, int(nb), self.flags)
 
@@ -1488,6 +1541,16 @@ class FBPCAPool:
                                                _stream()), "gsb_fbpca_accumulate")
         instrument.count(2)
         self.n += g * int(rows_per_group)
+
+    def state_dict(self):
+        """The pool so far: its state blob (n, mean, centred scatter) and row count."""
+        with torch.cuda.device(self.dev):
+            return {"state": _to_host(self.state), "n": self.n}
+
+    def load_state_dict(self, sd):
+        with torch.cuda.device(self.dev):
+            _load_blob(self.state, sd["state"], "FBPCAPool.load_state_dict")
+        self.n = int(sd["n"])
 
     def add_zero_rows(self, n_zero: int):
         if n_zero <= 0:

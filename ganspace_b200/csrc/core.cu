@@ -72,3 +72,11 @@ int tc_make_tmap(CUtensorMap *map, CUtensorMapDataType type, const void *base, i
 
 extern "C" int gsb_abi_version(void) { return GSB_ABI_VERSION; }
 extern "C" const char *gsb_last_error(void) { return gsb::g_err; }
+extern "C" int gsb_state_layout_version(int kind) {
+    switch (kind) {
+        case GSB_STATE_IPCA: return GSB_IPCA_STATE_LAYOUT;
+        case GSB_STATE_BIGD: return GSB_BIGD_STATE_LAYOUT;
+        case GSB_STATE_FBPCA: return GSB_FBPCA_STATE_LAYOUT;
+        default: return -1;
+    }
+}

@@ -24,6 +24,7 @@ from __future__ import annotations
 import copy
 import datetime
 import inspect
+import json
 import os
 import sys
 from pathlib import Path
@@ -212,13 +213,17 @@ def regression(comp, mean, stdev, inst, config, affine=None, native=False, act_b
     return linreg_lstsq(comp, mean, stdev, inst, config, affine=affine, native=native, act_buf=act_buf)
 
 
-def compute(config, dump_name, instrumented_model):
-    """decomposition.compute (:150-358): run the pipeline, rank 0 writes the 8-array .npz."""
+def compute(config, dump_name, instrumented_model, resume=None, state_path=None):
+    """decomposition.compute (:150-358): run the pipeline, rank 0 writes the 8-array .npz.  ``resume`` / ``state_path``: see
+    ``compute_arrays``; the direct-step retry after ``ChainNotConverged`` always runs from scratch."""
     timestamp = lambda: datetime.datetime.now().strftime("%d.%m %H:%M")
     print(f"[{timestamp()}] Computing", dump_name.name)
     state = {}
+    # get_or_extend's arguments reach compute_arrays only when given, so the default call is the one it always was
+    extend = {} if state_path is None else {"state_path": state_path}
+    first_try = extend if resume is None else dict(extend, resume=resume)
     try:
-        arrays = compute_arrays(config, instrumented_model, state)
+        arrays = compute_arrays(config, instrumented_model, state, **first_try)
     except _native.ChainNotConverged as err:
         # the iterated chain step found no spectral gap after component c (e.g. activations of numerical rank < n_components):
         # run again with sklearn's own exact per-step eigen-solve (every rank of a distributed run sees the same status)
@@ -226,7 +231,7 @@ def compute(config, dump_name, instrumented_model):
         _native.set_chain_mode(True)
         try:
             state = {}
-            arrays = compute_arrays(config, instrumented_model, state)
+            arrays = compute_arrays(config, instrumented_model, state, **extend)
         finally:
             _native.set_chain_mode(False)
     if state.get("canceled_at") is not None:
@@ -320,10 +325,14 @@ def _final_arrays(config, X_comp, X_global_mean, X_stdev, X_var_ratio, Z_comp, Z
     }
 
 
-def compute_arrays(config, instrumented_model, state=None):
+def compute_arrays(config, instrumented_model, state=None, resume=None, state_path=None):
     """Everything of compute() up to (not including) the file write; returns the 8 float32 arrays.
     ``state`` (optional dict) receives N and, after a KeyboardInterrupt in the fitting loop, ``canceled_at`` = the
-    number of samples fitted so far (single-process runs; the result then describes that prefix of the chain)."""
+    number of samples fitted so far (single-process runs; the result then describes that prefix of the chain).
+
+    Single-process runs only: ``resume`` (a ``StateFile``) continues from a saved engine state of the first K1 groups when its
+    key matches this run's and K1 <= K (else the run starts from scratch and says why); only groups K1 ... K-1 are generated
+    and fitted.  ``state_path``: where the engine state after the last merged group is written (also after a Ctrl-C)."""
     global B
     tick = _phase_timer()
     state = {} if state is None else state
@@ -455,6 +464,33 @@ def compute_arrays(config, instrumented_model, state=None):
     # rest of the first min(5000, N + NB) rows stay zero.  Each row is written by the rank that owns its group.
     first = torch.zeros((min(5000, N + NB), d), dtype=torch.float32, device=device) if pooled else None
 
+    # ---- a saved state of the first K1 groups (get_or_extend): the plan is prefix-stable, so they are this run's first groups
+    K1 = 0
+    key = None
+    if resume is not None or state_path is not None:
+        engine = "fbpca" if pooled else ("bigd" if large_d else "ipca")
+        key = _state_key(config, model, transformer.get_param_str(), B, NB, d, engine)
+    if resume is not None:
+        why = resume.mismatch(key, K)
+        if why:
+            print(f"Not resuming from {resume.path.name}: {why}; running from scratch", flush=True)
+        else:
+            blobs = resume.load()
+            transformer.load_state_dict(blobs, device)
+            if pooled:
+                saved = torch.from_numpy(blobs["first"]).to(device)
+                first[:saved.shape[0]] = saved
+            K1 = resume.groups
+            print(f"Resuming from {resume.path.name}: {K1} of {K} groups fitted", flush=True)
+
+    def keep_state():
+        """Write the engine state after the groups merged so far (for fbpca: before its zero rows, which depend on N)."""
+        if state_path is None or (pooled and transformer._pool is None) or (not pooled and tr._chain is None):
+            return
+        groups = int(transformer._pool.n if pooled else tr.n_samples_seen_) // NB
+        extra = {"first": first[:min(first.shape[0], groups * NB)]} if pooled else {}
+        StateFile.write(state_path, key, groups, transformer.state_dict(), extra)
+
     def group_rows(rows):
         """[n, d] activations of the hooked layer for latent rows ``rows`` (small-d engine; n is a multiple of NB)."""
         if samples_are_latents:
@@ -473,7 +509,8 @@ def compute_arrays(config, instrumented_model, state=None):
         return out
 
     try:
-        for c0 in range(0, K, groups_per_chunk):
+        # a resumed run starts at group K1; when K1 == K the last group is replayed for its rows only (random_stdevs)
+        for c0 in range(K - 1 if 0 < K1 == K else K1, K, groups_per_chunk):
             if stop:
                 break
             c1 = min(c0 + groups_per_chunk, K)
@@ -507,7 +544,9 @@ def compute_arrays(config, instrumented_model, state=None):
                                 with torch.no_grad():
                                     model.partial_forward(z, layer_key)
                                 X[a - lo:b_ - lo] = inst.retained_features()[layer_key].reshape((z.shape[0], -1))
-                        if not transformer.fit_partial_inplace(NB):
+                        if k < K1:
+                            tr.centre_last_batch()          # replayed: the rows as the saved state's last step left them
+                        elif not transformer.fit_partial_inplace(NB):
                             stop = True
                             break
             else:
@@ -547,6 +586,8 @@ def compute_arrays(config, instrumented_model, state=None):
                     if exchange is None:
                         for i, kk in enumerate(own):
                             k = kk
+                            if kk < K1:
+                                continue                    # replayed for its rows only
                             if not transformer.fit_partial_stats(NB, means[i], grams[i]):
                                 stop = True
                                 break
@@ -568,10 +609,13 @@ def compute_arrays(config, instrumented_model, state=None):
     except KeyboardInterrupt:
         if live:
             raise
+        keep_state()
         if pooled:
             sys.exit(1)          # nothing fitted yet, and the reference writes nothing (:269-270)
         # the reference's `gi` of the interrupted group (:268-272) = the samples merged so far
         state["canceled_at"] = int(tr.n_samples_seen_)
+    else:
+        keep_state()
     if pooled:
         if live:
             import torch.distributed as dist
@@ -691,6 +735,158 @@ def _dump_path(basedir, config):
         f"_seed{config.seed}" if config.seed else "",
     )
     return Path(basedir) / "cache" / "components" / dump_name
+
+
+# ---- extending a decomposition to more samples -----------------------------------------------------------------------------
+# environment switches (DESIGN.md section 7b) that change a result; a state is only continued under the ones it was written with
+RESULT_SWITCHES = ("CHAIN", "STATS", "MAPPING", "BIGD_GRAM", "BIGGAN_AFFINE")
+
+
+def _weights_key(model):
+    """Where the model's weights came from: the random-init seed, or the checkpoint with its size and mtime (None: unknown)."""
+    src = getattr(model, "weight_source", None)
+    if src is None:
+        return None
+    if isinstance(src, int):
+        return {"random_init": src}
+    p = Path(src).resolve()
+    st = p.stat()
+    return {"checkpoint": str(p), "size": st.st_size, "mtime_ns": st.st_mtime_ns}
+
+
+def _state_key(config, model, param_str, Bsz, NB, d, engine):
+    """Everything a saved engine state of the first groups depends on, as JSON-ready values."""
+    switches = {s: os.environ[f"GANSPACE_B200_{s}"] for s in RESULT_SWITCHES if os.environ.get(f"GANSPACE_B200_{s}") is not None}
+    if _native._chain_forced_direct:                     # compute()'s direct-step retry
+        switches["CHAIN"] = "direct"
+    return {"model": config.model, "class": config.output_class, "layer": config.layer, "estimator": param_str,
+            "c": int(config.components), "use_w": bool(config.use_w), "seed": config.seed, "B": int(Bsz), "NB": int(NB),
+            "d": int(d), "weights": _weights_key(model), "switches": switches,
+            "layout": {engine: _native.state_layout_version(engine)}}
+
+
+class StateFile:
+    """A saved engine state: ``GSBSTATE``, the length of a JSON header (8 bytes, little endian), the header (key, groups fitted,
+    blob table, scalars), then the raw blobs, uncompressed and 64-byte aligned (1.3 GB for the large-d engine at ``convs.8`` and
+    c = 80).  Opening reads the header and checks the file's length; ``load`` reads the blobs."""
+
+    MAGIC = b"GSBSTATE"
+    SUFFIX = ".gsbstate"
+    ALIGN = 64
+
+    def __init__(self, path):
+        self.path = Path(path)
+        size = self.path.stat().st_size
+        with open(self.path, "rb") as f:
+            head = f.read(16)
+            if len(head) < 16 or head[:8] != self.MAGIC:
+                raise ValueError(f"{self.path}: not a decomposition state file")
+            n = int.from_bytes(head[8:16], "little")
+            raw = f.read(n)
+        if len(raw) < n:
+            raise ValueError(f"{self.path}: the state file is cut short (its header needs {16 + n} bytes, the file has {size})")
+        self.meta = json.loads(raw.decode())
+        self.body = self._body(n)
+        end = max([self.body + b["offset"] + b["nbytes"] for b in self.meta["blobs"]], default=16 + n)
+        if size < end:
+            raise ValueError(f"{self.path}: the state file is cut short ({size} of {end} bytes); delete it to start from scratch")
+        self.groups = int(self.meta["groups"])
+
+    def mismatch(self, key, K):
+        """Why this state cannot start a run with ``key`` and K groups ('' when it can)."""
+        saved = self.meta["key"]
+        if key["weights"] is None:
+            return "the model does not say where its weights came from"
+        diff = [f"{k} {saved.get(k)!r} -> {key[k]!r}" for k in key if saved.get(k) != json.loads(json.dumps(key[k]))]
+        if diff:
+            return "the key differs: " + ", ".join(diff)
+        if self.groups > K:
+            return f"it holds {self.groups} groups, more than the {K} of this run"
+        return ""
+
+    def load(self):
+        """The blobs (NumPy arrays) and scalars of the saved ``state_dict``."""
+        out = dict(self.meta["scalars"])
+        for b in self.meta["blobs"]:
+            out[b["name"]] = np.fromfile(self.path, dtype=np.dtype(b["dtype"]), count=int(np.prod(b["shape"], dtype=np.int64)),
+                                         offset=self.body + b["offset"]).reshape(b["shape"])
+        return out
+
+    @classmethod
+    def _body(cls, header_bytes):
+        """Offset of the first blob: magic, length and header, padded to the alignment (blob offsets count from here)."""
+        return -(-(16 + header_bytes) // cls.ALIGN) * cls.ALIGN
+
+    @classmethod
+    def write(cls, path, key, groups, sd, extra=None):
+        """Write ``sd`` (a ``state_dict``: arrays become blobs, the rest scalars) plus ``extra`` device tensors; atomically."""
+        path = Path(path)
+        os.makedirs(path.parent, exist_ok=True)
+        arrays = {k: v for k, v in sd.items() if isinstance(v, np.ndarray)}
+        arrays.update({k: v.cpu().numpy() for k, v in (extra or {}).items()})
+        scalars = {k: v for k, v in sd.items() if not isinstance(v, np.ndarray)}
+        table, off = [], 0
+        for name, a in arrays.items():
+            table.append({"name": name, "dtype": a.dtype.str, "shape": list(a.shape), "offset": off, "nbytes": int(a.nbytes)})
+            off += -(-int(a.nbytes) // cls.ALIGN) * cls.ALIGN
+        head = json.dumps({"key": key, "groups": int(groups), "scalars": scalars, "blobs": table}).encode()
+        body = cls._body(len(head))
+        tmp = path.with_name(path.name + ".tmp")
+        with open(tmp, "wb") as f:
+            f.write(cls.MAGIC + len(head).to_bytes(8, "little") + head)
+            for (name, a), b in zip(arrays.items(), table):
+                f.seek(body + b["offset"])
+                f.write(np.ascontiguousarray(a).data)
+            f.truncate(body + off)
+        os.replace(tmp, path)
+        print(f"Saved the state after {groups} groups to {path.name}", flush=True)
+
+
+def _state_path(dump_path, config):
+    """``<run_dir>/cache/components/state/<the cache file's name without _n<n>>.gsbstate``: one state per decomposition, whatever
+    its N."""
+    name = dump_path.name
+    i = name.rindex(f"_n{config.n}")
+    return dump_path.parent / "state" / (name[:i] + name[i + len(f"_n{config.n}"):-len(".npz")] + StateFile.SUFFIX)
+
+
+def get_or_extend(config, model=None, submit_config=None, force_recompute=False):
+    """``get_or_compute`` that continues an earlier run instead of starting over: returns the same path and writes the same
+    file, with the same bits as a fresh run.
+
+    The cache file is returned if it exists (unless ``force_recompute``).  Otherwise the saved engine state under
+    ``<run_dir>/cache/components/state/`` -- the state after the first K1 groups of an earlier run of the same decomposition
+    with any N, or of an interrupted one -- is continued when it matches this run (model, class, layer, estimator, c, W space,
+    seed, batch size, group size, width, weights, result-changing switches and the library's state layout); only the groups
+    K1 ... K-1 are generated and fitted.  Any mismatch starts from scratch and says why; ``force_recompute`` always does.  The
+    final state is always left behind.  Ctrl-C writes, besides ``ipca``'s partial ``n{gi}`` file (as ``get_or_compute``), the
+    state after the last merged group, so the same call continues from there; ``fbpca`` writes its pool state and no ``.npz``.
+
+    Single process, with a fixed ``batch_size`` (the memory probe may pick another B from one run to the next)."""
+    if config.n is None:
+        raise RuntimeError("Must specify number of samples with -n=XXX")
+    if model and not isinstance(model, InstrumentedModel):
+        raise RuntimeError('Passed model has to be wrapped in "InstrumentedModel"')
+    if config.use_w and "StyleGAN" not in config.model:
+        raise RuntimeError(f"Cannot change latent space of non-StyleGAN model {config.model}")
+    if config.batch_size is None:
+        raise ValueError("get_or_extend needs a batch_size: the memory probe can pick a different B from one run to the next, "
+                         "and a saved state only continues a run with its own B")
+    if _dist()[2]:
+        raise NotImplementedError("get_or_extend runs in a single process; use get_or_compute in a distributed job")
+    if submit_config is None:
+        wrkdir = str(Path(__file__).parent.resolve())
+        submit_config = SimpleNamespace(run_dir_root=wrkdir, run_dir=wrkdir)
+    dump_path = _dump_path(submit_config.run_dir, config)
+    if dump_path.is_file() and not force_recompute:
+        return dump_path
+    state_path = _state_path(dump_path, config)
+    resume = StateFile(state_path) if (state_path.is_file() and not force_recompute) else None    # checked before any launch
+    print("Not cached" if resume is None else f"Not cached; found {state_path.name}")
+    t_start = datetime.datetime.now()
+    compute(config, dump_path, model, resume=resume, state_path=state_path)
+    print("Total time:", datetime.datetime.now() - t_start)
+    return dump_path
 
 
 # ---- several layers in one pass -------------------------------------------------------------------------------------------

@@ -140,6 +140,43 @@ class DeviceIncrementalPCA:
         self.merge(*self.batch_stats(X))
         return self
 
+    # -- saved state (decomposition.get_or_extend) ------------------------------------------------------
+    def state_dict(self):
+        """The engine after the batches merged so far, as host arrays (one device -> host copy per blob) plus its sizes:
+        ``engine`` is 'ipca' (small-d chain) or 'bigd' (large-d engine, with its batch size ``nb``)."""
+        if self._chain is None:
+            raise AttributeError("IncrementalPCA is not fitted yet")
+        if self._shard is not None:
+            raise NotImplementedError("a feature-sharded engine's state is not saved")
+        sd = self._chain.state_dict()
+        sd.update(engine="bigd" if self.is_large_d else "ipca", d=int(self._chain.d), c=int(self.n_components))
+        if self.is_large_d:
+            sd["nb"] = int(self._chain.nb_max)
+        return sd
+
+    def load_state_dict(self, sd, device=None):
+        """Continue from ``state_dict()``: the engine is created for its (d, nb) if there is none yet."""
+        if int(sd["c"]) != self.n_components:
+            raise ValueError(f"saved state has {sd['c']} components, this estimator {self.n_components}")
+        chain = self._ensure(int(sd["d"]), device if device is not None else self._device, nb=sd.get("nb"))
+        if (sd["engine"] == "bigd") != self.is_large_d:
+            raise ValueError(f"saved state of the {sd['engine']} engine does not fit this one")
+        chain.load_state_dict(sd)
+        self.n_samples_seen_ = np.int64(chain.n_seen)
+        self._host = None
+        return self
+
+    def centre_last_batch(self):
+        """Large-d engine after ``load_state_dict``: its producer has written the last batch's raw rows again into
+        ``batch_buffer``; centre them by the saved batch mean exactly as the step did (float32 of the fp64 difference), so that
+        ``last_batch_rows`` is what it was after that step, without stepping."""
+        ch = self._chain
+        rows = ch.batch_rows(ch.last_nb)
+        step = max(1, (256 << 20) // (8 * rows.shape[1]))
+        for r0 in range(0, rows.shape[0], step):
+            blk = rows[r0:r0 + step]
+            blk.copy_((blk.double() - ch.batch_mean[None, :]).float())
+
     def last_batch_mean(self):
         """Large-d engine: fp64 [d] mean of the batch the last partial_fit centred in place."""
         return self._chain.gathered(self._chain.batch_mean.unsqueeze(0)).reshape(-1)
@@ -248,6 +285,12 @@ class IPCAEstimator:
             print("\nIPCA error:", e)
             return False
 
+    def state_dict(self):
+        return self.transformer.state_dict()
+
+    def load_state_dict(self, sd, device=None):
+        self.transformer.load_state_dict(sd, device)
+
     def get_components(self):
         stdev = np.sqrt(self.transformer.explained_variance_)
         var_ratio = self.transformer.explained_variance_ratio_
@@ -308,6 +351,20 @@ class FacebookPCAEstimator:
 
     def add_zero_rows(self, n_zero):
         self._pool.add_zero_rows(int(n_zero))
+
+    def state_dict(self):
+        """The pool of the groups folded so far (save it before ``add_zero_rows``: the zero rows depend on the final N)."""
+        if self._pool is None:
+            raise AttributeError("nothing pooled yet")
+        sd = self._pool.state_dict()
+        sd.update(engine="fbpca", d=int(self._pool.d), c=int(self.n_components))
+        return sd
+
+    def load_state_dict(self, sd, device=None):
+        if int(sd["c"]) != self.n_components:
+            raise ValueError(f"saved state has {sd['c']} components, this estimator {self.n_components}")
+        self._pool = None
+        self._ensure(int(sd["d"]), device).load_state_dict(sd)
 
     def fit_pooled(self, omega=None, raw=False):
         """fbpca.pca on the pooled samples: ``raw`` = False when they were centred (the driver: X = samples - mean, so

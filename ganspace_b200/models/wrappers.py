@@ -106,13 +106,16 @@ class _DeviceGenerator(BaseModel):
 
     def _weight_source(self, checkpoint: Path, overrides=()):
         """The seed of random-init weights, an int: ``random_init=``, else env GANSPACE_B200_RANDOM_INIT (whose value the first
-        set variable of ``overrides`` replaces).  Without a seed, ``checkpoint`` if it is a file; else raises."""
+        set variable of ``overrides`` replaces).  Without a seed, ``checkpoint`` if it is a file; else raises.  The answer is
+        kept as ``weight_source`` (a saved decomposition state names the weights it was fitted with)."""
         seed = self._random_init
         if seed is None and os.environ.get("GANSPACE_B200_RANDOM_INIT"):
             seed = next(os.environ[e] for e in (*overrides, "GANSPACE_B200_RANDOM_INIT") if os.environ.get(e))
         if seed is not None:
+            self.weight_source = int(seed)
             return int(seed)
         if checkpoint.is_file():
+            self.weight_source = checkpoint
             return checkpoint
         raise RuntimeError(f"{self.model_name} checkpoint {checkpoint} not found and no network access to download it; pass "
                            "random_init=<seed> (or set GANSPACE_B200_RANDOM_INIT) for random-init weights")
