@@ -109,6 +109,9 @@ SIGNATURES = {
     "gsb_fbpca_solve": (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _Z, _P]),
     "gsb_fbpca_status": (_I, [_P, _I, _P, _P]),
     "gsb_fbpca_project_omega": (_I, [_P, _I, _I, _P, _I, _P, _P]),
+    "gsb_strip_workspace_bytes": (_Z, [_I, _I]),
+    "gsb_strip_latents": (_I, [_P, _I, _P, _I, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _Z, _P]),
+    "gsb_strip_pack_frames": (_I, [_P, _L, _L, _L, _L, _L, _I, _I, _I, _P, _P]),
 }
 
 
@@ -779,6 +782,43 @@ def project_std(x: torch.Tensor, dirs: torch.Tensor, sub: torch.Tensor = None) -
         _check(lib.gsb_project_std(C.c_void_p(x.data_ptr()), n, d, x.stride(0), _ptr(dirs), c, _ptr(sub), _ptr(out),
                                    _ptr(ws), ws.numel(), _stream()), "gsb_project_std")
     instrument.count(2)
+    return out
+
+
+def strip_latents(latents: torch.Tensor, comps: torch.Tensor, stdev: torch.Tensor, mean, sigmas: torch.Tensor, layer_start: int,
+                  layer_end: int, n_layers: int, center: bool) -> torch.Tensor:
+    """gsb_strip_latents: the [n_layers, F, D] per-layer latents of the F = n_comp * n_lat * n_frames frames of a strip set,
+    frame (c * n_lat + i) * n_frames + k editing latent i along component c by sigmas[k].  ``latents`` [n_lat, D], ``comps``
+    [n_comp, D], ``stdev`` [n_comp], ``mean`` [D] (None without centring) and ``sigmas`` [n_frames]: fp32 contiguous on one device."""
+    lib = load()
+    dev = latents.device
+    n_lat, D = latents.shape
+    n_comp, n_frames = comps.shape[0], sigmas.numel()
+    for t, shape in ((latents, (n_lat, D)), (comps, (n_comp, D)), (stdev, (n_comp,)), (sigmas, (n_frames,))) + \
+            (((mean, (D,)),) if center else ()):
+        assert t.device == dev and t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == shape, \
+            f"fp32 contiguous {shape} on {dev} expected, got {tuple(t.shape)} {t.dtype} on {t.device}"
+    out = torch.empty((n_layers, n_comp * n_lat * n_frames, D), dtype=torch.float32, device=dev)
+    ws = scratch.get("strips", lib.gsb_strip_workspace_bytes(n_lat, n_comp), dev)
+    with torch.cuda.device(dev), instrument.section("strips"):
+        _check(lib.gsb_strip_latents(_ptr(latents), n_lat, _ptr(comps), n_comp, _ptr(stdev), _ptr(mean if center else None),
+                                     _ptr(sigmas), n_frames, layer_start, layer_end, n_layers, D, int(center), _ptr(out), _ptr(ws),
+                                     ws.numel(), _stream()), "gsb_strip_latents")
+    instrument.count(2)
+    return out
+
+
+def pack_frames(img: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """gsb_strip_pack_frames: ``out`` [n, H, W, 3] (fp32, or uint8 as np.uint8(frame * 255)) = the images ``img`` [n, 3, H, W]
+    (fp32 on the device, any strides) clamped to [0, 1] as np.clip."""
+    n, ch, H, W = img.shape
+    assert img.is_cuda and img.dtype == torch.float32 and ch == 3
+    assert out.device == img.device and out.is_contiguous() and tuple(out.shape) == (n, H, W, 3) and \
+        out.dtype in (torch.float32, torch.uint8)
+    with torch.cuda.device(img.device), instrument.section("strips"):
+        _check(load().gsb_strip_pack_frames(C.c_void_p(img.data_ptr()), *img.stride(), n, H, W, int(out.dtype == torch.uint8),
+                                            _ptr(out), _stream()), "gsb_strip_pack_frames")
+    instrument.count(1)
     return out
 
 
