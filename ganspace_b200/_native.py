@@ -112,6 +112,7 @@ SIGNATURES = {
     "gsb_strip_workspace_bytes": (_Z, [_I, _I]),
     "gsb_strip_latents": (_I, [_P, _I, _P, _I, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _Z, _P]),
     "gsb_strip_pack_frames": (_I, [_P, _L, _L, _L, _L, _L, _I, _I, _I, _P, _P]),
+    "gsb_strip_offsets": (_I, [_P, _I, _P, _I, _P, _P, _P, _I, _I, _I, _L, _L, _P, _P, _Z, _P]),
 }
 
 
@@ -804,6 +805,29 @@ def strip_latents(latents: torch.Tensor, comps: torch.Tensor, stdev: torch.Tenso
         _check(lib.gsb_strip_latents(_ptr(latents), n_lat, _ptr(comps), n_comp, _ptr(stdev), _ptr(mean if center else None),
                                      _ptr(sigmas), n_frames, layer_start, layer_end, n_layers, D, int(center), _ptr(out), _ptr(ws),
                                      ws.numel(), _stream()), "gsb_strip_latents")
+    instrument.count(2)
+    return out
+
+
+def strip_offsets(acts, comps: torch.Tensor, stdev: torch.Tensor, mean, sigmas: torch.Tensor, n_lat: int, f0: int, n: int,
+                  center: bool) -> torch.Tensor:
+    """gsb_strip_offsets: the [n, W] activation edits of frames [f0, f0 + n) of a strip set in the frame order of
+    ``strip_latents`` (n_lat latents).  ``comps`` [n_comp, W], ``stdev`` [n_comp], ``sigmas`` [n_frames] and, when centring,
+    the layer's unedited values ``acts`` [n_lat, W] and ``mean`` [W] (None otherwise): fp32 contiguous on one device."""
+    lib = load()
+    dev = comps.device
+    n_comp, W = comps.shape
+    n_frames = sigmas.numel()
+    for t, shape in ((comps, (n_comp, W)), (stdev, (n_comp,)), (sigmas, (n_frames,))) + \
+            (((acts, (n_lat, W)), (mean, (W,))) if center else ()):
+        assert t.device == dev and t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == shape, \
+            f"fp32 contiguous {shape} on {dev} expected, got {tuple(t.shape)} {t.dtype} on {t.device}"
+    out = torch.empty((n, W), dtype=torch.float32, device=dev)
+    ws = scratch.get("strips", lib.gsb_strip_workspace_bytes(n_lat, n_comp), dev)
+    with torch.cuda.device(dev), instrument.section("strips"):
+        _check(lib.gsb_strip_offsets(_ptr(acts if center else None), n_lat, _ptr(comps), n_comp, _ptr(stdev),
+                                     _ptr(mean if center else None), _ptr(sigmas), n_frames, W, int(center), f0, n, _ptr(out),
+                                     _ptr(ws), ws.numel(), _stream()), "gsb_strip_offsets")
     instrument.count(2)
     return out
 

@@ -7,6 +7,11 @@
 //   strip_apply_kernel  out[l][f][:] = z - dotp * (zc / nrm) + (zc * sigma) * stdev for l in [layer_start, layer_end), z
 //                       elsewhere; every operation rounded on its own (no contraction), in the reference's order, so a frame
 //                       whose dotp matches is bit-identical to the reference's torch expression.
+// gsb_strip_offsets writes the activation edits of frames [f0, f0 + n) of a strip set (mode 'activation' / 'both'): the dots
+// come from strip_dots_kernel over the layer's unedited values a_i and the activation components x_c, then
+//   strip_offset_kernel  out[f - f0][:] = (xc * sigma) * stdev - (xc / nrm) * dotp, the centring term only when centring;
+//                        rounded one operation at a time in the reference's order, so without centring the offsets are the
+//                        reference's delta * act_stdev bit for bit.
 // gsb_strip_pack_frames clamps the generator's [n, 3, H, W] images (any strides) to [0, 1] as np.clip does and writes NHWC
 // fp32 frames, or uint8 frames with np.uint8(frame * 255) semantics.
 #include "common.cuh"
@@ -59,6 +64,22 @@ __global__ void strip_apply_kernel(const float *__restrict__ lat, int n_lat, con
     out[((int64_t)l * F + f) * D + d] = v;
 }
 
+// grid (n, ceil(W / 128)); frame f = f0 + blockIdx.x = (c * n_lat + i) * n_frames + k
+__global__ void strip_offset_kernel(const float *__restrict__ comp, int n_lat, const float *__restrict__ stdev,
+                                    const float *__restrict__ sigmas, int n_frames, const float *__restrict__ dots, int W, int64_t f0,
+                                    int center, float *__restrict__ out) {
+    const int64_t f = f0 + blockIdx.x;
+    const int d = blockIdx.y * blockDim.x + threadIdx.x;
+    if (d >= W) return;
+    const int64_t p = f / n_frames;
+    const int k = (int)(f % n_frames);
+    const int c = (int)(p / n_lat);
+    const float xc = comp[(int64_t)c * W + d];
+    float v = __fmul_rn(__fmul_rn(xc, sigmas[k]), stdev[c]);
+    if (center) v = __fsub_rn(v, __fmul_rn(__fdiv_rn(xc, dots[2 * p]), dots[2 * p + 1]));
+    out[(int64_t)blockIdx.x * W + d] = v;
+}
+
 // one thread per output byte-group: frame n, pixel (y, x), channel ch; src strides in elements
 template <bool U8>
 __global__ void strip_pack_kernel(const float *__restrict__ src, int64_t sn, int64_t sc, int64_t sh, int64_t sw, int64_t total,
@@ -108,6 +129,29 @@ extern "C" int gsb_strip_latents(const float *d_latents, int n_lat, const float 
     dim3 grid((unsigned)F, (unsigned)((D + 127) / 128), (unsigned)L);
     strip_apply_kernel<<<grid, 128, 0, st>>>(d_latents, n_lat, d_comps, d_stdev, d_sigmas, n_frames, dots, D, F, layer_start,
                                              layer_end, center, d_out);
+    GSB_CHECK_LAUNCH();
+    return GSB_OK;
+}
+
+extern "C" int gsb_strip_offsets(const float *d_acts, int n_lat, const float *d_comps, int n_comp, const float *d_stdev,
+                                 const float *d_mean, const float *d_sigmas, int n_frames, int W, int center, int64_t f0, int64_t n,
+                                 float *d_out, void *d_workspace, size_t workspace_bytes, gsb_stream_t stream) {
+    using namespace gsb;
+    GSB_CHECK_ARG(d_comps && d_stdev && d_sigmas && d_out && d_workspace, "strip_offsets: null pointer");
+    GSB_CHECK_ARG(!center || (d_acts && d_mean), "strip_offsets: centring needs the layer's values and act_mean");
+    GSB_CHECK_ARG(n_lat >= 1 && n_comp >= 1 && n_frames >= 1 && W >= 1 && W <= 65535 * 128,
+                  "strip_offsets: bad shape (n_lat=%d, n_comp=%d, n_frames=%d, W=%d)", n_lat, n_comp, n_frames, W);
+    const int64_t F = (int64_t)n_comp * n_lat * n_frames;
+    GSB_CHECK_ARG(0 <= f0 && 1 <= n && n <= 2147483647LL && f0 + n <= F,
+                  "strip_offsets: frames [%lld, %lld) outside [0, %lld)", (long long)f0, (long long)(f0 + n), (long long)F);
+    GSB_CHECK_ARG(workspace_bytes >= gsb_strip_workspace_bytes(n_lat, n_comp), "strip_offsets: workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    float *dots = static_cast<float *>(d_workspace);
+    const int pairs = n_comp * n_lat;
+    strip_dots_kernel<<<(pairs + 7) / 8, 256, 0, st>>>(d_acts, n_lat, d_comps, n_comp, d_mean, W, center, dots);
+    GSB_CHECK_LAUNCH();
+    dim3 grid((unsigned)n, (unsigned)((W + 127) / 128));
+    strip_offset_kernel<<<grid, 128, 0, st>>>(d_comps, n_lat, d_stdev, d_sigmas, n_frames, dots, W, f0, center, d_out);
     GSB_CHECK_LAUNCH();
     return GSB_OK;
 }

@@ -605,6 +605,11 @@ class BigGAN(_DeviceGenerator):
                 self._hand_off(mod, act, act.shape[1], act.shape[3], want_image or i < len(layers) - 1, f"generator.layers.{i}")
         return chain.rgb(act).permute(0, 3, 1, 2) if want_image else None
 
+    def edit_reaches_image(self, layer_name):
+        """gen_z's output is what the chain continues from, and a row layer's rows are what its block's BatchNorm tables are built
+        from; an edit on generator.layers.k would have to be re-fed into the chain."""
+        return layer_name == "generator.gen_z" or layer_name in dict(self.model.style_layers())
+
     def _modules_by_name(self):
         mods = getattr(self, "_by_name", None)
         if mods is None:

@@ -130,6 +130,11 @@ class _DeviceGenerator(BaseModel):
         if self.outclass != new_class:
             raise RuntimeError(f"{self.model_name}: cannot change output class without reloading")
 
+    def edit_reaches_image(self, layer_name):
+        """Whether an ``edit_layer`` offset on ``layer_name`` reaches the image ``forward`` returns.  A chain output (a conv map,
+        a ToRGB image, a block) is handed to the hooks as a view that the fused chain cannot take back: not by default."""
+        return False
+
     def _hand_off(self, module, act, res, channels, downstream, name):
         """Hands the fused chain's NHWC activation ``act`` of layer ``name`` to the forward hooks of ``module`` as an NCHW view,
         and returns the view.  A hook that returns another tensor edits the layer.  The chain cannot take an edit back, so when
@@ -195,6 +200,13 @@ class _StyledGenerator(_DeviceGenerator):
             raise ValueError(f"an edit on '{name}' must keep the style's shape {tuple(rows.shape)} (or [1, {rows.shape[1]}]), got "
                              f"{tuple(out.shape)}")
         return out.to(device=rows.device, dtype=torch.float32).contiguous()
+
+    def edit_reaches_image(self, layer_name):
+        """Style layers: their rows are handed to the hooks before the chain consumes them, in Z and in W.  The mapping network's
+        output: in Z only, where ``forward`` calls it as a module and continues from its result; in W ``forward`` never runs it."""
+        if layer_name in {t[0] for t in self._style_layers()}:
+            return True
+        return layer_name == self._MAPPING_LAYER and not self.w_primary
 
     def _module(self, name):
         mods = getattr(self, "_by_name", None)
@@ -300,6 +312,7 @@ class _StyledGenerator(_DeviceGenerator):
 
 
 class StyleGAN2(_StyledGenerator):
+    _MAPPING_LAYER = "style"
     CONFIGS = {"ffhq": 1024, "car": 512, "cat": 256, "church": 256, "horse": 256,
                "bedrooms": 256, "kitchen": 256, "places": 256}
     # deepest feature maps get_or_compute decomposes: convs.8 / convs.9, 128 x 128 x 256.  At c = 80 and a 2000-row batch the large-d
@@ -652,6 +665,7 @@ class StyleGAN(_StyledGenerator):
     to download it and no TensorFlow to convert a ``.pkl``); without one, ``random_init=<seed>`` (or env GANSPACE_B200_RANDOM_INIT)
     builds ``stylegan.random_init(seed)``."""
 
+    _MAPPING_LAYER = "g_mapping"
     CONFIGS = {"ffhq": 1024, "celebahq": 1024, "bedrooms": 256, "cars": 512, "cats": 256, "vases": 1024, "wikiart": 512,
                "fireworks": 512, "abstract": 512, "anime": 512, "ukiyo-e": 512}
     # deepest feature map get_or_compute decomposes (blocks.32x32, 512 x 32 x 32), the bound ProGAN uses: the large-d engine's
